@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — particle-update throughput of the hot path on config C5 (BASELINE.json configs[4]).
 
-    python bench.py --gpus N --steps K --warmup W            # this framework (CUDA, sm_100a)
+    python bench.py --gpus N --steps K --warmup W            # this framework (CUDA, sm_90a)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's path on the host CPU
 
 Workload (SURVEY.md §8d, C5): one effect instance of 64 Mi particles, attributes {position, velocity,
@@ -15,7 +15,7 @@ One JSON line is printed by rank 0 (see the task contract): value = particle-ste
 job with all state resident in HBM; e2e = same metric through the C ABI with the per-frame HOST tables
 (spawners, batch infos, prefix sums, sim params) uploaded and the draw-indirect instance count read
 back every step; roofline = update kernel algorithmic bytes (72 B/particle-step) / its CUDA-event
-duration vs the measured HBM copy peak; cpu_baseline = the CPU oracle (C port, OpenMP) on a bounded
+duration vs the HBM peak (MEASURED_PEAKS.json when present, else the H100 SXM data sheet's 3.35 TB/s); cpu_baseline = the CPU oracle (C port, OpenMP) on a bounded
 sample of the same workload.
 """
 from __future__ import annotations
@@ -51,11 +51,12 @@ def parse_args():
     ap.add_argument("--scaling", default="strong", choices=["strong", "weak"])
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="budget of the cpu_baseline leg")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed as DIR/<name>.npy")
     return ap.parse_args()
 
 
 # ---------------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md "clocks DURING the timed region")
+# clocks sampling during the timed region
 # ---------------------------------------------------------------------------------------------------
 class ClockSampler:
     """SM clock and throttle reasons sampled DURING the timed region. NVML in a thread (a query takes microseconds,
@@ -146,6 +147,19 @@ class ClockSampler:
                     reasons.add(name)
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(smax) if smax else None,
                 "reasons": sorted(reasons), "samples": len(sm), "source": "nvidia-smi"}
+
+
+def device_info(gpu_index: int):
+    """The card's name and power limit: a measured time is only meaningful next to them."""
+    import torch
+    info = {"name": torch.cuda.get_device_name(gpu_index), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={gpu_index}", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        info["power_limit_w"] = float(out)
+    except Exception:
+        pass
+    return info
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -288,6 +302,47 @@ def run_reference(args):
 # ---------------------------------------------------------------------------------------------------
 # GPU arm
 # ---------------------------------------------------------------------------------------------------
+DUMP_SAMPLE_ROWS = 1 << 20   # over all ranks: 56 B per sampled row (record + three indices) = 56 MiB, under 64 MB
+DUMP_LIMIT_BYTES = 64 * 10**6
+DUMP_BLOCK_ROWS = 4096       # rows are sampled as whole blocks, so only the sampled rows leave the device
+
+
+def dump_outputs(ctx, slab, rows, logical_first, out_dir, rank, world):
+    """What a caller of simulate() receives after the last timed step: the particle records, the alive list and the
+    counts, as .npy files (suffixed _rank<r> when several ranks write). Records and list entries are a fixed, seeded
+    sample of blocks of rows; the ranks share the DUMP_SAMPLE_ROWS budget."""
+    import numpy as np
+
+    from bevy_hanabi_b200 import recipes
+    out_dir.mkdir(parents=True, exist_ok=True)
+    suffix = f"_rank{rank}" if world > 1 else ""
+    md = ctx.read_metadata(0)
+    n_blocks = -(-rows // DUMP_BLOCK_ROWS)
+    k = min(n_blocks, max(1, DUMP_SAMPLE_ROWS // world // DUMP_BLOCK_ROWS))
+    blocks = np.sort(np.random.default_rng([20240607, logical_first]).choice(n_blocks, k, replace=False))
+    recs, idx, pick = [], [], []
+    for b in blocks:
+        first = int(b) * DUMP_BLOCK_ROWS
+        count = min(DUMP_BLOCK_ROWS, rows - first)
+        recs.append(ctx.slab_download_aos(slab, first, count, recipes.C5_STRIDE))
+        idx.append(ctx.slab_download_indirect(slab, first, count)[:, md.indirect_write_index])
+        pick.append(np.arange(first, first + count))
+    pick, idx = np.concatenate(pick), np.concatenate(idx)
+    alive = pick < md.alive_count
+    arrays = {
+        "particles": np.concatenate(recs).view(np.float32),  # (rows, 8): position.xyz, age, velocity.xyz, lifetime
+        "particle_rows": (pick + logical_first).astype(np.float64),
+        "alive_list": idx[alive].astype(np.float64),
+        "alive_list_positions": pick[alive].astype(np.float64),
+        "counts": np.array([md.alive_count, md.max_update, md.max_spawn, ctx.read_draw_args(0).instance_count], dtype=np.float64),
+    }
+    total = sum(a.nbytes for a in arrays.values())
+    if total * world > DUMP_LIMIT_BYTES:
+        raise RuntimeError(f"bench.py: dump of {total} bytes per rank x {world} ranks exceeds {DUMP_LIMIT_BYTES}")
+    for name, a in arrays.items():
+        np.save(out_dir / f"{name}{suffix}.npy", a)
+
+
 def run_b200(args):
     import torch
     import torch.distributed as dist
@@ -386,6 +441,8 @@ def run_b200(args):
     gpu_launches = ctx.launch_count - l0
     clocks = sampler.stop() if rank == 0 else None
     value = total * args.steps / (ms * 1e-3)
+    if args.dump_outputs:
+        dump_outputs(ctx, slab, per_rank, logical_first, Path(args.dump_outputs), rank, world)
 
     # -- roofline leg: the update kernel alone, timed by CUDA events recorded around each launch on the launching stream
     ctx.enable_kernel_timing(True)
@@ -436,7 +493,7 @@ def run_b200(args):
     for _ in range(3):
         step_e2e()
     drain_e2e()
-    # K steps, three times; the MEDIAN run is reported (all three are listed): the timed region is ~10 ms at 8 GPUs, where a
+    # K steps, three times; the MEDIAN run is reported (all three are listed): the timed region is short at 8 GPUs, where a
     # single scheduling hiccup of one rank's host process (the max over ranks sees it) shifts the result by tens of percent
     e2e_runs = []
     for _ in range(3):
@@ -464,10 +521,10 @@ def run_b200(args):
 
     peaks_path = ROOT / "MEASURED_PEAKS.json"
     if peaks_path.exists():
-        peak = json.loads(peaks_path.read_text()).get("hbm_gbs", 6650.0)
+        peak = json.loads(peaks_path.read_text()).get("hbm_gbs", 3350.0)
         peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        peak, peak_src = 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
     if rank == 0:
         line = {
@@ -492,26 +549,14 @@ def run_b200(args):
                             "they travel to the device with that step's first kernel launch; the draw-indirect instance_count of every "
                             "step comes back through the count mailbox and is checked on the host (two frames in flight: step i is "
                             "checked while step i+1 is queued); particle state stays in HBM as in the reference (it is never on the "
-                            "host there either). With explicit cudaMemcpyAsync both ways the same loop costs +14 us per step "
-                            "(profiles/r2_bench_n*_copy_engine_e2e.json: 0.7634 ms at N=1, 0.1231 ms at N=8)"},
+                            "host there either)"},
             "gpu_launches": int(gpu_launches),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "traffic": None, "kernel": "hnb_update", "kernel_ms": k_avg_ms, "peak_source": peak_src,
                          "bytes_per_particle_step": BYTES_PER_PARTICLE_STEP},
             "clocks": clocks,
+            "device": device_info(local_rank),
         }
-        prof = ROOT / "profiles" / "traffic.json"
-        if prof.exists():
-            try:
-                rec = json.loads(prof.read_text())
-                # one ncu capture per launch size (64 Mi on one GPU, 32 / 16 / 8 Mi per GPU on 2 / 4 / 8): quote the one of THIS size
-                by_size = rec.get("by_particles_per_launch", {})
-                if str(per_rank) in by_size:
-                    line["roofline"]["traffic"] = int(by_size[str(per_rank)]["dram_bytes"])
-                elif int(rec.get("particles_per_launch", 0)) == per_rank:
-                    line["roofline"]["traffic"] = rec.get("hnb_update_dram_bytes_per_launch")
-            except Exception:
-                pass
         if not args.no_cpu_baseline and n_gpus == 1:
             cb, arm = cpu_baseline(args.cpu_seconds)
             line["cpu_baseline"] = cb

@@ -1,4 +1,4 @@
-"""hanabi_b200 — B200-native particle simulation backend behind Hanabi's authoring API.
+"""hanabi_b200 — H100-native particle simulation backend behind Hanabi's authoring API.
 
 The package is a binding over ``libhanabi_b200.so`` (C ABI in ``include/hanabi_b200.h``); importing it
 fails loudly when the native library has not been built. There is no CPU execution path.

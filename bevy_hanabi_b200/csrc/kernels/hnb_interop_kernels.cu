@@ -1,7 +1,7 @@
 // hnb_interop_kernels.cu — layout conversion between the slab's SoA storage and the reference's buffer layouts
 // (SURVEY.md §8 f-2): AoS `Particle` records (ParticleLayout, attributes.rs:1807-1913) and interleaved `IndirectEntry`
 // rows {particle_index[2], dead_index} (vfx_common.wgsl:66-78, mod.rs:139-146). Compiled ahead of time by nvcc for
-// sm_100a. Used by the host up/download entry points and by the device-to-device export a renderer binds.
+// sm_90a. Used by the host up/download entry points and by the device-to-device export a renderer binds.
 #include <algorithm>
 #include <cstdint>
 #include <cuda_runtime.h>

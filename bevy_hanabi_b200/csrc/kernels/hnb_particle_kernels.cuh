@@ -1,4 +1,4 @@
-// hnb_particle_kernels.cuh — hand-written sm_100a kernel templates for the two per-particle passes
+// hnb_particle_kernels.cuh — hand-written sm_90a kernel templates for the two per-particle passes
 // of the hot path. They play the role of the reference's WGSL templates
 //   src/render/vfx_init.wgsl   (entry :101-196)   → hnb_init
 //   src/render/vfx_update.wgsl (entry :106-167)   → hnb_update
@@ -52,7 +52,7 @@ namespace hnb {
 #endif
 #define HNB_SMEM_PREFIX_BYTES ((HNB_SMEM_EFFECTS + 1) * 4)
 #ifndef HNB_MIN_BLOCKS
-#define HNB_MIN_BLOCKS 3  // 3 CTAs x 85 registers measured 2.4 % faster than 4 x 64 on C5 (profiles/)
+#define HNB_MIN_BLOCKS 3  // H100, C5 at 64 / 8 Mi: 4 CTAs (64 registers) 6 % slower, 2 CTAs within 1 %
 #endif
 #ifndef HNB_DEFER_COMPACTION
 #define HNB_DEFER_COMPACTION (!HNB_RELAXED_ORDER)  // park a tile's compaction behind the warp's next pass 1
@@ -132,7 +132,7 @@ template <typename Ptr> HNB_DI u32 hnb_find_effect(Ptr prefix, u32 lo, u32 hi, u
 // ---------------------------------------------------------------------------------------------
 // Each CUDA thread runs HNB_INIT_ITEMS of the reference's init threads (logical thread index = CTA base +
 // k*HNB_BLOCK + threadIdx, so every k is a coalesced row of the dead stack / alive list). One spawn per thread is
-// latency-bound: the work is a chain broadcast loads -> dead-slot load -> PRNG -> stores, so a thread lives ~2 us
+// latency-bound: the work is a chain broadcast loads -> dead-slot load -> PRNG -> stores, so a thread lives long
 // for 40 bytes of traffic; with the items' chains issued together the launch is bandwidth-bound instead.
 #ifndef HNB_INIT_ITEMS
 #define HNB_INIT_ITEMS 4
@@ -507,9 +507,9 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
     }
 #endif
 
-    // (Reading the host-written batch info / first spawner row before the wait was tried: it saves ~1 us per frame on a 1 Mi chain
-    // and costs 3-4 us on a launch that is NOT overlapped with its predecessor, because the wait then separates two groups of
-    // dependent loads that used to be issued together: profiles/r2_ab_prologue.txt. The bookkeeping kernel keeps its variant.)
+    // (Reading the host-written batch info / first spawner row before the wait was tried: it gains a little on an overlapped
+    // chain and loses more on a launch that is NOT overlapped with its predecessor, because the wait then separates two groups
+    // of dependent loads that used to be issued together. The bookkeeping kernel keeps its variant.)
     const u32 bi_spawner_base = P.bi_spawner_base, bi_prefix_sum_offset = P.bi_prefix_sum_offset, n_effects = P.bi_prefix_sum_count;  // (kernel parameters: no load)
     const u32* g_tile_prefix = P.tile_prefix + bi_prefix_sum_offset;
     const u32 total_tiles = *P.batch_tiles;

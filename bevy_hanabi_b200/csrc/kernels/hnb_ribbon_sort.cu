@@ -1,4 +1,4 @@
-// hnb_ribbon_sort.cu — ribbon sort (SURVEY.md §8f-4), compiled ahead of time by nvcc for sm_100a.
+// hnb_ribbon_sort.cu — ribbon sort (SURVEY.md §8f-4), compiled ahead of time by nvcc for sm_90a.
 //
 // Replaces the reference's three dispatches per ribbon effect instance (mod.rs:7444-7610):
 //     vfx_sort_fill.wgsl :38-57   pairs[k] = {particle[RIBBON_ID], particle[AGE], particle_index}

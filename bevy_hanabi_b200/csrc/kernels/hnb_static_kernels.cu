@@ -1,4 +1,4 @@
-// hnb_static_kernels.cu — effect-independent kernels, compiled ahead of time by nvcc for sm_100a.
+// hnb_static_kernels.cu — effect-independent kernels, compiled ahead of time by nvcc for sm_90a.
 //
 //   k_indirect        ≙ src/render/vfx_indirect.wgsl main()   (:31-90)
 //   k_prefix_sum      ≙ src/render/vfx_prefix_sum.wgsl main() (:14-43)
@@ -661,7 +661,7 @@ cudaError_t launch_measure_sm_clock(u64* out2, u64 window_ns, cudaStream_t st) {
 }
 cudaError_t launch_checksum(const PlaneSet& planes, u32 first, u32 count, u32 stride_words, u64 index_base, u64* out, cudaStream_t st) {
     if (count == 0) return cudaSuccess;
-    k_checksum<<<148 * 4, 256, 0, st>>>(planes, first, count, stride_words, index_base, out);
+    k_checksum<<<132 * 4, 256, 0, st>>>(planes, first, count, stride_words, index_base, out);
     return cudaGetLastError();
 }
 

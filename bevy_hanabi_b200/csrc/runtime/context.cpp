@@ -151,7 +151,7 @@ struct LaunchPlan;
 
 struct hnb_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     std::vector<uint8_t> init_pending;   // per batch: a stand-alone hnb_pass_init whose accounting hnb_pass_indirect has not applied yet
     std::vector<LaunchPlan> frame_plans;  // hnb_simulate's per-frame launch plans (kept to avoid a heap allocation per frame)
     cudaStream_t stream = nullptr;
@@ -421,7 +421,7 @@ KernelModule* get_module(hnb_ctx* c, const std::string& source, const std::strin
     if (it != c->modules.end()) return it->second.get();
     std::string cubin, log;
     if (precompiled) cubin = *precompiled;
-    else if (!nvrtc_compile_sm100a(source, name + ".cu", cubin, log, fast_math)) fail(HNB_ERR_NVRTC, log);
+    else if (!nvrtc_compile_sm90a(source, name + ".cu", cubin, log, fast_math)) fail(HNB_ERR_NVRTC, log);
     auto km = std::make_unique<KernelModule>();
     km->log = log;
     CUresult r = c->drv.ModuleLoadData(&km->mod, cubin.data());
@@ -476,14 +476,13 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
         fail(HNB_ERR_OUT_OF_RANGE, "batch references instances outside the uploaded spawner table");
     // Rows per warp tile: 32 lanes x K rows per lane x chunks. Larger tiles shorten the look-back chain and
     // amortise the per-tile work (ticket, state word, instance lookup); smaller tiles spread a small slab over more
-    // warps. With W = one sub-tile per resident warp (C5 on a B200: 3552 warps x 128 rows = 444 Ki rows):
-    //  * from 8 W up the launch streams at the HBM rate and the largest tile wins at every size (tools/sweep_small.py,
-    //    profiles/r2_quantization_sweep.txt: no quantisation at whole numbers of tiles per warp);
+    // warps. With W = one sub-tile per resident warp (C5 on an H100: 3168 warps x 128 rows = 396 Ki rows):
+    //  * from 8 W up the launch streams at the HBM rate and the largest tile wins at every size;
     //  * below, the launch is latency-bound and runs in ROUNDS: every resident warp takes one tile per round, and a tile
-    //    costs a fixed part (ticket, first alive-list entries, look-back, compaction: ~5.5 us) plus ~1.5 us per sub-tile
-    //    (fit of the 1-4 chunk timings at 2 Mi rows, profiles/r2_chunks_sweep.txt): pick the chunk count that minimises
-    //    rounds x (3.6 + chunks), preferring larger tiles on a tie. 1 Mi rows -> 3 chunks (every warp takes exactly one
-    //    tile), 2 Mi -> 3, 512 Ki -> 2, 256 Ki -> 1.
+    //    costs a fixed part (ticket, first alive-list entries, look-back, compaction) plus a part per sub-tile: pick the
+    //    chunk count that minimises rounds x (3.6 + chunks), preferring larger tiles on a tie. The constant was fitted on
+    //    an earlier GPU. On an H100 (tools/sweep_small.py, C5) the rule is within 3 % of the best forced chunk count from
+    //    1 Mi rows up; at 256-512 Ki rows forcing 3-4 chunks shortens the frame by 15-20 % (not retuned).
     const uint32_t sub_tile = 32u * lp.fx->tile_k;
     const uint32_t total_warps = uint32_t(lp.fx->update_blocks_per_sm) * uint32_t(c->sm_count) * 8u;
     const uint32_t max_chunks = std::max(1u, lp.fx->rows_per_lane / lp.fx->tile_k);
@@ -784,7 +783,7 @@ extern "C" {
 const char* hnb_last_error(void) { return g_last_error.c_str(); }
 // shared with graph/graph_cabi.cpp (not part of the public ABI: hidden visibility)
 __attribute__((visibility("hidden"))) void hnb_set_last_error_(const char* msg) { g_last_error = msg ? msg : ""; }
-const char* hnb_version(void) { return "hanabi_b200 0.1.0 (sm_100a)"; }
+const char* hnb_version(void) { return "hanabi_b200 0.1.0 (sm_90a)"; }
 
 int32_t hnb_ctx_create(int32_t cuda_device, uintptr_t external_stream, hnb_ctx** out) {
     return guarded([&] {
@@ -807,7 +806,7 @@ int32_t hnb_ctx_create(int32_t cuda_device, uintptr_t external_stream, hnb_ctx**
         cudaDeviceProp prop;
         CUDA_CHECK(cudaGetDeviceProperties(&prop, cuda_device));
         c->sm_count = prop.multiProcessorCount;
-        if (prop.major != 10) fail(HNB_ERR_NO_DEVICE, "hanabi_b200 kernels are built for sm_100a only; device is sm_" + std::to_string(prop.major * 10 + prop.minor));
+        if (prop.major != 9 || prop.minor != 0) fail(HNB_ERR_NO_DEVICE, "hanabi_b200 kernels are built for sm_90a only; device is sm_" + std::to_string(prop.major * 10 + prop.minor));
         if (external_stream) {
             c->stream = (cudaStream_t)external_stream;
         } else {
@@ -1171,7 +1170,7 @@ int32_t hnb_nvrtc_check(const char* source, size_t* cubin_size) {
         std::string cubin, log;
         // generated sources state their own compile mode (effect_source.cpp)
         const bool fast_math = std::string(source).find("#define HNB_FAST_MATH 1") != std::string::npos;
-        if (!nvrtc_compile_sm100a(source, "check.cu", cubin, log, fast_math)) fail(HNB_ERR_NVRTC, log);
+        if (!nvrtc_compile_sm90a(source, "check.cu", cubin, log, fast_math)) fail(HNB_ERR_NVRTC, log);
         g_last_error = log;  // compiler log (ptxas -v) available to the caller even on success
         if (cubin_size) *cubin_size = cubin.size();
     });
@@ -1254,7 +1253,7 @@ hnb_compile_job* hnb_compile_job_start(const hnb_effect_desc* desc) {
         j->bp = make_blueprint(*desc);  // copies every string of the descriptor
         hnb_compile_job* raw = j.get();
         raw->worker = std::thread([raw] {
-            const bool ok = nvrtc_compile_sm100a(raw->bp.source, raw->bp.name + ".cu", raw->cubin, raw->log, raw->bp.fast_math);
+            const bool ok = nvrtc_compile_sm90a(raw->bp.source, raw->bp.name + ".cu", raw->cubin, raw->log, raw->bp.fast_math);
             raw->state.store(ok ? 1 : -1, std::memory_order_release);
         });
         job = j.release();
@@ -1468,7 +1467,7 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
         // ... or, third way, with the bookkeeping LAUNCH: when the frame has no init pass (nothing reads the tables before the
         // bookkeeping kernel) and the host-written part of the arena fits the kernel parameter space, it travels there and CTA 0
         // stores it into the device arena. A copy-engine operation between two kernels of the chain costs its own latency and
-        // the programmatic overlap of the kernel behind it (~10 us per frame of a host that rewrites its tables every frame).
+        // the programmatic overlap of the kernel behind it, every frame of a host that rewrites its tables every frame.
         const bool copy_block = c->dirty_tables || c->plan_dirty;
         bool any_init = false;
         for (auto& lp : plans) any_init |= lp.init_blocks != 0;

@@ -1,4 +1,4 @@
-// nvrtc_compile.cpp — run-time compilation of generated effect kernels for sm_100a.
+// nvrtc_compile.cpp — run-time compilation of generated effect kernels for sm_90a.
 // ≙ the naga WGSL->SPIR-V step behind wgpu's create_shader_module in the reference; the result is a
 // cubin (not PTX) so no driver JIT is involved at load time.
 #include "nvrtc_compile.h"
@@ -18,7 +18,7 @@ uint64_t fnv1a64(const std::string& s) {
     return h;
 }
 
-bool nvrtc_compile_sm100a(const std::string& source, const std::string& name, std::string& cubin, std::string& log, bool fast_math) {
+bool nvrtc_compile_sm90a(const std::string& source, const std::string& name, std::string& cubin, std::string& log, bool fast_math) {
     nvrtcProgram prog = nullptr;
     nvrtcResult r = nvrtcCreateProgram(&prog, source.c_str(), name.c_str(), 0, nullptr, nullptr);
     if (r != NVRTC_SUCCESS) {
@@ -29,7 +29,7 @@ bool nvrtc_compile_sm100a(const std::string& source, const std::string& name, st
     // (SURVEY.md §7 "fp parity"). No fast-math: IEEE division and square root.
     // HNB_EFFECT_FAST_MATH: contraction and approximate div/sqrt, but NOT --use_fast_math (its sin/cos/exp
     // intrinsics have absolute, not relative, error bounds and would break the 1e-5 relative tolerance).
-    std::vector<const char*> opts = {"-arch=sm_100a", "-std=c++17", "-lineinfo", "-default-device", "-diag-suppress=550", "-diag-suppress=177",
+    std::vector<const char*> opts = {"-arch=sm_90a", "-std=c++17", "-lineinfo", "-default-device", "-diag-suppress=550", "-diag-suppress=177",
                                      "--ptxas-options=-v"};
     if (fast_math) {
         opts.push_back("-fmad=true");

@@ -122,7 +122,7 @@ class CompileJob:
 
 
 def nvrtc_check(source: str) -> tuple[int, str]:
-    """Compile a translation unit for sm_100a with NVRTC (no GPU needed). Returns (cubin bytes, log)."""
+    """Compile a translation unit for sm_90a with NVRTC (no GPU needed). Returns (cubin bytes, log)."""
     n = C.c_size_t(0)
     check(lib.hnb_nvrtc_check(source.encode(), C.byref(n)))
     return n.value, N.last_error()

@@ -96,7 +96,7 @@ int main(int argc, char** argv) {
     hnb_effect_spawner* spawner = hnb_effect_spawner_create(&settings, 42);
     hnb_batcher* batcher = hnb_batcher_create();
 
-    /* ---- runtime (needs a B200) */
+    /* ---- runtime (needs an H100) */
     hnb_ctx* ctx = NULL;
     CHECK(hnb_ctx_create(0, 0, &ctx));
     hnb_effect effect;

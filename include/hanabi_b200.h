@@ -1,5 +1,5 @@
 /*
- * hanabi_b200.h — C ABI of the B200-native Hanabi particle simulation backend.
+ * hanabi_b200.h — C ABI of the H100-native Hanabi particle simulation backend.
  *
  * This is the drop-in boundary for the hot path of djeedai/bevy_hanabi: it replaces the
  * wgpu compute dispatch recorded by `simulate()` (reference src/render/mod.rs:6942-7613)
@@ -337,7 +337,7 @@ typedef struct hnb_effect_desc {
     uint32_t num_event_bindings;    /* number of child event buffers this effect appends to */
 } hnb_effect_desc;
 
-/** Compile (NVRTC, sm_100a, cached by source hash ≙ ShaderCache) the init+update kernels. */
+/** Compile (NVRTC, sm_90a, cached by source hash ≙ ShaderCache) the init+update kernels. */
 HNB_API int32_t hnb_effect_compile(hnb_ctx* ctx, const hnb_effect_desc* desc, hnb_effect* out);
 HNB_API int32_t hnb_effect_destroy(hnb_ctx* ctx, hnb_effect effect);
 
@@ -361,7 +361,7 @@ HNB_API int32_t hnb_effect_create_from_job(hnb_ctx* ctx, hnb_compile_job* job, h
  * in *len. Used by the CPU test-suite (≙ the reference's naga validation tests).
  */
 HNB_API int32_t hnb_effect_generate_source(const hnb_effect_desc* desc, char* out, size_t cap, size_t* len);
-/** NVRTC-compile a translation unit for sm_100a without loading it (no GPU needed). On failure
+/** NVRTC-compile a translation unit for sm_90a without loading it (no GPU needed). On failure
  *  the compiler log is available from hnb_last_error(). `cubin_size` may be NULL. */
 HNB_API int32_t hnb_nvrtc_check(const char* source, size_t* cubin_size);
 

@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA GPU (B200); run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA GPU (H100); run with -m gpu")
     # emulation tests spin on real OS threads: a protocol bug must fail, not hang (marker of pytest-timeout; a no-op without it)
     config.addinivalue_line("markers", "timeout(seconds): per-test time limit (pytest-timeout)")
 

@@ -6,7 +6,7 @@ unit tests and of its naga "the generated shader parses" validation tests (SURVE
   particle layout packing   src/attributes.rs:2379-2521
   property layout           src/properties.rs:1010-1165, :1395-1422
   modifier validity         src/modifier/mod.rs:1066-1286 — here every modifier's generated translation
-                            unit is compiled for sm_100a by NVRTC
+                            unit is compiled for sm_90a by NVRTC
   generated update body     src/lib.rs:2155-2308 / SURVEY.md Appendix E
 """
 import re

@@ -1,5 +1,5 @@
 """bench.py's driver contract, as far as it can be checked without a GPU: the reference arm prints ONE JSON line with
-every key the contract names, on this arm's metric / unit / config; the B200 arm refuses to run without a device (there
+every key the contract names, on this arm's metric / unit / config; the GPU arm refuses to run without a device (there
 is no CPU path) instead of measuring something else."""
 import json
 import subprocess

@@ -1,7 +1,7 @@
 """CPU-side fuzz of the expression lowering over the WHOLE operator table (reference src/graph/expr.rs:1833-2360):
 random typed expression trees over scalars, vec2/3/4, uint and bool values are lowered to CUDA C and
 
-  * compiled for sm_100a with NVRTC (no GPU needed) — catches text that is not valid C++ against hnb_wgsl.cuh
+  * compiled for sm_90a with NVRTC (no GPU needed) — catches text that is not valid C++ against hnb_wgsl.cuh
     (missing overloads, ambiguous calls, precedence of pasted text), and
   * interpreted by the numpy oracle on a few particles — catches operators the oracle cannot evaluate or evaluates
     with the wrong shape / type.
@@ -223,7 +223,7 @@ def Value_vec(n, xs):
 @given(st.data())
 def test_random_matrix_graphs_generated_code_equals_interpreter(orc, data):
     """Matrix values (all nine matCxR shapes, chosen at random) in random product / sum graphs: the generated code must
-    compile for sm_100a and, run on the CPU, equal the interpreter bit for bit."""
+    compile for sm_90a and, run on the CPU, equal the interpreter bit for bit."""
     from tests.host_exec import HostEffect, replay_frame
     w = G.ExprWriter()
     depth = lambda: data.draw(st.integers(1, 3))

@@ -1,6 +1,6 @@
 """Diagnostics: why does hnb_update run slower when the host synchronises every step?"""
-import sys, time, ctypes as C
-sys.path.insert(0, "/root/repo")
+import os, sys, time, ctypes as C
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import bevy_hanabi_b200 as hb
 from bevy_hanabi_b200 import _native as N, recipes, runtime as R

@@ -3,7 +3,7 @@ of the HNB_PROFILE build (ring of 64 frames): for consecutive frames N, N+1 of a
 of frame N's last warp: when the first CTA of N+1 became resident, when the first warp of N+1 passed the dependency wait,
 when the first sub-tile (128 rows) of N+1 was done, and when N+1's last warp ended. Usage: python tools/diag_frame_chain.py [Mi ...]"""
 import os, sys
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 os.environ["HNB_DEFINES"] = os.environ.get("HNB_DEFINES", "") + ";HNB_PROFILE=1"
 import numpy as np
 import torch

@@ -1,5 +1,5 @@
 import sys, time, os
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import bevy_hanabi_b200 as hb
 from bevy_hanabi_b200 import _native as N, recipes, runtime as R

@@ -1,6 +1,6 @@
 """Where does the fixed cost of one hnb_update launch go? Timeline probes of the HNB_PROFILE build (%globaltimer)."""
 import os, sys
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 os.environ["HNB_DEFINES"] = os.environ.get("HNB_DEFINES", "") + ";HNB_PROFILE=1"
 import torch
 import bevy_hanabi_b200 as hb

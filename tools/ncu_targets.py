@@ -5,18 +5,18 @@ usage (on a GPU box):
       python tools/ncu_targets.py <scenario>
 Every scenario sets its state up and warms the kernels OUTSIDE the profiled range, then brackets ONE frame (or one call)
 with cudaProfilerStart / cudaProfilerStop, so a report holds one launch of each kernel of that frame: hnb_init (when the
-frame spawns), k_bookkeeping, hnb_update. `tools/ncu_summary.py` turns the report into the text kept under profiles/.
+frame spawns), k_bookkeeping, hnb_update. `tools/ncu_summary.py` turns the report into a text summary.
 """
-import sys
+import os, sys
 
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 
 import bevy_hanabi_b200 as hb
 from bevy_hanabi_b200 import _native as N, graph as G, recipes, runtime as R
 
-sys.path.insert(0, "/root/repo/tools")
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import perf_matrix as PM   # scenario helpers (single_instance, recipes of the other configs)
 
 A = G.Attribute

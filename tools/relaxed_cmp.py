@@ -1,5 +1,5 @@
-import sys
-sys.path.insert(0, "/root/repo"); sys.path.insert(0, "/root/repo/tools")
+import os, sys
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__)))); sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import perf_matrix as PM
 from perf_matrix import *
 for mi in (64, 8):

@@ -8,9 +8,12 @@ saved baseline.
 
 Compiles with nvcc offline (no GPU needed), with the flags the NVRTC path uses for default effects.
 """
+import os
 import subprocess
 import sys
 from pathlib import Path
+
+CUDA = Path(os.environ.get("CUDA_HOME", "/usr/local/cuda"))  # the same nvcc as bevy_hanabi_b200/build.py
 
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 
@@ -27,7 +30,7 @@ def sources():
 def sass(name, src, d: Path):
     cu, cubin = d / f"{name}.cu", d / f"{name}.cubin"
     cu.write_text(src)
-    subprocess.run(["/usr/local/cuda/bin/nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "--fmad=false",
+    subprocess.run([str(CUDA / "bin" / "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "--fmad=false",
                     "-diag-suppress", "550,177", "-cubin", str(cu), "-o", str(cubin)], check=True)
     return subprocess.run(["cuobjdump", "-sass", str(cubin)], capture_output=True, text=True, check=True).stdout
 

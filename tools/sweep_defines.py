@@ -1,6 +1,6 @@
 """Kernel-variant sweep: time hnb_update for several HNB_DEFINES settings on the C5 workload."""
 import os, sys, time
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import bevy_hanabi_b200 as hb
 from bevy_hanabi_b200 import _native as N, recipes, runtime as R

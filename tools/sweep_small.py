@@ -1,7 +1,7 @@
 """Shard-size sweep: hnb_update time vs particles per GPU for each tile-chunk setting (HNB_TILE_CHUNKS) and
 optional HNB_DEFINES variants. Usage: sweep_small.py [defines ...]  (env SWEEP_PS="4,8,16,32" in Mi rows)"""
 import os, sys
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import bevy_hanabi_b200 as hb
 from bevy_hanabi_b200 import _native as N, recipes, runtime as R

@@ -1,6 +1,6 @@
 """Time hnb_pass_sort (ribbon sort) for several sizes; wide = all eight radix passes, narrow = typical ribbon keys."""
-import sys, time
-sys.path.insert(0, "/root/repo")
+import os, sys, time
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 import bevy_hanabi_b200 as hb
