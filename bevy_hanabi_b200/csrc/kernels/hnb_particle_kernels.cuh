@@ -282,7 +282,12 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK) hnb_init(const BatchPara
         Particle particle = Particle();
         hnb_init_body(particle, hnb_ctx);
 
-        // Append to the alive list (:191-192) and write the particle back (:195)
+        // Append to the alive list (:191-192) and write the particle back (:195). The instance's first appended row ends what an
+        // identity claim on the column can cover.
+        if (it.update_index == 0u && P.slab.ident_claim) {
+            u64* const claim = &P.slab.ident_claim[md->indirect_write_index];
+            if (hnb_claim_len(hnb_claim_load(claim), base_particle) > it.alive_index) hnb_claim_store(claim, hnb_claim_pack(base_particle, it.alive_index));
+        }
         P.slab.particle_index[md->indirect_write_index][base_particle + it.alive_index] = particle_index;
 #if HNB_SLOT_ORDER
         atomicOr(&P.slab.alive_bits[(base_particle + particle_index) >> 5u], 1u << ((base_particle + particle_index) & 31u));
@@ -303,7 +308,10 @@ struct PendingTile {
     u32 valid, tile, row0, tile_alive;
     u32 base_particle, max_update, write_index, render_index;
     u32 inst_first_tile, inst_end_tile, metadata_index, buffer;
-    u32 tile_valid, _pad[3];  // slot order: rows of the tile that were alive before the pass
+    u32 tile_valid;  // slot order: rows of the tile that were alive before the pass
+    // identity claims as read when the instance was bound (a parked tile may be compacted after the instance's last tile has
+    // rewritten the claim): read-column rows known to be the identity, length of the write column's claim for this instance
+    u32 trust_r, claim_w, _pad;
 };  // 64 bytes (mirrored by update_smem_bytes on the host)
 
 // Compaction of one tile: exclusive prefix of survivors over the previous tiles of the instance
@@ -426,6 +434,7 @@ HNB_DI void hnb_compact_tile(const BatchParams& P, const PendingTile& pt, const 
         if (valid_before + pt.tile_valid != max_update && P.debug) atomicAdd(&P.debug[15], 1ull);
     }
 #else
+    const u32 claim_w = pt.claim_w;
 #pragma unroll 4
     for (u32 jk = 0; jk < chunks * HNB_TILE_K; ++jk) {
         const u32 row = row0 + jk * 32u + lane;
@@ -434,7 +443,7 @@ HNB_DI void hnb_compact_tile(const BatchParams& P, const PendingTile& pt, const 
             const u32 pidx = pidx_stash[jk][lane];
             const u32 alive_rank = alive_rank_base + __popc(ballot & hnb_lanemask_lt());  // surviving rows before `row`
             if ((ballot >> lane) & 1u) {
-                write_col[alive_rank] = pidx;
+                if (pidx != alive_rank || alive_rank >= claim_w) write_col[alive_rank] = pidx;  // (else: the claim says it is there)
             } else {
 #if HNB_RELAXED_ORDER
                 const u32 alive_index = atomicSub(&md->alive_count, 1u) - 1u;
@@ -460,6 +469,13 @@ HNB_DI void hnb_compact_tile(const BatchParams& P, const PendingTile& pt, const 
         hnb_post_count(P, epoch, pt.render_index, alive_total);
         md->alive_count = md->alive_count - dead_total;
         md->max_spawn = md->max_spawn + dead_total;
+        // The next claim on the write column: with an identity read list and no death, rows [0, max_update) now hold their own
+        // index (rows beyond were not written, so a longer claim still holds there); otherwise drop the instance's claim.
+        if (P.slab.ident_claim) {
+            u64* const claim = &P.slab.ident_claim[pt.write_index];
+            if (pt.trust_r >= max_update && alive_total == max_update) hnb_claim_store(claim, hnb_claim_pack(base_particle, claim_w > max_update ? claim_w : max_update));
+            else if (claim_w != 0u) hnb_claim_store(claim, 0ull);
+        }
     }
 #endif
 #endif  // HNB_SLOT_ORDER
@@ -534,6 +550,7 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
     Spawner* spawner = nullptr;
     u32 metadata_index = 0u;
     u32 base_particle = 0u, spawner_seed = 0u, max_update = 0u, write_index = 0u, render_index = 0u;
+    u32 trust_r = 0u, claim_w = 0u;  // identity claims of the instance (see PendingTile)
 #if HNB_SLOT_ORDER
     u32 inst_capacity = 0u;  // slots of the cached instance
 #endif
@@ -566,6 +583,17 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
         write_index = md->indirect_write_index;
         render_index = md->indirect_render_index;
         read_col = P.slab.particle_index[1u - write_index] + base_particle;
+#if HNB_RELAXED_ORDER || HNB_SLOT_ORDER
+        // these orders trust no identity claim, and the list they write ends the instance's claim on the write column
+        if (lane == 0 && P.slab.ident_claim && hnb_claim_len(hnb_claim_load(&P.slab.ident_claim[write_index]), base_particle) != 0u)
+            hnb_claim_store(&P.slab.ident_claim[write_index], 0ull);
+#else
+        if (P.slab.ident_claim) {
+            const u32 claim_r = hnb_claim_len(hnb_claim_load(&P.slab.ident_claim[1u - write_index]), base_particle);
+            trust_r = claim_r < max_update ? claim_r : max_update;
+            claim_w = hnb_claim_len(hnb_claim_load(&P.slab.ident_claim[write_index]), base_particle);
+        }
+#endif
         hnb_ctx.spawner = spawner;
         hnb_ctx.transform = hnb_transform_from_rows(spawner->transform, spawner->transform + 4, spawner->transform + 8);
         hnb_ctx.inverse_transform = hnb_transform_from_rows(spawner->inverse_transform, spawner->inverse_transform + 4,
@@ -652,11 +680,14 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
         u32 my_new_bits = 0u, tile_valid = 0u;
         (void)read_col;
 #else
+        // Rows below trust_r hold their own index (identity claim): their alive-list entries are not loaded. When that covers
+        // the whole tile (warp-uniform), neither are the next sub-tiles' entries prefetched.
+        const bool tile_known = row0 + tile_rows <= trust_r;
         u32 pidx_next[HNB_TILE_K];
 #pragma unroll
         for (int k = 0; k < HNB_TILE_K; ++k) {
             const u32 row = row0 + k * 32u + lane;
-            pidx_next[k] = row < max_update ? read_col[row] : 0u;
+            pidx_next[k] = row < trust_r ? row : (row < max_update ? read_col[row] : 0u);
         }
 #endif
 #pragma unroll 1
@@ -688,10 +719,15 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
             }
             // prefetch the alive-list entries of the next sub-tile (coalesced u32)
             if (j + 1 < chunks) {
+                if (tile_known) {
 #pragma unroll
-                for (int k = 0; k < HNB_TILE_K; ++k) {
-                    const u32 row = row0 + ((j + 1) * HNB_TILE_K + k) * 32u + lane;
-                    pidx_next[k] = row < max_update ? read_col[row] : 0u;
+                    for (int k = 0; k < HNB_TILE_K; ++k) pidx_next[k] = row0 + ((j + 1) * HNB_TILE_K + k) * 32u + lane;
+                } else {
+#pragma unroll
+                    for (int k = 0; k < HNB_TILE_K; ++k) {
+                        const u32 row = row0 + ((j + 1) * HNB_TILE_K + k) * 32u + lane;
+                        pidx_next[k] = row < trust_r ? row : (row < max_update ? read_col[row] : 0u);
+                    }
                 }
             }
 #endif
@@ -774,6 +810,7 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
             pending.render_index = render_index; pending.inst_first_tile = inst_first_tile; pending.inst_end_tile = inst_end_tile;
             pending.metadata_index = metadata_index;
             pending.buffer = cur;
+            pending.trust_r = trust_r; pending.claim_w = claim_w;
 #if HNB_SLOT_ORDER
             pending.tile_valid = tile_valid;
 #endif
@@ -789,6 +826,7 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
             pt.max_update = max_update; pt.write_index = write_index; pt.render_index = render_index;
             pt.inst_first_tile = inst_first_tile; pt.inst_end_tile = inst_end_tile; pt.metadata_index = metadata_index;
             pt.buffer = cur;
+            pt.trust_r = trust_r; pt.claim_w = claim_w;
 #if HNB_SLOT_ORDER
             pt.tile_valid = tile_valid;
             hnb_compact_tile(P, pt, survivors, valids, pidx_stash, chunks, epoch, lane, prof_polls);

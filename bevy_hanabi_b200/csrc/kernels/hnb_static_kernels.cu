@@ -408,10 +408,14 @@ __global__ void k_bits_from_list(u32* bits, const u32* list, u32 base, u32 alive
 //   s = pcg_hash(row ^ seed); six successive pcg_hash -> position, velocity in [-1,1); one more -> lifetime
 // `logical_first`: row of the LOGICAL instance stored at slab row `first` (a shard of an instance split by index range
 // over several devices holds the unsharded instance's values under shard-local indices).
-__global__ void k_fill_c5(float4* pos_age, float4* vel_life, u32* ping, u32* pong, u32 first, u32 count, u32 seed,
+__global__ void k_fill_c5(float4* pos_age, float4* vel_life, u32* ping, u32* pong, u64* claim, u32 first, u32 count, u32 seed,
                           f32 lifetime_lo, f32 lifetime_hi, u32 logical_first) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
+    if (i == 0u) {
+        hnb_claim_store(&claim[0], hnb_claim_pack(first, count));
+        hnb_claim_store(&claim[1], hnb_claim_pack(first, count));
+    }
     const u32 row = first + i;
     u32 s = pcg_hash((logical_first + i) ^ seed);
     f32 v[7];
@@ -650,9 +654,9 @@ cudaError_t launch_bits_from_list(u32* bits, const u32* list, u32 base, u32 aliv
     k_bits_from_list<<<blocks_for(alive_count, 256), 256, 0, st>>>(bits, list, base, alive_count);
     return cudaGetLastError();
 }
-cudaError_t launch_fill_c5(void* pos_age, void* vel_life, u32* ping, u32* pong, u32 first, u32 count, u32 seed, f32 lo, f32 hi, u32 logical_first, cudaStream_t st) {
+cudaError_t launch_fill_c5(void* pos_age, void* vel_life, u32* ping, u32* pong, u64* claim, u32 first, u32 count, u32 seed, f32 lo, f32 hi, u32 logical_first, cudaStream_t st) {
     if (count == 0) return cudaSuccess;
-    k_fill_c5<<<blocks_for(count, 256), 256, 0, st>>>((float4*)pos_age, (float4*)vel_life, ping, pong, first, count, seed, lo, hi, logical_first);
+    k_fill_c5<<<blocks_for(count, 256), 256, 0, st>>>((float4*)pos_age, (float4*)vel_life, ping, pong, claim, first, count, seed, lo, hi, logical_first);
     return cudaGetLastError();
 }
 cudaError_t launch_measure_sm_clock(u64* out2, u64 window_ns, cudaStream_t st) {

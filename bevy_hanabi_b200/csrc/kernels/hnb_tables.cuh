@@ -65,6 +65,18 @@ HNB_HD u32 hnb_tile_count(u32 rows, u32 word) {
     return (rows + S - 1u) / S;
 }
 
+// ---- identity claim of an alive-list column (SlabView::ident_claim, DESIGN.md §3) ------------------------------
+// One 64-bit word per index column: (base << 32) | len means  particle_index[c][base + i] == i  for every i < len that lies
+// in the slice of the instance whose slab offset is `base` (0: no claim). An ordered update pass reads no alive-list entry the
+// claim covers and stores no entry that already holds its value. Every writer of an index column keeps the claim true or
+// shrinks it, in stream order, before any later reader. The word is always read and written as ONE aligned 64-bit access:
+// update passes of other batches on side streams may read it concurrently and must never see a new base with an old length.
+HNB_HD u64 hnb_claim_pack(u32 base, u32 len) { return (u64(base) << 32) | u64(len); }
+HNB_HD u64 hnb_claim_load(const u64* claim) { return *(const volatile u64*)claim; }
+HNB_HD void hnb_claim_store(u64* claim, u64 word) { *(volatile u64*)claim = word; }
+// length of the claim `word` for the instance at slab offset `base` (0 when the claim is another instance's)
+HNB_HD u32 hnb_claim_len(u64 word, u32 base) { return u32(word >> 32) == base ? u32(word) : 0u; }
+
 #define HNB_DRAW_INDEXED_INDIRECT_STRIDE 5u  // vfx_common.wgsl:146
 #define HNB_MAX_PLANES 16
 #define HNB_MAX_EVENT_BINDINGS 4
@@ -87,6 +99,7 @@ struct SlabView {
     u32* particle_index[2];  // ping / pong alive lists (instance-local particle indices)
     u32* dead_index;         // dead stack (slab-global rows)
     u32* alive_bits;         // one bit per slab row: the row holds a particle (kept current by HNB_EFFECT_SLOT_ORDER effects)
+    u64* ident_claim;        // [2]: identity claim of particle_index[0] / [1] (see hnb_claim_pack); NULL = no claims
     u32 capacity_rows;
     u32 _pad;
 };

@@ -88,6 +88,7 @@ struct Slab {
     void* d_planes[HNB_RT_MAX_PLANES] = {};
     uint32_t *ping = nullptr, *pong = nullptr, *dead = nullptr;
     uint32_t* alive_bits = nullptr;  // one bit per row (HNB_EFFECT_SLOT_ORDER effects keep it current)
+    unsigned long long* ident_claim = nullptr;  // [2]: identity claims of ping / pong (hnb_claim_pack)
     // HNB_EFFECT_ORDERED_EVENTS scratch, allocated on first use: per channel the per-row event counts and their block sums
     uint32_t* event_counts[HNB_MAX_EVENT_BINDINGS] = {};
     uint32_t* event_block_sums[HNB_MAX_EVENT_BINDINGS] = {};
@@ -403,8 +404,14 @@ hnb::SlabView slab_view(const Slab& s) {
     v.particle_index[1] = s.pong;
     v.dead_index = s.dead;
     v.alive_bits = s.alive_bits;
+    v.ident_claim = s.ident_claim;
     v.capacity_rows = s.capacity;
     return v;
+}
+
+// Drops both identity claims of the slab, in stream order: for writers of the index columns that do not keep them true.
+void clear_ident_claims(hnb_ctx* c, const Slab& s) {
+    CUDA_CHECK(cudaMemsetAsync(s.ident_claim, 0, 2 * sizeof(unsigned long long), c->stream));
 }
 
 void check_rows(const Slab& s, uint32_t first, uint32_t count) {
@@ -726,6 +733,7 @@ void launch_ribbon_sort(hnb_ctx* c, const LaunchPlan& lp) {
     a.scratch_rows = c->sort_rows;
     a.scratch_grid = uint32_t(c->sm_count);
     if (any_large) CUDA_CHECK(cudaMemsetAsync(c->d_sort_hist, 0, size_t(2 * 8 * 256) * 4, c->stream));
+    clear_ident_claims(c, *lp.slab);  // the sort permutes the column the update just wrote
     uint32_t launched = 0;
     CUDA_CHECK(hnb::launch_ribbon_sort(a, any_large, uint32_t(c->sm_count), c->stream, &launched));
     c->launches += launched;
@@ -832,7 +840,7 @@ void hnb_ctx_destroy(hnb_ctx* c) {
     for (auto& s : c->slabs) {
         if (!s.live) continue;
         for (auto p : s.d_planes) if (p) cudaFree(p);
-        cudaFree(s.ping); cudaFree(s.pong); cudaFree(s.dead); cudaFree(s.alive_bits);
+        cudaFree(s.ping); cudaFree(s.pong); cudaFree(s.dead); cudaFree(s.alive_bits); cudaFree(s.ident_claim);
         for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) { cudaFree(s.event_counts[i]); cudaFree(s.event_block_sums[i]); }
     }
     for (auto& e : c->effects) if (e.d_props) cudaFree(e.d_props);
@@ -892,6 +900,8 @@ int32_t hnb_slab_create_ex(hnb_ctx* c, uint32_t capacity_rows, uint32_t stride, 
         CUDA_CHECK(cudaMalloc((void**)&s.dead, size_t(capacity_rows) * 4));
         CUDA_CHECK(cudaMalloc((void**)&s.alive_bits, (size_t(capacity_rows) / 32 + 2) * 4));
         CUDA_CHECK(cudaMemsetAsync(s.alive_bits, 0, (size_t(capacity_rows) / 32 + 2) * 4, c->stream));
+        CUDA_CHECK(cudaMalloc((void**)&s.ident_claim, 2 * sizeof(unsigned long long)));
+        clear_ident_claims(c, s);
         CUDA_CHECK(hnb::launch_slab_reset(s.ping, s.pong, s.dead, 0, capacity_rows, c->stream));
         c->launches++;
         s.live = true;
@@ -905,8 +915,9 @@ int32_t hnb_slab_destroy(hnb_ctx* c, hnb_slab h) {
         Slab& s = get_slab(c, h);
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
         for (auto& p : s.d_planes) if (p) { cudaFree(p); p = nullptr; }
-        cudaFree(s.ping); cudaFree(s.pong); cudaFree(s.dead); cudaFree(s.alive_bits);
+        cudaFree(s.ping); cudaFree(s.pong); cudaFree(s.dead); cudaFree(s.alive_bits); cudaFree(s.ident_claim);
         s.alive_bits = nullptr;
+        s.ident_claim = nullptr;
         for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
             cudaFree(s.event_counts[i]); cudaFree(s.event_block_sums[i]);
             s.event_counts[i] = s.event_block_sums[i] = nullptr;
@@ -919,6 +930,7 @@ int32_t hnb_slab_reset_rows(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t cou
     return guarded([&] {
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
+        clear_ident_claims(c, s);
         CUDA_CHECK(hnb::launch_slab_reset(s.ping, s.pong, s.dead, first, count, c->stream));
         CUDA_CHECK(hnb::launch_bits_range(s.alive_bits, first, count, false, c->stream));
         c->launches += 2;
@@ -984,6 +996,7 @@ int32_t hnb_slab_upload_indirect(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_
         uint32_t* stage = nullptr;
         CUDA_CHECK(cudaMalloc((void**)&stage, size_t(count) * 12));
         CUDA_CHECK(cudaMemcpyAsync(stage, rows, size_t(count) * 12, cudaMemcpyHostToDevice, c->stream));
+        clear_ident_claims(c, s);
         CUDA_CHECK(hnb::launch_indirect_deinterleave(stage, s.ping, s.pong, s.dead, first, count, c->stream));
         c->launches++;
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
@@ -1043,6 +1056,7 @@ int32_t hnb_slab_import_indirect_device(hnb_ctx* c, hnb_slab h, uint32_t first, 
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
         if (count && !d_src) fail(HNB_ERR_INVALID_ARG, "d_src is NULL");
+        clear_ident_claims(c, s);
         CUDA_CHECK(hnb::launch_indirect_deinterleave((const uint32_t*)d_src, s.ping, s.pong, s.dead, first, count, c->stream));
         c->launches += count ? 1 : 0;
     });
@@ -1102,7 +1116,7 @@ int32_t hnb_slab_fill_c5_ex(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t cou
         check_rows(s, first, count);
         if (s.stride != 32) fail(HNB_ERR_LAYOUT, "hnb_slab_fill_c5 needs the 32-byte {position,age,velocity,lifetime} layout");
         if (s.sector_planes) fail(HNB_ERR_LAYOUT, "hnb_slab_fill_c5 writes the default plane layout; spawn through the init pass or use hnb_slab_upload_aos");
-        CUDA_CHECK(hnb::launch_fill_c5(s.d_planes[0], s.d_planes[1], s.ping, s.pong, first, count, seed, lo, hi, logical_first, c->stream));
+        CUDA_CHECK(hnb::launch_fill_c5(s.d_planes[0], s.d_planes[1], s.ping, s.pong, s.ident_claim, first, count, seed, lo, hi, logical_first, c->stream));
         CUDA_CHECK(hnb::launch_bits_range(s.alive_bits, first, count, true, c->stream));
         c->launches += 2;
     });

@@ -242,6 +242,9 @@ typedef struct hnb_slab_view {
     uint32_t plane_width[16];  /* 16, 8 or 4 bytes (32 with HNB_SLAB_SECTOR_PLANES: two 16-byte pieces per element) */
     uint32_t *ping, *pong, *dead; /* the three u32 columns of IndirectEntry */
 } hnb_slab_view;
+/** A read path for renderers. Writing the index columns (ping / pong) through it is not supported: the update pass may
+ * skip alive-list loads and stores where it knows a column to be the identity, and a write through the view does not
+ * drop that knowledge. Use hnb_slab_import_indirect_device or hnb_slab_upload_indirect to change the lists. */
 HNB_API int32_t hnb_slab_device_view(hnb_ctx* ctx, hnb_slab slab, hnb_slab_view* out);
 /** Rows [first,first+count) as AoS records into `d_dst` (count * particle_stride bytes). */
 HNB_API int32_t hnb_slab_export_aos_device(hnb_ctx* ctx, hnb_slab slab, uint32_t first, uint32_t count, void* d_dst);
