@@ -213,6 +213,7 @@ SIGNATURES = {
     "hnb_read_batch_info": (i32, [vp, u32, P(BatchInfo)]),
     "hnb_read_prefix_sum": (i32, [vp, u32, u32, P(u32)]),
     "hnb_read_dispatch_args": (i32, [vp, u32, P(DispatchIndirectArgs)]),
+    "hnb_read_tile_size": (i32, [vp, u32, P(u32)]),
     "hnb_read_draw_args_async": (i32, [vp, u32, u32, vp]),
     "hnb_ctx_set_count_mailbox": (i32, [vp, vp, u32, u32]),
     "hnb_ctx_last_epoch": (i32, [vp, P(u32)]),

@@ -1715,6 +1715,13 @@ int32_t hnb_read_dispatch_args(hnb_ctx* c, uint32_t row, hnb_dispatch_indirect_a
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
     });
 }
+int32_t hnb_read_tile_size(hnb_ctx* c, uint32_t row, uint32_t* out) {
+    return guarded([&] {
+        if (!out) fail(HNB_ERR_INVALID_ARG, "NULL argument");
+        if (row >= c->B) fail(HNB_ERR_OUT_OF_RANGE, "batch row out of range");
+        *out = c->h_at<uint32_t>(c->lay.off_tile_size)[row];  // host copy of the word plan_batch passed to the batch's last launch
+    });
+}
 
 int32_t hnb_ctx_set_count_mailbox(hnb_ctx* c, uint64_t* pinned_host, uint32_t rows, uint32_t ring) {
     return guarded([&] {

@@ -494,3 +494,9 @@ class Context:
         a = DispatchIndirectArgs()
         check(lib.hnb_read_dispatch_args(self._h, row, C.byref(a)))
         return a
+
+    def read_tile_size(self, row: int) -> int:
+        """Rows per update tile of batch `row` at its last launch (the low 16 bits of hnb_read_tile_size's word)."""
+        w = N.u32()
+        check(lib.hnb_read_tile_size(self._h, row, C.byref(w)))
+        return w.value & 0xFFFF

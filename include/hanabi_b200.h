@@ -442,6 +442,9 @@ HNB_API int32_t hnb_read_spawner(hnb_ctx* ctx, uint32_t row, hnb_spawner* out);
 HNB_API int32_t hnb_read_batch_info(hnb_ctx* ctx, uint32_t row, hnb_batch_info* out);
 HNB_API int32_t hnb_read_prefix_sum(hnb_ctx* ctx, uint32_t first, uint32_t count, uint32_t* out);
 HNB_API int32_t hnb_read_dispatch_args(hnb_ctx* ctx, uint32_t row, hnb_dispatch_indirect_args* out);
+/** Tile size word of batch `row` as its last update launch used it (0 before the first launch): rows per update tile
+ *  (low 16 bits: 32 x K rows per sub-tile x the sub-tile count, see HNB_TILE_CHUNKS) | 0x80000000 for HNB_EFFECT_SLOT_ORDER. */
+HNB_API int32_t hnb_read_tile_size(hnb_ctx* ctx, uint32_t row, uint32_t* out);
 /** Enqueue an async copy of draw-args rows [first,first+count) into caller PINNED memory. */
 HNB_API int32_t hnb_read_draw_args_async(hnb_ctx* ctx, uint32_t first, uint32_t count,
                                          hnb_draw_indexed_indirect_args* pinned_out);

@@ -9,8 +9,51 @@ from dataclasses import dataclass
 from typing import Sequence
 
 import numpy as np
+import pytest
 
 from oracle import c_oracle as O
+
+SUB_TILE_C5 = 128  # rows of an update sub-tile for C5 records: 32 lanes x K = 4 rows in flight per lane
+
+
+@pytest.fixture(params=[1, 2, 3, 4], ids=lambda n: f"{n}sub")
+def tiled_ctx(request, native, monkeypatch):
+    """A fresh context on cuda:0 whose update tiles hold `tile_chunks` sub-tiles, forced with HNB_TILE_CHUNKS (None: the
+    slab-size rule of plan_batch, which picks 1 below one wave of resident warps, about 400 Ki rows for C5, so without the
+    override almost every row-exact test would run 1). The results are the same at every tile size by design, so after a
+    forced run the fixture reads back the tile size of the last launch of batch `tile_batch` (default 0; its effect must
+    have records of at most 36 bytes, as C5's, for 128-row sub-tiles) to prove that the size under test was the one that
+    ran."""
+    chunks = request.param
+    if chunks is None:
+        monkeypatch.delenv("HNB_TILE_CHUNKS", raising=False)
+    else:
+        monkeypatch.setenv("HNB_TILE_CHUNKS", str(chunks))
+    c = native.Context(0)
+    c.tile_chunks, c.tile_batch = chunks, 0
+    try:
+        yield c
+        if chunks is not None:
+            assert c.read_tile_size(c.tile_batch) == SUB_TILE_C5 * chunks, "the update ran at another tile size than the one under test"
+    finally:
+        c.close()
+
+
+FORCED_SUB_TILES = (2, 3, 4)
+
+
+def at_tile_sizes(argnames, values, ids=None, forced_values=()):
+    """`pytest.mark.parametrize` of a test taking `tiled_ctx` and `argnames`: each of `values` runs under its usual id
+    with the slab-size rule, then again at 2, 3 and 4 forced sub-tiles under `<id>-<n>sub`, as do `forced_values`."""
+    names = [n.strip() for n in argnames.split(",")]
+    as_tuple = (lambda v: tuple(v)) if len(names) > 1 else (lambda v: (v,))
+    auto = lambda v: "-".join(str(x) for x in as_tuple(v))  # noqa: E731  (pytest's own ids for ints and strings)
+    ids = list(ids) if ids is not None else [auto(v) for v in values]
+    params = [pytest.param(None, *as_tuple(v), id=i) for v, i in zip(values, ids)]
+    for chunks in FORCED_SUB_TILES:
+        params += [pytest.param(chunks, *as_tuple(v), id=f"{i}-{chunks}sub") for v, i in zip(values, ids)]
+        params += [pytest.param(chunks, *as_tuple(v), id=f"{auto(v)}-{chunks}sub") for v in forced_values]
+    return pytest.mark.parametrize(["tiled_ctx"] + names, params, indirect=["tiled_ctx"])
 
 
 @dataclass

@@ -21,7 +21,8 @@ def _declared():
 def test_headers_declare_something():
     names = [n for _, n in _declared()]
     assert len(names) >= 70
-    for must in ("hnb_ctx_create", "hnb_simulate", "hnb_slab_create", "hnb_effect_compile", "hnb_asset_generate", "hnb_module_binary"):
+    for must in ("hnb_ctx_create", "hnb_simulate", "hnb_slab_create", "hnb_effect_compile", "hnb_asset_generate", "hnb_module_binary",
+                 "hnb_read_tile_size"):  # the tests' proof that HNB_TILE_CHUNKS reached the update launch
         assert must in names
 
 

@@ -8,18 +8,18 @@ from bevy_hanabi_b200 import _native as N
 from bevy_hanabi_b200 import graph as G
 from bevy_hanabi_b200 import runtime as R
 from oracle.hanabi_oracle import EffectOracle, pcg_hash
-from tests.helpers import Instance, RefWorld
+from tests.helpers import Instance, RefWorld, at_tile_sizes, tiled_ctx  # noqa: F401
 from tests.test_gpu_events import EVENT_CAP, _oracle_append_events, _oracle_child_init
 
 pytestmark = pytest.mark.gpu
 A = G.Attribute
 
 
-@pytest.mark.parametrize("pcap", [1024, 6000])
-def test_ordered_events_two_children(ctx, orc, pcap):
+@at_tile_sizes("pcap", [1024, 6000])
+def test_ordered_events_two_children(tiled_ctx, orc, pcap):
     """HNB_EFFECT_ORDERED_EVENTS on the device : with
     ordered append the buffers must hold EXACTLY the canonical sequence, overflow included, and the children need no
-    re-ordering of the oracle's events. Scenario: one parent, two event channels: channel 0 fed every frame by particles that are alive (EventEmitCondition::Always,
+    re-ordering of the oracle's events. With the slab-size rule and at 2-4 forced sub-tiles per tile: an event's row is row0 + (j*K + k)*32 + lane. Scenario: one parent, two event channels: channel 0 fed every frame by particles that are alive (EventEmitCondition::Always,
     count 0 or 1 drawn per particle), channel 1 by dying particles (OnDie, 4 events each). Each child consumes its
     own buffer the frame after. Children come BEFORE the parent in batch order, as EffectSorter places them
     (batch.rs:599-603), so a child's init reads the parent's records before the parent's init recycles slots."""
@@ -44,6 +44,8 @@ def test_ordered_events_two_children(ctx, orc, pcap):
     c_fx = [c.generate(parent=parent) for c in children]
     p_stride, c_stride = p_fx.particle_stride, c_fx[0].particle_stride
     dt = 1.0 / 30.0
+    ctx = tiled_ctx
+    ctx.tile_batch = 2  # the parent: 32-byte records, 128-row sub-tiles (the children's 48-byte records have 64-row ones)
     pw = RefWorld(pcap, p_stride // 4, [Instance(0, pcap, alive=0, seed=1)], dt=dt)
     cw = [RefWorld(4096, c_stride // 4, [Instance(0, 4096, alive=0, seed=2 + k)], dt=dt) for k in (0, 1)]
     po, co = EffectOracle(parent), [EffectOracle(c) for c in children]

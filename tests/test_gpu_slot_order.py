@@ -10,7 +10,7 @@ import pytest
 
 from bevy_hanabi_b200 import _native as N, graph as G, recipes, runtime as R
 from oracle.hanabi_oracle import EffectOracle
-from tests.helpers import GpuWorld, Instance, RefWorld, assert_world_equal
+from tests.helpers import GpuWorld, Instance, RefWorld, assert_world_equal, at_tile_sizes, tiled_ctx  # noqa: F401
 from tests.test_gpu_update_c5 import ACCEL_DRAG, _fill
 
 pytestmark = pytest.mark.gpu
@@ -34,13 +34,14 @@ def _run_c5(ctx, orc, ref, steps):
     return gpu
 
 
-@pytest.mark.parametrize("capacity,alive", [(8192, 5000), (8192, 8192), (8192, 1), (70, 70), (33, 0), (400_000, 380_000), (2_200_000, 2_000_001)])
-def test_c5_with_deaths(ctx, orc, capacity, alive):
-    """1, 2 and 4 sub-tiles per tile (slab sizes as plan_batch picks them), capacities that are no multiple of 32 or of the tile."""
+@at_tile_sizes("capacity,alive", [(8192, 5000), (8192, 8192), (8192, 1), (70, 70), (33, 0), (400_000, 380_000), (2_200_000, 2_000_001)])
+def test_c5_with_deaths(tiled_ctx, orc, capacity, alive):
+    """The sub-tile counts plan_batch picks (1 up to 8192 rows, more at 400 K and 2.2 M), then 2, 3 and 4 forced at every size
+    (the bitmap words a warp owns: chunks x K of them), capacities that are no multiple of 32 or of the tile."""
     rng = np.random.default_rng(capacity + alive)
     ref = RefWorld(capacity, 8, [Instance(0, capacity, alive=alive, seed=42)])
     _fill(ref, rng, 0.02, 0.3)
-    _run_c5(ctx, orc, ref, 8 if capacity > 100_000 else 24)
+    _run_c5(tiled_ctx, orc, ref, 8 if capacity > 100_000 else 24)
     assert ref.metadata[0].alive_count < max(alive, 1)
 
 

@@ -11,7 +11,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.helpers import GpuWorld, Instance, RefWorld, assert_world_equal
+from tests.helpers import FORCED_SUB_TILES, SUB_TILE_C5, GpuWorld, Instance, RefWorld, assert_world_equal, at_tile_sizes, tiled_ctx  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -51,8 +51,16 @@ def test_single_instance_with_deaths(ctx, orc):
     assert ref.metadata[0].alive_count == 0  # everything died, dead stack fully rebuilt
 
 
-@pytest.mark.parametrize("alive", [1, 63, 64, 1023, 1024, 1025, 2048, 4097])
-def test_tile_boundaries(ctx, orc, alive):
+# Alive counts at the edges of a 128-row sub-tile and of larger powers of two; with forced sub-tiles also at the edges of
+# the tile S = 128 x sub-tiles.
+_TILE_EDGES = {"S-1": lambda S: S - 1, "S": lambda S: S, "S+1": lambda S: S + 1, "2S+1": lambda S: 2 * S + 1}
+
+
+@at_tile_sizes("alive", [1, 63, 64, 127, 128, 129, 1023, 1024, 1025, 2048, 4097], forced_values=list(_TILE_EDGES))
+def test_tile_boundaries(tiled_ctx, orc, alive):
+    ctx = tiled_ctx
+    if isinstance(alive, str):
+        alive = _TILE_EDGES[alive](SUB_TILE_C5 * ctx.tile_chunks)
     rng = np.random.default_rng(alive)
     ref = RefWorld(8192, 8, [Instance(0, 8192, alive=alive, seed=7)])
     _fill(ref, rng, 0.02, 0.2)
@@ -90,3 +98,12 @@ def test_no_deaths_identity_list(ctx, orc):
     assert got["draw"][1] == 20000
     np.testing.assert_array_equal(got["indirect"][:, 0], np.arange(20000))
     np.testing.assert_array_equal(got["indirect"][:, 1], np.arange(20000))
+
+
+@pytest.mark.parametrize("tiled_ctx", FORCED_SUB_TILES, ids=lambda n: f"{n}sub", indirect=True)
+@pytest.mark.parametrize("test", [test_single_instance_with_deaths, test_many_instances_one_batch, test_two_batches, test_no_deaths_identity_list],
+                         ids=lambda t: t.__name__[len("test_"):])
+def test_at_forced_tile_sizes(test, tiled_ctx, orc):
+    """The tests above at 2, 3 and 4 sub-tiles per update tile (the slab-size rule picks 1 at their sizes): the prefetch of
+    the next sub-tile's alive-list entries and the stash and ballot slots of sub-tiles after the first."""
+    test(tiled_ctx, orc)
