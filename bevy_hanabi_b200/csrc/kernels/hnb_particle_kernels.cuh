@@ -43,6 +43,9 @@ namespace hnb {
 #define HNB_ROWS_PER_LANE 16
 #endif
 #define HNB_MAX_CHUNKS (HNB_ROWS_PER_LANE / HNB_TILE_K)
+#if HNB_SLOT_ORDER && HNB_ROWS_PER_LANE > 32
+#error "slot order gives each lane one alive-bitmap word of a tile: HNB_ROWS_PER_LANE must be at most 32"
+#endif
 #ifndef HNB_LOOKBACK_GROUPS
 #define HNB_LOOKBACK_GROUPS 1  // predecessors examined per look-back round trip = 32 * groups (with deferred
                                // compaction the first window almost always holds a PREFIX: 1 beat 4 by 2.7 %)

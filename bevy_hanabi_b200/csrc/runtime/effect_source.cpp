@@ -206,10 +206,12 @@ const char* nz(const char* s) { return s ? s : ""; }
 }  // namespace
 
 uint32_t rows_per_lane() {
-    // rows of a tile handled by one lane (tile <= 32 * rows_per_lane rows); HNB_ROWS_PER_LANE env for tuning
+    // rows of a tile handled by one lane (tile <= 32 * rows_per_lane rows); HNB_ROWS_PER_LANE env for tuning, 4-32.
+    // Larger values are clamped to 32: slot order gives each lane one alive-bitmap word of the tile, so a tile may span at
+    // most 32 words (32 x 32 rows).
     if (const char* e = getenv("HNB_ROWS_PER_LANE")) {
         int v = atoi(e);
-        if (v >= 4 && v <= 64) return (uint32_t)v;
+        if (v >= 4) return (uint32_t)std::min(v, 32);
     }
     return 16;
 }

@@ -226,7 +226,7 @@ def build_emulated_effect(lowered, allow_events: bool = False) -> C.CDLL:
     text = PRELUDE + src + DRIVER
     OUT.mkdir(parents=True, exist_ok=True)
     tag = hashlib.sha1(text.encode()).hexdigest()[:16]
-    cpp, so = OUT / f"emu_{tag}.cpp", OUT / f"emu_{tag}.so"
+    cpp, so = OUT / f"emu_{tag}.{os.getpid()}.cpp", OUT / f"emu_{tag}.so"  # per process: workers may build the same tag at once
     if not so.exists():
         cpp.write_text(text)
         cmd = ["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-shared", "-pthread", "-w", str(cpp), "-o", str(so) + f".{os.getpid()}.tmp"]

@@ -166,7 +166,7 @@ def build() -> C.CDLL:
     text = PRELUDE + EXTRA_PRELUDE + wgsl + "\n" + tables + "\n" + header + "\n" + body + DRIVER
     OUT.mkdir(parents=True, exist_ok=True)
     tag = hashlib.sha1(text.encode()).hexdigest()[:16]
-    cpp, so = OUT / f"static_{tag}.cpp", OUT / f"static_{tag}.so"
+    cpp, so = OUT / f"static_{tag}.{os.getpid()}.cpp", OUT / f"static_{tag}.so"  # per process: workers may build the same tag at once
     if not so.exists():
         cpp.write_text(text)
         cmd = ["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-fPIC", "-shared", "-pthread", "-w", str(cpp), "-o", str(so) + f".{os.getpid()}.tmp"]
