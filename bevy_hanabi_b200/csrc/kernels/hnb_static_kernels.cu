@@ -427,6 +427,82 @@ __global__ void k_fill_c5(float4* pos_age, float4* vel_life, u32* ping, u32* pon
     pong[row] = i;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Repack of one instance (hnb_slab_repack): local row i receives the record of local row src[i], the alive slots first in
+// alive-list order, then the dead slots in stack order; afterwards both alive lists and the dead stack are the identity.
+// One gather launch per physical column (into a scratch of `rows` elements, copied back over the slice by the host), then
+// one launch for the lists, the claims and the alive bitmap. n and W come from the device metadata row.
+// ---------------------------------------------------------------------------------------------
+#define RP_THREADS 256
+#define RP_ITEMS 4  // rows per thread in flight: a gather is bound by latency (as hnb_init, DESIGN.md §4.2)
+#define RP_ROWS_PER_BLOCK (RP_THREADS * RP_ITEMS)
+
+// One element of a physical column: 1, 2, 4 or 8 words (4, 8, 16 or 32 bytes; 32 = a sector-plane column).
+template <int W> struct alignas(W >= 4 ? 16 : W * 4) RepackPiece { u32 w[W]; };
+
+// src[i], clamped to the slice: a state that breaks the update invariant gives an unspecified result, never an access
+// outside the slice.
+__device__ __forceinline__ u32 repack_source(const RepackArgs& a, const u32* list, u32 n, u32 i) {
+    const u32 s = i < n ? list[a.first + i] : a.dead[a.first + i] - a.first;
+    return min(s, a.rows - 1u);
+}
+
+template <int W>
+__global__ void __launch_bounds__(RP_THREADS) k_repack_gather(RepackArgs a, const RepackPiece<W>* col, RepackPiece<W>* scratch) {
+    const u32 n = min(a.metadata->alive_count, a.rows);
+    const u32* list = a.metadata->indirect_write_index == 0u ? a.ping : a.pong;
+    const u32 i0 = blockIdx.x * RP_ROWS_PER_BLOCK + threadIdx.x;
+    u32 src[RP_ITEMS];
+#pragma unroll
+    for (u32 k = 0; k < RP_ITEMS; ++k) {
+        const u32 i = i0 + k * RP_THREADS;
+        src[k] = i < a.rows ? repack_source(a, list, n, i) : 0u;
+    }
+    RepackPiece<W> v[RP_ITEMS];
+#pragma unroll
+    for (u32 k = 0; k < RP_ITEMS; ++k)
+        if (i0 + k * RP_THREADS < a.rows) v[k] = col[u64(a.first) + src[k]];
+#pragma unroll
+    for (u32 k = 0; k < RP_ITEMS; ++k)
+        if (i0 + k * RP_THREADS < a.rows) scratch[i0 + k * RP_THREADS] = v[k];
+}
+
+// After every gather (they read the lists): ping = pong = identity below n, dead = identity from n, both claims
+// {first, n}, alive bits set below n and cleared above. Thread t owns row t and, for t < words, bitmap word t of the slice.
+__global__ void __launch_bounds__(RP_THREADS) k_repack_lists(RepackArgs a) {
+    const u32 n = min(a.metadata->alive_count, a.rows);
+    const u32 i = blockIdx.x * RP_THREADS + threadIdx.x;
+    if (i == 0u) {
+        hnb_claim_store(&a.claim[0], hnb_claim_pack(a.first, n));
+        hnb_claim_store(&a.claim[1], hnb_claim_pack(a.first, n));
+    }
+    if (i < a.rows) {
+        if (i < n) {
+            a.ping[a.first + i] = i;
+            a.pong[a.first + i] = i;
+        } else {
+            a.dead[a.first + i] = a.first + i;
+        }
+    }
+    const u32 w0 = a.first >> 5u;
+    const u64 end = u64(a.first) + a.rows, alive_end = u64(a.first) + n;
+    const u32 w = w0 + i;
+    if (u64(w) * 32u >= end) return;
+    const u64 lo = u64(w) * 32u > a.first ? u64(w) * 32u : u64(a.first);
+    const u64 hi = u64(w) * 32u + 32u < end ? u64(w) * 32u + 32u : end;
+    const u64 alive_hi = hi < alive_end ? hi : alive_end;
+    const u32 sh = u32(lo - u64(w) * 32u);
+    const u32 span = u32(hi - lo), alive = alive_hi > lo ? u32(alive_hi - lo) : 0u;
+    const u32 inside = (span == 32u ? 0xffffffffu : ((1u << span) - 1u)) << sh;
+    const u32 set = (alive == 32u ? 0xffffffffu : ((1u << alive) - 1u)) << sh;
+    if (inside == 0xffffffffu) {
+        a.alive_bits[w] = set;
+    } else {  // a word shared with a neighbouring instance: change only the slice's bits
+        atomicAnd(&a.alive_bits[w], ~inside | set);
+        if (set) atomicOr(&a.alive_bits[w], set);
+    }
+}
+
 // Order-independent checksum: sum over rows of a 64-bit mix of the row's AoS words and row index.
 __global__ void k_checksum(PlaneSet planes, u32 first, u32 count, u32 stride_words, u64 index_base, u64* out) {
     u64 acc = 0;
@@ -657,6 +733,23 @@ cudaError_t launch_bits_from_list(u32* bits, const u32* list, u32 base, u32 aliv
 cudaError_t launch_fill_c5(void* pos_age, void* vel_life, u32* ping, u32* pong, u64* claim, u32 first, u32 count, u32 seed, f32 lo, f32 hi, u32 logical_first, cudaStream_t st) {
     if (count == 0) return cudaSuccess;
     k_fill_c5<<<blocks_for(count, 256), 256, 0, st>>>((float4*)pos_age, (float4*)vel_life, ping, pong, claim, first, count, seed, lo, hi, logical_first);
+    return cudaGetLastError();
+}
+cudaError_t launch_repack_gather(const RepackArgs& a, const void* col, void* scratch, u32 width, cudaStream_t st) {
+    if (a.rows == 0) return cudaSuccess;
+    const unsigned blocks = blocks_for(a.rows, RP_ROWS_PER_BLOCK);
+    switch (width) {
+    case 4: k_repack_gather<1><<<blocks, RP_THREADS, 0, st>>>(a, (const RepackPiece<1>*)col, (RepackPiece<1>*)scratch); break;
+    case 8: k_repack_gather<2><<<blocks, RP_THREADS, 0, st>>>(a, (const RepackPiece<2>*)col, (RepackPiece<2>*)scratch); break;
+    case 16: k_repack_gather<4><<<blocks, RP_THREADS, 0, st>>>(a, (const RepackPiece<4>*)col, (RepackPiece<4>*)scratch); break;
+    case 32: k_repack_gather<8><<<blocks, RP_THREADS, 0, st>>>(a, (const RepackPiece<8>*)col, (RepackPiece<8>*)scratch); break;
+    default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
+}
+cudaError_t launch_repack_lists(const RepackArgs& a, cudaStream_t st) {
+    if (a.rows == 0) return cudaSuccess;
+    k_repack_lists<<<blocks_for(a.rows, RP_THREADS), RP_THREADS, 0, st>>>(a);
     return cudaGetLastError();
 }
 cudaError_t launch_measure_sm_clock(u64* out2, u64 window_ns, cudaStream_t st) {

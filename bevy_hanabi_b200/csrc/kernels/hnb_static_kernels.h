@@ -70,6 +70,22 @@ struct EventAppendArgs {
 cudaError_t launch_ordered_event_append(const EventAppendArgs& a, u32 capacity_rows, cudaStream_t st);
 inline u32 ordered_event_blocks(u32 capacity_rows) { return (capacity_rows + 2047u) / 2048u; }
 
+// Repack of one instance (hnb_slab_repack): slab rows [first, first+rows), its metadata row (alive_count, and
+// indirect_write_index naming the alive list to follow). Pointers are the slab's row-0 columns.
+struct RepackArgs {
+    const EffectMetadata* metadata;
+    u32* ping;
+    u32* pong;
+    u32* dead;
+    u32* alive_bits;
+    u64* claim;  // [2]: the slab's identity claims
+    u32 first, rows;
+};
+// scratch[i] = col[first + src[i]] for i < rows, `width` = bytes per element of the column (4, 8, 16 or 32)
+cudaError_t launch_repack_gather(const RepackArgs& a, const void* col, void* scratch, u32 width, cudaStream_t st);
+// lists, claims and alive bits; enqueue after every gather of the instance
+cudaError_t launch_repack_lists(const RepackArgs& a, cudaStream_t st);
+
 cudaError_t launch_indirect(const StaticTables& T, u32 num_effects, cudaStream_t st);
 cudaError_t launch_prefix_sum(const StaticTables& T, u32 num_batches, cudaStream_t st);
 cudaError_t launch_tile_prefix(const StaticTables& T, u32 batch_index, u32 tile, cudaStream_t st);

@@ -1122,6 +1122,52 @@ int32_t hnb_slab_fill_c5_ex(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t cou
     });
 }
 
+// The scratch (rows x the widest column) is taken with cudaMallocAsync and given back with cudaFreeAsync on the context
+// stream: the call stays asynchronous (no synchronisation to grow or free a buffer the stream may still use), and a
+// context does not keep up to 2 GiB between repacks that may be seconds apart.
+int32_t hnb_slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows) {
+    return guarded([&] {
+        Slab& s = get_slab(c, h);
+        const Effect& fx = get_effect(c, e);
+        if (uint64_t(first) + rows > s.capacity) fail(HNB_ERR_INVALID_ARG, "hnb_slab_repack: rows outside the slab");
+        if (metadata_row >= c->md_rows) fail(HNB_ERR_INVALID_ARG, "hnb_slab_repack: metadata row out of range");
+        if (fx.particle_stride != s.stride) fail(HNB_ERR_INVALID_ARG, "hnb_slab_repack: effect particle stride does not match the slab");
+        if (((fx.flags & HNB_EFFECT_SECTOR_PLANES) != 0) != s.sector_planes)
+            fail(HNB_ERR_INVALID_ARG, "hnb_slab_repack: effect and slab disagree on HNB_EFFECT_SECTOR_PLANES / HNB_SLAB_SECTOR_PLANES");
+        if (fx.flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS)
+            fail(HNB_ERR_INVALID_ARG, "hnb_slab_repack: pending GPU spawn events name parent slots; an emitting effect cannot be repacked");
+        if (rows == 0) return;
+        CUDA_CHECK(cudaSetDevice(c->device));
+        hnb::RepackArgs a{};
+        a.metadata = c->d_metadata + metadata_row;
+        a.ping = s.ping;
+        a.pong = s.pong;
+        a.dead = s.dead;
+        a.alive_bits = s.alive_bits;
+        a.claim = s.ident_claim;
+        a.first = first;
+        a.rows = rows;
+        uint32_t widest = 0;
+        for (const Plane& p : s.planes) widest = std::max(widest, p.width);
+        void* scratch = nullptr;
+        CUDA_CHECK(cudaMallocAsync(&scratch, size_t(rows) * widest, c->stream));
+        cudaError_t err = cudaSuccess;
+        for (size_t p = 0; p < s.planes.size() && err == cudaSuccess; ++p) {
+            const uint32_t width = s.planes[p].width;
+            err = hnb::launch_repack_gather(a, s.d_planes[p], scratch, width, c->stream);
+            if (err == cudaSuccess)
+                err = cudaMemcpyAsync((char*)s.d_planes[p] + size_t(first) * width, scratch, size_t(rows) * width, cudaMemcpyDeviceToDevice, c->stream);
+            c->launches++;
+        }
+        // the lists last: every gather reads them
+        if (err == cudaSuccess) err = hnb::launch_repack_lists(a, c->stream);
+        c->launches++;
+        const cudaError_t freed = cudaFreeAsync(scratch, c->stream);
+        CUDA_CHECK(err);
+        CUDA_CHECK(freed);
+    });
+}
+
 int32_t hnb_slab_checksum(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, uint64_t* out) {
     return hnb_slab_checksum_ex(c, h, first, count, 0, out);
 }

@@ -280,6 +280,12 @@ class Context:
         """`logical_first`: the slab rows hold logical rows [logical_first, +count) of an instance sharded over devices."""
         check(lib.hnb_slab_fill_c5_ex(self._h, slab, first, count, seed, lifetime_lo, lifetime_hi, first if logical_first is None else logical_first))
 
+    def slab_repack(self, slab: int, effect: int, metadata_row: int, first: int, rows: int) -> None:
+        """Move the live particles of the instance at slab rows [first, first+rows) (`rows` = its capacity) to the front of
+        its slice in alive-list order; both alive lists and the dead stack become the identity and carry identity claims
+        again (hnb_slab_repack). Call between frames; only enqueues work on the context stream."""
+        check(lib.hnb_slab_repack(self._h, slab, effect, metadata_row, first, rows))
+
     def slab_checksum(self, slab: int, first: int, count: int, index_base: int = 0) -> int:
         out = C.c_uint64(0)
         check(lib.hnb_slab_checksum_ex(self._h, slab, first, count, index_base, C.byref(out)))

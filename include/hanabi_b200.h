@@ -166,6 +166,7 @@ HNB_API void hnb_ctx_frame_count(hnb_ctx* ctx, uint64_t* frames, uint64_t* frame
 /* 3. Particle slabs ≙ ParticleSlab::new (reference src/render/effect_cache.rs:246-356)  */
 /* ------------------------------------------------------------------------------------ */
 typedef uint32_t hnb_slab;
+typedef uint32_t hnb_effect;  /* a compiled effect registered with a context (section 4) */
 
 /**
  * Allocate a slab of `capacity_rows` particles whose reference AoS record is
@@ -215,6 +216,37 @@ HNB_API int32_t hnb_slab_fill_c5(hnb_ctx* ctx, hnb_slab slab, uint32_t first, ui
  *  holding the whole instance would have there — under shard-local particle indices. */
 HNB_API int32_t hnb_slab_fill_c5_ex(hnb_ctx* ctx, hnb_slab slab, uint32_t first, uint32_t count,
                                     uint32_t seed, float lifetime_lo, float lifetime_hi, uint32_t logical_first);
+/**
+ * Repack one instance so that its particles are contiguous again and the update pass reads its alive list as the identity
+ * (coalesced record access, and the 64 B per particle-step path of DESIGN.md §4.1). A long-running effect spawns into
+ * whatever slots died, so its alive list drifts into a permutation of its slice; call this between frames, for example
+ * every few seconds for each long-running instance.
+ *
+ * The instance occupies slab rows [first, first+rows) (`rows` must be its capacity: a precondition, not checked on the
+ * device), its metadata row is `metadata_row`, and `effect` is the effect it runs. Call it between hnb_simulate calls,
+ * where the update invariant holds. With W = indirect_write_index and n = min(alive_count, rows) read from the DEVICE
+ * metadata row, list = column W (instance-local values) and dead = the dead stack (slab-global values):
+ *   - local row i takes the record of local row src[i], for every plane and all `rows` rows (dead ones too):
+ *     src[i] = list[first+i] for i < n, dead[first+i] - first for n <= i < rows (alive slots in list order, then dead slots
+ *     in stack order; a bijection when the invariant holds);
+ *   - ping[first+i] = pong[first+i] = i for i < n (rows >= n of both columns are left as they are);
+ *     dead[first+i] = first+i for n <= i < rows (rows < n are left as they are), so later spawns take slots n, n+1, ...;
+ *   - both identity claims of the slab become {first, n} (a claim another instance of the slab held is dropped);
+ *   - the alive bitmap of the slice has bits < n set and the rest cleared (HNB_EFFECT_SLOT_ORDER).
+ * Metadata, draw args, spawners, counters and the count mailbox do not change. Ribbon effects may be repacked: the
+ * repack makes the sorted order the slot order, and PREV/NEXT words move with their record unchanged (no pass maintains
+ * links: they keep the value init gave them).
+ *
+ * Work is only enqueued on the context stream (no host synchronisation, no device->host read): it is ordered after
+ * every launch of the previous hnb_simulate and before the next one. A state that breaks the invariant gives an
+ * unspecified result, but no access outside the slice. The scratch (rows x the widest physical column: 1 GiB for a
+ * 64 Mi-row 32-byte instance) comes from cudaMallocAsync on the context stream and is released the same way.
+ * HNB_ERR_INVALID_ARG, with nothing enqueued, when the rows lie outside the slab, the metadata row is out of range, the
+ * effect's stride or HNB_EFFECT_SECTOR_PLANES flag does not match the slab, or the effect has
+ * HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS (pending events name parent slots that the child's next init reads).
+ */
+HNB_API int32_t hnb_slab_repack(hnb_ctx* ctx, hnb_slab slab, hnb_effect effect, uint32_t metadata_row, uint32_t first,
+                                uint32_t rows);
 /** 64-bit FNV-style checksum of the AoS bytes of rows [first,first+count), computed on device
  *  (order-independent sum of per-row hashes), for whole-slab comparisons at sizes the host
  *  cannot download cheaply. */
@@ -262,7 +294,7 @@ HNB_API int32_t hnb_device_upload(hnb_ctx* ctx, void* d_dst, const void* host_sr
 /* 4. Compiled effects ≙ pipeline specialisation (reference mod.rs:1758,1866;            */
 /*    templates vfx_init.wgsl / vfx_update.wgsl)                                          */
 /* ------------------------------------------------------------------------------------ */
-typedef uint32_t hnb_effect;
+/* hnb_effect: declared with hnb_slab above */
 
 /** Value types of attributes/properties (reference src/graph/mod.rs ValueType). */
 typedef enum hnb_value_type {

@@ -208,11 +208,8 @@ def many_batches():
         ctx.close()
 
 
-def churn(sector_planes: bool = False, slot_order: bool = False):
-    """Steady-state churn: constant spawn rate into recycled slots until the alive list is a random-looking permutation
-    of the slab (survivors keep their relative order, new particles land in whatever slots died). The gathers then touch
-    scattered 16-byte plane elements (half-used 32-byte sectors): the honest number for long-running effects, unlike the
-    freshly filled slabs of the other rows."""
+def _churned(sector_planes: bool = False, slot_order: bool = False):
+    """16 Mi slots of drifting sparks after 240 frames of constant spawning into recycled slots."""
     from tests.test_gpu_scene import _drifting_sparks
     P = 16 << 20
     ctx = hb.Context(0, stream.cuda_stream)
@@ -229,6 +226,15 @@ def churn(sector_planes: bool = False, slot_order: bool = False):
         ctx.set_sim_params(dt, f * dt, 1)
         ctx.upload_spawners([R.make_spawner(spawn=rate, seed=1000 + f)])
         ctx.simulate([N.BatchLaunch.make(effect, slab, 0, rate)])
+    return P, ctx, slab, effect, stride, dt, rate
+
+
+def churn(sector_planes: bool = False, slot_order: bool = False):
+    """Steady-state churn: constant spawn rate into recycled slots until the alive list is a random-looking permutation
+    of the slab (survivors keep their relative order, new particles land in whatever slots died). The gathers then touch
+    scattered 16-byte plane elements (half-used 32-byte sectors): the honest number for long-running effects, unlike the
+    freshly filled slabs of the other rows."""
+    P, ctx, slab, effect, stride, dt, rate = _churned(sector_planes, slot_order)
     alive = ctx.read_metadata(0).alive_count
     ind = ctx.slab_download_indirect(slab, 0, 1 << 16)
     col = ctx.read_metadata(0).indirect_write_index
@@ -289,6 +295,109 @@ def c5_slot():
 def churn_sector():
     """The same with HNB_SLAB_SECTOR_PLANES (32-byte-wide columns): one full sector per gathered record."""
     churn(sector_planes=True)
+
+
+def _card():
+    """Name and power limit of cuda:0 (read-only query), printed with the numbers they qualify."""
+    import subprocess
+    try:
+        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        q = f"nvidia-smi unavailable ({type(e).__name__})"
+    print(f"card: {torch.cuda.get_device_name(0)} | {q}", flush=True)
+
+
+def _repack_bytes(ctx, slab, rows, alive):
+    """Bytes hnb_slab_repack moves: per column a gather (src word + scattered element read + scratch write) and the copy
+    back (read + write); then ping / pong below n, dead from n, and the alive bitmap."""
+    v = ctx.slab_device_view(slab)
+    widths = [v.plane_width[p] for p in range(v.num_planes)]
+    return sum(rows * (4 + 4 * w) for w in widths) + 8 * alive + 4 * (rows - alive) + rows // 8
+
+
+def _timed_repack(ctx, slab, effect, rows):
+    ctx.sync()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(stream)
+    ctx.slab_repack(slab, effect, 0, 0, rows)
+    e1.record(stream)
+    e1.synchronize()
+    return e0.elapsed_time(e1)
+
+
+def churn_repack():
+    """hnb_slab_repack on the churn steady state: the update time of the churned slab, the repack's own time (CUDA events
+    around the call: gathers, copies back, lists; the scratch comes from cudaMallocAsync inside the window), then the update
+    time at frames +1..+10, +60 and +240 under the same constant spawning, and a second repack at +240. Then an init-filled
+    C5 instance (64 Mi rows, one burst through hnb_init: identity list, no claim) before and after a repack."""
+    _card()
+    P, ctx, slab, effect, stride, dt, rate = _churned()
+    frame = [240]
+
+    def step_ms():
+        f = frame[0]
+        ctx.set_sim_params(dt, f * dt, 1)
+        ctx.upload_spawners([R.make_spawner(spawn=rate, seed=1000 + f)])
+        frame[0] += 1
+        return timed_update(ctx, [N.BatchLaunch.make(effect, slab, 0, rate)], 1)
+
+    ms = sum(step_ms() for _ in range(10)) / 10
+    alive = ctx.read_metadata(0).alive_count
+    report(f"churn_repack: churned update, {alive >> 10} Ki of {P >> 10} Ki alive", ms, (8 + 2 * stride) * alive, "mean of 10 frames")
+    def repack(label):
+        alive = ctx.read_metadata(0).alive_count
+        rp = _timed_repack(ctx, slab, effect, P)
+        report(f"churn_repack: {label} repack of {P >> 20} Mi rows, {alive >> 10} Ki alive", rp, _repack_bytes(ctx, slab, P, alive),
+               "bytes: gathers + copies back + lists")
+
+    repack("first")
+    since, out = 0, []
+    for target in list(range(1, 11)) + [60, 240]:
+        while since < target:
+            t = step_ms()
+            since += 1
+        out.append((target, t, ctx.read_metadata(0).alive_count))
+    for target, t, a in out:
+        report(f"churn_repack: update at frame +{target} after the repack", t, (8 + 2 * stride) * a, f"{a >> 10} Ki alive")
+    repack("second (+240)")
+    ctx.close()
+
+    # init-filled C5-like instance: the identity list of a burst into a fresh slab carries no claim until a repack
+    P = 64 << 20
+    w = G.ExprWriter()
+    asset = (G.EffectAsset(P, w.module, name="c5_spawned")
+             .init(G.SetAttributeModifier(A.POSITION, w.rand(G.VEC3) * w.lit(2.) - w.lit(1.)))
+             .init(G.SetAttributeModifier(A.VELOCITY, w.rand(G.VEC3) * w.lit(2.) - w.lit(1.)))
+             .init(G.SetAttributeModifier(A.AGE, w.lit(0.)))
+             .init(G.SetAttributeModifier(A.LIFETIME, w.lit(1e9)))
+             .update(G.AccelModifier(w.lit(G.Vec3(0., -9.8, 0.))))
+             .update(G.LinearDragModifier(w.lit(0.5))))
+    ctx = hb.Context(0, stream.cuda_stream)
+    fx = asset.generate()
+    slab = ctx.slab_create(P, fx.particle_stride)
+    effect = ctx.effect_compile(fx)
+    ctx.metadata_insert(0, R.initial_metadata(P, 0, fx.particle_stride // 4))
+    ctx.draw_args_insert(0)
+    ctx.upload_batches([N.BatchInfo(0, 0, 0, 0, 0, 1)], [0])
+    ctx.set_sim_params(1 / 60, 0.0, 1)
+    ctx.upload_spawners([R.make_spawner(spawn=P, seed=7)])
+    ctx.simulate([N.BatchLaunch.make(effect, slab, 0, P)])
+    ctx.upload_spawners([R.make_spawner(spawn=0, seed=8)])
+    la = [N.BatchLaunch.make(effect, slab, 0, 0)]
+    for _ in range(3):
+        ctx.simulate(la)
+    alive = ctx.read_metadata(0).alive_count
+    before = timed_update(ctx, la, 30)
+    rp = _timed_repack(ctx, slab, effect, P)
+    for _ in range(3):
+        ctx.simulate(la)
+    after = timed_update(ctx, la, 30)
+    report(f"churn_repack: init-filled C5 {alive >> 20} Mi, update before repack", before, 72 * alive, "72 B per particle-step")
+    report(f"churn_repack: init-filled C5 {alive >> 20} Mi, repack", rp, _repack_bytes(ctx, slab, P, alive))
+    report(f"churn_repack: init-filled C5 {alive >> 20} Mi, update after repack", after, 64 * alive,
+           f"64 B per particle-step; {100 * (after - before) / before:+.1f} % per launch")
+    ctx.close()
 
 
 def fresh_sector():
@@ -481,7 +590,7 @@ def c3_chain():
         ctx.close()
 
 
-SCENARIOS = {"c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
+SCENARIOS = {"c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
 if __name__ == "__main__":
     for name in (sys.argv[1:] or list(SCENARIOS)):
         try:
