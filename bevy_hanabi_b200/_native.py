@@ -172,6 +172,9 @@ SIGNATURES = {
     "hnb_slab_checksum_indirect": (i32, [vp, u32, u32, u32, P(C.c_uint64)]),
     "hnb_slab_fill_c5_ex": (i32, [vp, u32, u32, u32, u32, f32, f32, u32]),
     "hnb_slab_repack": (i32, [vp, u32, u32, u32, u32, u32]),
+    "hnb_instance_snapshot_bytes": (C.c_size_t, [u32, u32]),
+    "hnb_instance_snapshot": (i32, [vp, u32, u32, u32, u32, u32, vp, C.c_size_t]),
+    "hnb_instance_restore": (i32, [vp, u32, u32, u32, u32, u32, vp, C.c_size_t]),
     "hnb_slab_checksum_ex": (i32, [vp, u32, u32, u32, C.c_uint64, P(C.c_uint64)]),
     "hnb_slab_device_view": (i32, [vp, u32, P(SlabView)]),
     "hnb_slab_export_aos_device": (i32, [vp, u32, u32, u32, vp]),

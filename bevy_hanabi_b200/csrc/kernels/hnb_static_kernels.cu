@@ -503,6 +503,139 @@ __global__ void __launch_bounds__(RP_THREADS) k_repack_lists(RepackArgs a) {
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Snapshot / restore of one instance (hnb_instance_snapshot / hnb_instance_restore). A snapshot is a 64-byte header
+// followed by reference AoS records in alive-list order: record i sits at word HNB_SNAPSHOT_HEADER_WORDS + i * stride_words.
+// Both kernels move one physical column at a time, RP_ITEMS rows in flight per thread, and split a piece into the widest
+// accesses the record stride and the piece's offset in the record allow (16, 8 or 4 bytes; the buffer is 16-byte aligned).
+// ---------------------------------------------------------------------------------------------
+template <int Q, int W> __device__ __forceinline__ void snapshot_store(u32* dst, const RepackPiece<W>& v) {
+#pragma unroll
+    for (int j = 0; j < W / Q; ++j) {
+        RepackPiece<Q> q;
+#pragma unroll
+        for (int k = 0; k < Q; ++k) q.w[k] = v.w[j * Q + k];
+        ((RepackPiece<Q>*)dst)[j] = q;
+    }
+}
+template <int Q, int W> __device__ __forceinline__ void snapshot_load(const u32* src, RepackPiece<W>& v) {
+#pragma unroll
+    for (int j = 0; j < W / Q; ++j) {
+        const RepackPiece<Q> q = ((const RepackPiece<Q>*)src)[j];
+#pragma unroll
+        for (int k = 0; k < Q; ++k) v.w[j * Q + k] = q.w[k];
+    }
+}
+// words of alignment shared by every record's piece at word `off`: 4, 2 or 1
+__device__ __forceinline__ u32 snapshot_align(u32 stride_words, u32 off) {
+    const u32 m = stride_words | off;
+    return (m & 3u) == 0u ? 4u : ((m & 1u) == 0u ? 2u : 1u);
+}
+
+// records i0 + k * RP_THREADS < n of column p: local rows src[k] -> AoS records in `dst`
+template <int W>
+__device__ __forceinline__ void snapshot_column(const SnapshotArgs& a, u32 p, const u32 (&src)[RP_ITEMS], u32 i0, u32 n, u32* dst) {
+    const RepackPiece<W>* col = (const RepackPiece<W>*)a.planes.ptr[p] + a.first;
+    const u32 off = a.planes.word_off[p], al = snapshot_align(a.stride_words, off);
+    RepackPiece<W> v[RP_ITEMS];
+#pragma unroll
+    for (u32 k = 0; k < RP_ITEMS; ++k)
+        if (i0 + k * RP_THREADS < n) v[k] = col[src[k]];
+#pragma unroll
+    for (u32 k = 0; k < RP_ITEMS; ++k) {
+        const u32 i = i0 + k * RP_THREADS;
+        if (i >= n) continue;
+        u32* d = dst + HNB_SNAPSHOT_HEADER_WORDS + u64(i) * a.stride_words + off;
+        if (W >= 4 && al == 4u) snapshot_store<4>(d, v[k]);
+        else if (W >= 2 && al >= 2u) snapshot_store<2>(d, v[k]);
+        else snapshot_store<1>(d, v[k]);
+    }
+}
+
+// Header by the first 16 threads, then record i < n = min(alive_count, rows) from local row list_W[i] (clamped to the
+// slice as repack_source clamps it). Reads nothing but the metadata row, column W and the planes.
+__global__ void __launch_bounds__(RP_THREADS) k_snapshot_gather(SnapshotArgs a, u32* dst) {
+    const EffectMetadata* md = a.metadata;
+    const u32 n = min(md->alive_count, a.rows);
+    if (blockIdx.x == 0u && threadIdx.x < HNB_SNAPSHOT_HEADER_WORDS) {
+        const u32 t = threadIdx.x;
+        dst[t] = t == 0u ? HNB_SNAPSHOT_MAGIC_WORD
+               : t == 1u ? HNB_SNAPSHOT_VERSION_WORD
+               : t == 2u ? a.stride_words * 4u
+               : t == 3u ? n
+               : t == 4u ? md->particle_counter
+               : t == 5u ? a.rows
+               : 0u;
+    }
+    const u32* list = md->indirect_write_index == 0u ? a.ping : a.pong;
+    const u32 i0 = blockIdx.x * RP_ROWS_PER_BLOCK + threadIdx.x;
+    if (i0 >= n) return;
+    u32 src[RP_ITEMS];
+#pragma unroll
+    for (u32 k = 0; k < RP_ITEMS; ++k) {
+        const u32 i = i0 + k * RP_THREADS;
+        src[k] = i < n ? min(list[a.first + i], a.rows - 1u) : 0u;
+    }
+    for (u32 p = 0; p < a.num_planes; ++p) {
+        switch (a.planes.words[p]) {
+        case 1: snapshot_column<1>(a, p, src, i0, n, dst); break;
+        case 2: snapshot_column<2>(a, p, src, i0, n, dst); break;
+        case 4: snapshot_column<4>(a, p, src, i0, n, dst); break;
+        default: snapshot_column<8>(a, p, src, i0, n, dst); break;
+        }
+    }
+}
+
+// m = min(count, rows, records the buffer holds); 0 for a header that is not a version-1 snapshot of this stride
+__device__ __forceinline__ u32 restore_count(const SnapshotArgs& a, const u32* src) {
+    if (src[0] != HNB_SNAPSHOT_MAGIC_WORD || src[1] != HNB_SNAPSHOT_VERSION_WORD || src[2] != a.stride_words * 4u) return 0u;
+    const u64 fit = (a.src_bytes - HNB_SNAPSHOT_HEADER_WORDS * 4u) / (a.stride_words * 4u);
+    const u64 m = src[3] < a.rows ? src[3] : a.rows;
+    return u32(m < fit ? m : fit);
+}
+
+template <int W>
+__device__ __forceinline__ void restore_column(const SnapshotArgs& a, u32 p, u32 i0, u32 m, const u32* src) {
+    RepackPiece<W>* col = (RepackPiece<W>*)a.planes.ptr[p] + a.first;
+    const u32 off = a.planes.word_off[p], al = snapshot_align(a.stride_words, off);
+    RepackPiece<W> v[RP_ITEMS];
+#pragma unroll
+    for (u32 k = 0; k < RP_ITEMS; ++k) {
+        const u32 i = i0 + k * RP_THREADS;
+        if (i >= m) continue;
+        const u32* s = src + HNB_SNAPSHOT_HEADER_WORDS + u64(i) * a.stride_words + off;
+        if (W >= 4 && al == 4u) snapshot_load<4>(s, v[k]);
+        else if (W >= 2 && al >= 2u) snapshot_load<2>(s, v[k]);
+        else snapshot_load<1>(s, v[k]);
+    }
+#pragma unroll
+    for (u32 k = 0; k < RP_ITEMS; ++k)
+        if (i0 + k * RP_THREADS < m) col[i0 + k * RP_THREADS] = v[k];
+}
+
+// Record i < m -> local row i of every column; thread 0 writes alive_count = m, max_spawn = capacity - m (0 if the row's
+// capacity is below m) and, for an accepted header, particle_counter. k_repack_lists follows and reads m back.
+__global__ void __launch_bounds__(RP_THREADS) k_restore_scatter(SnapshotArgs a, const u32* src) {
+    const u32 m = restore_count(a, src);
+    const u32 i0 = blockIdx.x * RP_ROWS_PER_BLOCK + threadIdx.x;
+    if (i0 == 0u) {
+        EffectMetadata* md = a.metadata;
+        md->alive_count = m;
+        md->max_spawn = md->capacity > m ? md->capacity - m : 0u;
+        if (src[0] == HNB_SNAPSHOT_MAGIC_WORD && src[1] == HNB_SNAPSHOT_VERSION_WORD && src[2] == a.stride_words * 4u)
+            md->particle_counter = src[4];
+    }
+    if (i0 >= m) return;
+    for (u32 p = 0; p < a.num_planes; ++p) {
+        switch (a.planes.words[p]) {
+        case 1: restore_column<1>(a, p, i0, m, src); break;
+        case 2: restore_column<2>(a, p, i0, m, src); break;
+        case 4: restore_column<4>(a, p, i0, m, src); break;
+        default: restore_column<8>(a, p, i0, m, src); break;
+        }
+    }
+}
+
 // Order-independent checksum: sum over rows of a 64-bit mix of the row's AoS words and row index.
 __global__ void k_checksum(PlaneSet planes, u32 first, u32 count, u32 stride_words, u64 index_base, u64* out) {
     u64 acc = 0;
@@ -750,6 +883,16 @@ cudaError_t launch_repack_gather(const RepackArgs& a, const void* col, void* scr
 cudaError_t launch_repack_lists(const RepackArgs& a, cudaStream_t st) {
     if (a.rows == 0) return cudaSuccess;
     k_repack_lists<<<blocks_for(a.rows, RP_THREADS), RP_THREADS, 0, st>>>(a);
+    return cudaGetLastError();
+}
+cudaError_t launch_snapshot_gather(const SnapshotArgs& a, u32* dst, cudaStream_t st) {
+    if (a.rows == 0) return cudaSuccess;
+    k_snapshot_gather<<<blocks_for(a.rows, RP_ROWS_PER_BLOCK), RP_THREADS, 0, st>>>(a, dst);
+    return cudaGetLastError();
+}
+cudaError_t launch_restore_scatter(const SnapshotArgs& a, const u32* src, cudaStream_t st) {
+    if (a.rows == 0) return cudaSuccess;
+    k_restore_scatter<<<blocks_for(a.rows, RP_ROWS_PER_BLOCK), RP_THREADS, 0, st>>>(a, src);
     return cudaGetLastError();
 }
 cudaError_t launch_measure_sm_clock(u64* out2, u64 window_ns, cudaStream_t st) {

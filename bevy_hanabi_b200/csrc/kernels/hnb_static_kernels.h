@@ -86,6 +86,26 @@ cudaError_t launch_repack_gather(const RepackArgs& a, const void* col, void* scr
 // lists, claims and alive bits; enqueue after every gather of the instance
 cudaError_t launch_repack_lists(const RepackArgs& a, cudaStream_t st);
 
+// Snapshot / restore of one instance (hnb_instance_snapshot / hnb_instance_restore): the header words of
+// hnb_instance_snapshot_header (include/hanabi_b200.h), then reference AoS records of stride_words words each.
+#define HNB_SNAPSHOT_HEADER_WORDS 16u
+#define HNB_SNAPSHOT_MAGIC_WORD 0x53424E48u  // "HNBS" in little-endian byte order
+#define HNB_SNAPSHOT_VERSION_WORD 1u
+struct SnapshotArgs {
+    EffectMetadata* metadata;  // the instance's row: read by a snapshot, written by a restore
+    const u32* ping;           // alive-list columns of the slab (row 0), read by a snapshot
+    const u32* pong;
+    PlaneSet planes;           // the slab's physical columns (row 0)
+    u32 num_planes;
+    u32 stride_words;          // the effect's record stride
+    u32 first, rows;           // the slice
+    u64 src_bytes;             // restore: bytes readable at the source (>= 64)
+};
+// header + records i < min(alive_count, rows) in alive-list order
+cudaError_t launch_snapshot_gather(const SnapshotArgs& a, u32* dst, cudaStream_t st);
+// records i < m to local rows i, and alive_count / max_spawn / particle_counter; enqueue launch_repack_lists after it
+cudaError_t launch_restore_scatter(const SnapshotArgs& a, const u32* src, cudaStream_t st);
+
 cudaError_t launch_indirect(const StaticTables& T, u32 num_effects, cudaStream_t st);
 cudaError_t launch_prefix_sum(const StaticTables& T, u32 num_batches, cudaStream_t st);
 cudaError_t launch_tile_prefix(const StaticTables& T, u32 batch_index, u32 tile, cudaStream_t st);

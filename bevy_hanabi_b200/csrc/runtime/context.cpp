@@ -1125,17 +1125,27 @@ int32_t hnb_slab_fill_c5_ex(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t cou
 // The scratch (rows x the widest column) is taken with cudaMallocAsync and given back with cudaFreeAsync on the context
 // stream: the call stays asynchronous (no synchronisation to grow or free a buffer the stream may still use), and a
 // context does not keep up to 2 GiB between repacks that may be seconds apart.
+namespace {
+// The checks every call that rewrites or reads one instance's slice through its lists makes (`what`: the call's name).
+void check_instance_slice(hnb_ctx* c, const Slab& s, const Effect& fx, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                          const char* what) {
+    const std::string w = what;
+    if (uint64_t(first) + rows > s.capacity) fail(HNB_ERR_INVALID_ARG, w + ": rows outside the slab");
+    if (metadata_row >= c->md_rows) fail(HNB_ERR_INVALID_ARG, w + ": metadata row out of range");
+    if (fx.particle_stride != s.stride) fail(HNB_ERR_INVALID_ARG, w + ": effect particle stride does not match the slab");
+    if (((fx.flags & HNB_EFFECT_SECTOR_PLANES) != 0) != s.sector_planes)
+        fail(HNB_ERR_INVALID_ARG, w + ": effect and slab disagree on HNB_EFFECT_SECTOR_PLANES / HNB_SLAB_SECTOR_PLANES");
+    if (fx.flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS)
+        fail(HNB_ERR_INVALID_ARG, w + ": pending GPU spawn events name parent slots; an emitting effect cannot be " +
+                                      (w == "hnb_slab_repack" ? "repacked" : "snapshot or restored"));
+}
+}  // namespace
+
 int32_t hnb_slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows) {
     return guarded([&] {
         Slab& s = get_slab(c, h);
         const Effect& fx = get_effect(c, e);
-        if (uint64_t(first) + rows > s.capacity) fail(HNB_ERR_INVALID_ARG, "hnb_slab_repack: rows outside the slab");
-        if (metadata_row >= c->md_rows) fail(HNB_ERR_INVALID_ARG, "hnb_slab_repack: metadata row out of range");
-        if (fx.particle_stride != s.stride) fail(HNB_ERR_INVALID_ARG, "hnb_slab_repack: effect particle stride does not match the slab");
-        if (((fx.flags & HNB_EFFECT_SECTOR_PLANES) != 0) != s.sector_planes)
-            fail(HNB_ERR_INVALID_ARG, "hnb_slab_repack: effect and slab disagree on HNB_EFFECT_SECTOR_PLANES / HNB_SLAB_SECTOR_PLANES");
-        if (fx.flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS)
-            fail(HNB_ERR_INVALID_ARG, "hnb_slab_repack: pending GPU spawn events name parent slots; an emitting effect cannot be repacked");
+        check_instance_slice(c, s, fx, metadata_row, first, rows, "hnb_slab_repack");
         if (rows == 0) return;
         CUDA_CHECK(cudaSetDevice(c->device));
         hnb::RepackArgs a{};
@@ -1165,6 +1175,76 @@ int32_t hnb_slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_
         const cudaError_t freed = cudaFreeAsync(scratch, c->stream);
         CUDA_CHECK(err);
         CUDA_CHECK(freed);
+    });
+}
+
+static_assert(HNB_SNAPSHOT_MAGIC == HNB_SNAPSHOT_MAGIC_WORD && HNB_SNAPSHOT_VERSION == HNB_SNAPSHOT_VERSION_WORD &&
+                  sizeof(hnb_instance_snapshot_header) == HNB_SNAPSHOT_HEADER_WORDS * 4,
+              "snapshot header of include/hanabi_b200.h and of the kernels");
+
+size_t hnb_instance_snapshot_bytes(uint32_t particle_stride, uint32_t rows) {
+    return sizeof(hnb_instance_snapshot_header) + size_t(rows) * particle_stride;
+}
+
+namespace {
+hnb::SnapshotArgs snapshot_args(hnb_ctx* c, const Slab& s, uint32_t metadata_row, uint32_t first, uint32_t rows) {
+    hnb::SnapshotArgs a{};
+    a.metadata = c->d_metadata + metadata_row;
+    a.ping = s.ping;
+    a.pong = s.pong;
+    a.planes = plane_set(s);
+    a.num_planes = (uint32_t)s.planes.size();
+    a.stride_words = s.stride / 4;
+    a.first = first;
+    a.rows = rows;
+    return a;
+}
+}  // namespace
+
+// One launch: the kernel reads n, W and particle_counter on the device, so the host never waits for them.
+int32_t hnb_instance_snapshot(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                              void* d_dst, size_t dst_bytes) {
+    return guarded([&] {
+        Slab& s = get_slab(c, h);
+        const Effect& fx = get_effect(c, e);
+        check_instance_slice(c, s, fx, metadata_row, first, rows, "hnb_instance_snapshot");
+        if (!d_dst || ((uintptr_t)d_dst & 15u)) fail(HNB_ERR_INVALID_ARG, "hnb_instance_snapshot: d_dst is NULL or not 16-byte aligned");
+        if (dst_bytes < hnb_instance_snapshot_bytes(s.stride, rows))
+            fail(HNB_ERR_INVALID_ARG, "hnb_instance_snapshot: dst_bytes is below hnb_instance_snapshot_bytes(stride, rows)");
+        if (rows == 0) return;
+        CUDA_CHECK(cudaSetDevice(c->device));
+        CUDA_CHECK(hnb::launch_snapshot_gather(snapshot_args(c, s, metadata_row, first, rows), (uint32_t*)d_dst, c->stream));
+        c->launches++;
+    });
+}
+
+// Two launches: the records and the metadata words, then hnb_slab_repack's list writer, which reads m back from
+// alive_count.
+int32_t hnb_instance_restore(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                             const void* d_src, size_t src_bytes) {
+    return guarded([&] {
+        Slab& s = get_slab(c, h);
+        const Effect& fx = get_effect(c, e);
+        check_instance_slice(c, s, fx, metadata_row, first, rows, "hnb_instance_restore");
+        if (!d_src || ((uintptr_t)d_src & 15u)) fail(HNB_ERR_INVALID_ARG, "hnb_instance_restore: d_src is NULL or not 16-byte aligned");
+        if (src_bytes < sizeof(hnb_instance_snapshot_header)) fail(HNB_ERR_INVALID_ARG, "hnb_instance_restore: src_bytes is below the 64-byte header");
+        if (rows == 0) return;
+        CUDA_CHECK(cudaSetDevice(c->device));
+        hnb::SnapshotArgs a = snapshot_args(c, s, metadata_row, first, rows);
+        a.src_bytes = src_bytes;
+        CUDA_CHECK(hnb::launch_restore_scatter(a, (const uint32_t*)d_src, c->stream));
+        c->launches++;
+        hnb::RepackArgs r{};
+        r.metadata = a.metadata;
+        r.ping = s.ping;
+        r.pong = s.pong;
+        r.dead = s.dead;
+        r.alive_bits = s.alive_bits;
+        r.claim = s.ident_claim;
+        r.first = first;
+        r.rows = rows;
+        CUDA_CHECK(hnb::launch_repack_lists(r, c->stream));
+        c->launches++;
     });
 }
 

@@ -286,6 +286,25 @@ class Context:
         again (hnb_slab_repack). Call between frames; only enqueues work on the context stream."""
         check(lib.hnb_slab_repack(self._h, slab, effect, metadata_row, first, rows))
 
+    @staticmethod
+    def instance_snapshot_bytes(particle_stride: int, rows: int) -> int:
+        """Bytes a snapshot of a `rows`-row instance may need: the 64-byte header and `rows` records."""
+        return lib.hnb_instance_snapshot_bytes(particle_stride, rows)
+
+    def instance_snapshot(self, slab: int, effect: int, metadata_row: int, first: int, rows: int, d_dst: int,
+                          dst_bytes: int) -> None:
+        """Write the header and the live records, in alive-list order, of the instance at slab rows [first, first+rows) to
+        the device buffer `d_dst` (16-byte aligned, at least instance_snapshot_bytes(stride, rows) bytes; a
+        hnb_device_alloc pointer or a torch tensor's data_ptr()). The instance is not modified; only enqueues work."""
+        check(lib.hnb_instance_snapshot(self._h, slab, effect, metadata_row, first, rows, d_dst, dst_bytes))
+
+    def instance_restore(self, slab: int, effect: int, metadata_row: int, first: int, rows: int, d_src: int,
+                         src_bytes: int) -> None:
+        """Put the particles of a snapshot at the front of the instance at slab rows [first, first+rows) (any slice, slab
+        or context whose effect has the snapshot's stride); its lists, claims and alive bits become what slab_repack
+        leaves. `src_bytes`: bytes readable at `d_src` (>= 64). Only enqueues work."""
+        check(lib.hnb_instance_restore(self._h, slab, effect, metadata_row, first, rows, d_src, src_bytes))
+
     def slab_checksum(self, slab: int, first: int, count: int, index_base: int = 0) -> int:
         out = C.c_uint64(0)
         check(lib.hnb_slab_checksum_ex(self._h, slab, first, count, index_base, C.byref(out)))

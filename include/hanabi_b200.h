@@ -247,6 +247,60 @@ HNB_API int32_t hnb_slab_fill_c5_ex(hnb_ctx* ctx, hnb_slab slab, uint32_t first,
  */
 HNB_API int32_t hnb_slab_repack(hnb_ctx* ctx, hnb_slab slab, hnb_effect effect, uint32_t metadata_row, uint32_t first,
                                 uint32_t rows);
+
+/**
+ * Snapshots of one instance's live particles, in a device buffer the caller owns: a 64-byte header written on the device,
+ * then `count` reference AoS `Particle` records (the effect's particle_stride bytes each) in alive-list order. The first
+ * 64 + count * particle_stride bytes are a complete snapshot: a host may read the header, then copy just that prefix.
+ * A snapshot carries records and particle_counter only: properties, spawners, clocks and pending GPU spawn events are
+ * the host's to carry.
+ */
+#define HNB_SNAPSHOT_MAGIC 0x53424E48u /* "HNBS" in little-endian byte order */
+#define HNB_SNAPSHOT_VERSION 1u
+typedef struct hnb_instance_snapshot_header {
+    uint32_t magic;            /* HNB_SNAPSHOT_MAGIC */
+    uint32_t version;          /* HNB_SNAPSHOT_VERSION */
+    uint32_t particle_stride;  /* bytes per record = the effect's reference AoS stride */
+    uint32_t count;            /* n: records that follow, in alive-list order */
+    uint32_t particle_counter; /* the metadata row's particle_counter */
+    uint32_t rows;             /* the source slice's rows (informational) */
+    uint32_t reserved[10];     /* zero */
+} hnb_instance_snapshot_header;
+
+/** Bytes a snapshot of a `rows`-row slice may need: 64 + rows * particle_stride. */
+HNB_API size_t hnb_instance_snapshot_bytes(uint32_t particle_stride, uint32_t rows);
+/**
+ * Snapshot the instance at slab rows [first, first+rows) (`rows` = its capacity), metadata row `metadata_row`, running
+ * `effect`, into `d_dst` (`dst_bytes` >= hnb_instance_snapshot_bytes(stride, rows)). With n = min(alive_count, rows),
+ * W = indirect_write_index and particle_counter read from the DEVICE metadata row, record i < n is the record of local
+ * row list_W[first+i] (clamped to the slice, as hnb_slab_repack does); bytes past 64 + n * stride are not written. The
+ * instance is not modified. Call between hnb_simulate calls; work is only enqueued on the context stream.
+ */
+HNB_API int32_t hnb_instance_snapshot(hnb_ctx* ctx, hnb_slab slab, hnb_effect effect, uint32_t metadata_row, uint32_t first,
+                                      uint32_t rows, void* d_dst, size_t dst_bytes);
+/**
+ * Restore a snapshot into the instance at slab rows [first, first+rows) (`rows` = its capacity; any slice, slab or
+ * context whose effect has the snapshot's stride). `d_src` is read on this context's device (any allocation that device
+ * can read); `src_bytes` >= 64 is how many bytes it holds. On the device, m = min(count, rows, (src_bytes - 64) / stride),
+ * or 0 when magic, version or particle_stride do not match the effect (a corrupt snapshot restores an empty instance and
+ * is never read out of bounds). Then:
+ *   - record i < m goes to slab row first+i of every plane; rows >= m of the planes are left as they are;
+ *   - the metadata row gets alive_count = m, max_spawn = capacity - m (its own capacity word; 0 if that is below m) and,
+ *     for an accepted header, particle_counter = header.particle_counter; no other metadata word or draw argument
+ *     changes (the next frame's indirect pass rewrites instance_count);
+ *   - the lists, dead stack, both identity claims {first, m} and the alive bits are what hnb_slab_repack writes for n = m.
+ * So restore(snapshot(X)) into X's own slice leaves the lists, claims, bits, metadata and live records that
+ * hnb_slab_repack(X) leaves; into another slice, slab or context, the same state shifted to the new `first`. With
+ * rows < n the first `rows` particles in alive-list order are kept, as the reference drops spawns beyond capacity.
+ *
+ * Both calls return HNB_ERR_INVALID_ARG, with nothing enqueued, when the rows lie outside the slab, the metadata row is
+ * out of range, the effect's stride or HNB_EFFECT_SECTOR_PLANES flag does not match the slab, the effect has
+ * HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS, the buffer is NULL or not 16-byte aligned, dst_bytes is below
+ * hnb_instance_snapshot_bytes(stride, rows), or src_bytes is below 64. rows == 0 is a no-op. Neither call synchronises
+ * or allocates.
+ */
+HNB_API int32_t hnb_instance_restore(hnb_ctx* ctx, hnb_slab slab, hnb_effect effect, uint32_t metadata_row, uint32_t first,
+                                     uint32_t rows, const void* d_src, size_t src_bytes);
 /** 64-bit FNV-style checksum of the AoS bytes of rows [first,first+count), computed on device
  *  (order-independent sum of per-row hashes), for whole-slab comparisons at sizes the host
  *  cannot download cheaply. */

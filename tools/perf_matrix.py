@@ -400,6 +400,63 @@ def churn_repack():
     ctx.close()
 
 
+def _events_ms(fn, reps=5):
+    """Best of `reps` CUDA-event windows around fn() on the scenario's stream, in ms."""
+    best = float("inf")
+    for _ in range(reps):
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        fn()
+        e1.record(stream)
+        e1.synchronize()
+        best = min(best, e0.elapsed_time(e1))
+    return best
+
+
+def _snapshot_pair(label, ctx, slab, effect, rows, stride, alive):
+    """Time hnb_instance_snapshot of metadata row 0 and hnb_instance_restore of it into a second slab (metadata row 1).
+    Bytes: a snapshot reads 4 B of list and S B of record and writes S B per live particle; a restore reads and writes
+    S B, then writes 8 B of lists per particle, 4 B of dead stack per free slot and the alive bitmap."""
+    nbytes = ctx.instance_snapshot_bytes(stride, rows)
+    buf = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
+    dst = ctx.slab_create(rows, stride, sector_planes=False)
+    ctx.metadata_insert(1, R.initial_metadata(rows, 1, stride // 4))
+    snap = _events_ms(lambda: ctx.instance_snapshot(slab, effect, 0, 0, rows, buf.data_ptr(), nbytes))
+    rest = _events_ms(lambda: ctx.instance_restore(dst, effect, 1, 0, rows, buf.data_ptr(), nbytes))
+    assert ctx.read_metadata(1).alive_count == alive
+    report(f"snapshot_restore: {label} snapshot", snap, (4 + 2 * stride) * alive, f"{alive >> 10} Ki alive, best of 5")
+    report(f"snapshot_restore: {label} restore", rest, (8 + 2 * stride) * alive + 4 * (rows - alive) + rows // 8, "into another slab, best of 5")
+    del buf
+    ctx.slab_destroy(dst)
+
+
+def snapshot_restore():
+    """hnb_instance_snapshot / hnb_instance_restore: a filled 64 Mi C5 instance (identity list), the 16 Mi-slot churn steady
+    state (gathers through a permuted list), and a 2 GiB device-to-device torch copy for scale."""
+    _card()
+    a = torch.empty(2 << 30, dtype=torch.uint8, device="cuda")
+    b = torch.empty_like(a)
+    ms = _events_ms(lambda: b.copy_(a))
+    report("snapshot_restore: 2 GiB device-to-device copy", ms, 2 * a.numel(), "torch copy_, best of 5")
+    del a, b
+    torch.cuda.empty_cache()
+
+    P = 64 << 20
+    ctx = hb.Context(0, stream.cuda_stream)
+    slab = ctx.slab_create(P, 32)
+    ctx.slab_fill_c5(slab, 0, P, 42, 1e9, 1e9)
+    single_instance(ctx, P, 32, alive=P)
+    effect = ctx.effect_compile(recipes.c5_lowered())
+    _snapshot_pair(f"filled C5 {P >> 20} Mi", ctx, slab, effect, P, 32, P)
+    ctx.close()
+    torch.cuda.empty_cache()
+
+    P, ctx, slab, effect, stride, dt, rate = _churned()
+    _snapshot_pair(f"churned {P >> 20} Mi slots", ctx, slab, effect, P, stride, ctx.read_metadata(0).alive_count)
+    ctx.close()
+
+
 def fresh_sector():
     """Cost of sector planes when access IS coalesced: C5 recipe burst + update, like `c5_init`, on a sector slab."""
     w = G.ExprWriter()
@@ -590,7 +647,7 @@ def c3_chain():
         ctx.close()
 
 
-SCENARIOS = {"c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
+SCENARIOS = {"c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
 if __name__ == "__main__":
     for name in (sys.argv[1:] or list(SCENARIOS)):
         try:
