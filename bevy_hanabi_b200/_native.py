@@ -221,6 +221,7 @@ SIGNATURES = {
     "hnb_read_draw_args_async": (i32, [vp, u32, u32, vp]),
     "hnb_ctx_set_count_mailbox": (i32, [vp, vp, u32, u32]),
     "hnb_ctx_last_epoch": (i32, [vp, P(u32)]),
+    "hnb_ctx_tile_state_clears": (i32, [vp, P(C.c_uint64)]),
     "hnb_host_alloc": (vp, [C.c_size_t]),
     "hnb_host_free": (None, [vp]),
     "hnb_ctx_read_debug": (i32, [vp, P(C.c_uint64), i32]),

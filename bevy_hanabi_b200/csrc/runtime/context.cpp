@@ -25,6 +25,7 @@
 #include "effect_source.h"
 #include "hanabi_b200.h"
 #include "nvrtc_compile.h"
+#include "tile_state_rule.h"
 
 using namespace hnb_rt;
 
@@ -181,7 +182,8 @@ struct hnb_ctx {
     uint32_t *d_tile_prefix = nullptr, *d_dispatch_args = nullptr, *d_batch_tiles = nullptr, *d_tickets = nullptr;
     std::vector<unsigned long long*> d_tile_state;  // per batch
     std::vector<uint32_t> tile_state_cap;
-    std::vector<uint64_t> tile_state_sig;  // what the batch's states were last written for (see plan_batch, slot order)
+    std::vector<hnb_rt::TileStateSlot> tile_state_slot;  // when the batch's states were last zeroed (tile_state_rule.h)
+    uint64_t tile_state_clears = 0;  // zeroings tile_state_needs_clear asked for (hnb_ctx_tile_state_clears)
     uint64_t md_generation = 1;            // bumped by hnb_metadata_insert
 
     std::vector<Slab> slabs;
@@ -314,7 +316,7 @@ void ensure_scratch(hnb_ctx* c) {
         c->scratch_B = cap;
         c->d_tile_state.resize(cap, nullptr);
         c->tile_state_cap.resize(cap, 0);
-        c->tile_state_sig.resize(cap, 0);
+        c->tile_state_slot.resize(cap);
     }
 }
 
@@ -463,7 +465,7 @@ void ensure_tile_state(hnb_ctx* c, uint32_t batch, uint32_t tiles) {
     CUDA_CHECK(cudaMalloc((void**)&c->d_tile_state[batch], size_t(cap) * 8));
     CUDA_CHECK(cudaMemsetAsync(c->d_tile_state[batch], 0, size_t(cap) * 8, c->stream));
     c->tile_state_cap[batch] = cap;
-    c->tile_state_sig[batch] = 0;
+    c->tile_state_slot[batch] = hnb_rt::TileStateSlot{};
 }
 
 // Build the kernel parameters of one batch and write its per-instance init thread ranges and tile
@@ -519,6 +521,8 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
         const hnb_spawner* sp = c->h_at<hnb_spawner>(c->lay.off_spawners);
         for (uint32_t i = 0; i < bi.prefix_sum_count; ++i)
             if (sp[bi.spawner_base + i].slab_offset & 31u) fail(HNB_ERR_LAYOUT, "HNB_EFFECT_SLOT_ORDER needs every instance to start on a multiple of 32 slab rows");
+        // a slot-order state word packs each running count into 28 bits
+        if (lp.slab->capacity >= (1u << 28)) fail(HNB_ERR_LAYOUT, "HNB_EFFECT_SLOT_ORDER needs a slab of fewer than 2^28 rows");
     }
     if (c->h_at<uint32_t>(c->lay.off_tile_size)[lp.batch] != tile_word) {
         c->h_at<uint32_t>(c->lay.off_tile_size)[lp.batch] = tile_word;
@@ -557,9 +561,11 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
         }
     }
     ensure_tile_state(c, lp.batch, lp.slab->capacity / small_tile + bi.prefix_sum_count + 1);  // ceil(rows_i / tile) summed over the instances
-    if (slot_order || c->tile_state_sig[lp.batch]) {
-        // Slot-order state words carry only 6 bits of epoch: enough while every tile of the batch is rewritten every
-        // frame (its tile count depends on capacities only), not across a change of what the batch slot is used for.
+    {
+        // Slot-order state words carry only 6 bits of epoch: the array is zeroed when the slot's use changes (signature)
+        // and at least every 64 frames of the slot (tile_state_rule.h). The signature alone is not enough: a batch slot
+        // that sits out for 64 frames, or serves another instance of the same effect and slab with fewer tiles, leaves
+        // words whose tag matches a later frame's.
         uint64_t sig = 0;
         if (slot_order) {
             sig = 0xcbf29ce484222325ull;
@@ -567,9 +573,9 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
                 sig = (sig ^ v) * 0x100000001b3ull;
             sig |= 1;
         }
-        if (sig != c->tile_state_sig[lp.batch]) {
+        if (hnb_rt::tile_state_needs_clear(c->tile_state_slot[lp.batch], sig, hnb_rt::tile_state_run_epoch(c->epoch))) {
             CUDA_CHECK(cudaMemsetAsync(c->d_tile_state[lp.batch], 0, size_t(c->tile_state_cap[lp.batch]) * 8, c->stream));
-            c->tile_state_sig[lp.batch] = sig;
+            c->tile_state_clears++;
         }
     }
 
@@ -1870,6 +1876,12 @@ int32_t hnb_ctx_last_epoch(hnb_ctx* c, uint32_t* epoch) {
     return guarded([&] {
         if (!c || !epoch) fail(HNB_ERR_INVALID_ARG, "NULL argument");
         *epoch = c->epoch;
+    });
+}
+int32_t hnb_ctx_tile_state_clears(hnb_ctx* c, uint64_t* clears) {
+    return guarded([&] {
+        if (!c || !clears) fail(HNB_ERR_INVALID_ARG, "NULL argument");
+        *clears = c->tile_state_clears;
     });
 }
 

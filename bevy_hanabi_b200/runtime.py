@@ -442,6 +442,12 @@ class Context:
         check(lib.hnb_ctx_last_epoch(self._h, C.byref(e)))
         return e.value
 
+    def tile_state_clears(self) -> int:
+        """How often a batch's look-back tile states were zeroed before an update launch (hnb_ctx_tile_state_clears)."""
+        n = C.c_uint64(0)
+        check(lib.hnb_ctx_tile_state_clears(self._h, C.byref(n)))
+        return n.value
+
     def mailbox_count(self, epoch: int, row: int = 0, spin: bool = True):
         """instance_count the frame `epoch` published for draw-indirect row `row` (spins until the word has landed)."""
         import time

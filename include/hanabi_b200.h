@@ -543,6 +543,10 @@ HNB_API int32_t hnb_read_draw_args_async(hnb_ctx* ctx, uint32_t first, uint32_t 
 HNB_API int32_t hnb_ctx_set_count_mailbox(hnb_ctx* ctx, uint64_t* pinned_host, uint32_t rows, uint32_t ring);
 /** Epoch (frame number, 30 bits, never 0) of the frame the last hnb_simulate enqueued. */
 HNB_API int32_t hnb_ctx_last_epoch(hnb_ctx* ctx, uint32_t* epoch);
+/** Number of times the context zeroed a batch's look-back tile states before an update launch because the batch's use
+ *  changed (effect, slab, tile size or instance set of an HNB_EFFECT_SLOT_ORDER batch) or because an HNB_EFFECT_SLOT_ORDER
+ *  batch's states were 64 or more frames old (their words keep 6 bits of epoch). Batches of the other orders never add to it. */
+HNB_API int32_t hnb_ctx_tile_state_clears(hnb_ctx* ctx, uint64_t* clears);
 /** Pinned host memory helpers for the async paths. */
 HNB_API void* hnb_host_alloc(size_t bytes);
 HNB_API void hnb_host_free(void* p);

@@ -200,6 +200,17 @@ extern "C" void emu_planes_to_aos(const EmuBatch* b, uint8_t* aos, uint32_t firs
         memcpy(aos + size_t(r) * stride, (const void*)&raw, stride);
     }
 }
+// the look-back's tile state word as this effect's order packs it (`valid` is dropped outside slot order)
+extern "C" uint64_t emu_pack_state(uint32_t epoch, uint64_t flag, uint32_t survivors, uint32_t valid) {
+#if HNB_SLOT_ORDER
+    return hnb::hnb_pack_state(epoch, flag, survivors, valid);
+#else
+    (void)valid;
+    return hnb::hnb_pack_state(epoch, flag, survivors);
+#endif
+}
+extern "C" uint32_t emu_state_flag(uint64_t s, uint32_t epoch) { return hnb::hnb_state_flag(s, epoch); }
+extern "C" uint64_t emu_state_value(uint64_t s) { return hnb::hnb_state_value(s); }
 extern "C" uint32_t emu_tile_k(void) { return HNB_TILE_K; }
 extern "C" uint32_t emu_rows_per_lane(void) { return HNB_ROWS_PER_LANE; }
 extern "C" uint32_t emu_init_items(void) { return HNB_INIT_ITEMS; }
@@ -243,6 +254,12 @@ def build_emulated_effect(lowered, allow_events: bool = False) -> C.CDLL:
         getattr(lib, f).restype = None
     for f in ("emu_tile_k", "emu_rows_per_lane", "emu_init_items"):
         getattr(lib, f).restype = C.c_uint32
+    lib.emu_pack_state.argtypes = [C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32]
+    lib.emu_pack_state.restype = C.c_uint64
+    lib.emu_state_flag.argtypes = [C.c_uint64, C.c_uint32]
+    lib.emu_state_flag.restype = C.c_uint32
+    lib.emu_state_value.argtypes = [C.c_uint64]
+    lib.emu_state_value.restype = C.c_uint64
     return lib
 
 
