@@ -46,10 +46,6 @@ namespace hnb {
 #if HNB_SLOT_ORDER && HNB_ROWS_PER_LANE > 32
 #error "slot order gives each lane one alive-bitmap word of a tile: HNB_ROWS_PER_LANE must be at most 32"
 #endif
-#ifndef HNB_LOOKBACK_GROUPS
-#define HNB_LOOKBACK_GROUPS 1  // predecessors examined per look-back round trip = 32 * groups (with deferred
-                               // compaction the first window almost always holds a PREFIX: 1 beat 4 by 2.7 %)
-#endif
 #ifndef HNB_SMEM_EFFECTS
 #define HNB_SMEM_EFFECTS 2047  // tile_prefix entries staged in shared memory (8 KB with the end sentinel)
 #endif
@@ -57,21 +53,9 @@ namespace hnb {
 #ifndef HNB_MIN_BLOCKS
 #define HNB_MIN_BLOCKS 3  // H100, C5 at 64 / 8 Mi: 4 CTAs (64 registers) 6 % slower, 2 CTAs within 1 %
 #endif
-#ifndef HNB_DEFER_COMPACTION
-#define HNB_DEFER_COMPACTION (!HNB_RELAXED_ORDER)  // park a tile's compaction behind the warp's next pass 1
-#endif
 #ifndef HNB_PROFILE
 #define HNB_PROFILE 0  // 1: accumulate per-phase cycle counters into BatchParams::debug (diagnostics)
 #endif
-#ifndef HNB_LOOKBACK_SLEEP_NS
-#define HNB_LOOKBACK_SLEEP_NS 0  // back-off between polls of an unpublished predecessor (0 = spin)
-#endif
-
-#ifndef HNB_PARK
-#define HNB_PARK 1  // tiles a warp keeps parked (simulated, compaction still to do) behind the one it streams; the stash has HNB_PARK + 1
-                    // buffers per warp (host mirror: hnb_rt::park_depth, update_smem_bytes)
-#endif
-#define HNB_STASH_BUFFERS (HNB_PARK + 1)
 #ifndef HNB_SLOT_ORDER
 #define HNB_SLOT_ORDER 0  // 1 (HNB_EFFECT_SLOT_ORDER): the update pass walks the instance's SLOTS in ascending order, guided by
                           // the slab's alive bitmap, instead of walking the alive list. See "slot order" below.
@@ -308,14 +292,15 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK) hnb_init(const BatchPara
 // A tile whose rows have been simulated (pass 1) and whose compaction is still to be done. Lives in
 // shared memory (one per warp) so that it costs no registers while the next tile is being streamed.
 struct PendingTile {
-    u32 valid, tile, row0, tile_alive;
+    u32 tile, row0, tile_alive;
     u32 base_particle, max_update, write_index, render_index;
     u32 inst_first_tile, inst_end_tile, metadata_index, buffer;
     u32 tile_valid;  // slot order: rows of the tile that were alive before the pass
     // identity claims as read when the instance was bound (a parked tile may be compacted after the instance's last tile has
     // rewritten the claim): read-column rows known to be the identity, length of the write column's claim for this instance
-    u32 trust_r, claim_w, _pad;
-};  // 64 bytes (mirrored by update_smem_bytes on the host)
+    u32 trust_r, claim_w, _pad[2];
+};
+static_assert(sizeof(PendingTile) == 64, "update_smem_bytes on the host reserves 64 bytes per warp for the parked tile");
 
 // Compaction of one tile: exclusive prefix of survivors over the previous tiles of the instance
 // (decoupled look-back), then survivors -> write list, dead -> dead stack (vfx_update.wgsl:148-166).
@@ -341,57 +326,40 @@ HNB_DI void hnb_compact_tile(const BatchParams& P, const PendingTile& pt, const 
     alive_before = __shfl_sync(0xffffffffu, alive_before, 0);
 #else
     if (tile != inst_first_tile) {
-        // Walk back over the predecessors' states, HNB_LOOKBACK_GROUPS x 32 of them per round trip (lane l
-        // of group g examines tile pos - 32g - l), summing AGGREGATEs until the first PREFIX. Tiles before
-        // the instance's first tile count as a PREFIX of 0.
+        // Walk back over the predecessors' states, 32 of them per round trip (lane l examines tile pos - l), summing
+        // AGGREGATEs until the first PREFIX. Tiles before the instance's first tile count as a PREFIX of 0. With deferred
+        // compaction the first window almost always holds a PREFIX (128 predecessors per round trip measured 2.7 % slower).
         u32 pos = tile - 1u;  // newest predecessor not yet accounted for
         for (;;) {
-            u64 s[HNB_LOOKBACK_GROUPS];
-#pragma unroll
-            for (int g = 0; g < HNB_LOOKBACK_GROUPS; ++g) {
-                const u32 back = 32u * g + lane;
 #if HNB_SLOT_ORDER
-                s[g] = (pos >= inst_first_tile + back) ? hnb_ld_state(&states[pos - back]) : hnb_pack_state(epoch, HNB_FLAG_PREFIX, 0u, 0u);
+            const u64 s = (pos >= inst_first_tile + lane) ? hnb_ld_state(&states[pos - lane]) : hnb_pack_state(epoch, HNB_FLAG_PREFIX, 0u, 0u);
 #else
-                s[g] = (pos >= inst_first_tile + back) ? hnb_ld_state(&states[pos - back]) : hnb_pack_state(epoch, HNB_FLAG_PREFIX, 0u);
+            const u64 s = (pos >= inst_first_tile + lane) ? hnb_ld_state(&states[pos - lane]) : hnb_pack_state(epoch, HNB_FLAG_PREFIX, 0u);
 #endif
-            }
-            bool done = false, stalled = false;
-#pragma unroll
-            for (int g = 0; g < HNB_LOOKBACK_GROUPS; ++g) {
-                if (!done && !stalled) {
-                    const u32 flag = hnb_state_flag(s[g], epoch);
-                    const u32 ready_mask = __ballot_sync(0xffffffffu, flag != 0u);
-                    const u32 prefix_mask = __ballot_sync(0xffffffffu, flag == u32(HNB_FLAG_PREFIX));
-                    const u32 first_p = prefix_mask ? (u32)(__ffs(prefix_mask) - 1) : 32u;
-                    const u32 need = first_p >= 31u ? 0xffffffffu : ((2u << first_p) - 1u);
-                    if ((ready_mask & need) != need) {
-                        stalled = true;  // a needed predecessor has not published yet: poll again from here
-                    } else {
-#if HNB_SLOT_ORDER
-                        u64 contrib = lane <= first_p ? hnb_state_value(s[g]) : 0ull;
-#pragma unroll
-                        for (int d = 16; d > 0; d >>= 1) contrib += __shfl_xor_sync(0xffffffffu, contrib, d);
-                        sum_before += contrib;
-#else
-                        u32 contrib = lane <= first_p ? u32(s[g]) : 0u;
-#pragma unroll
-                        for (int d = 16; d > 0; d >>= 1) contrib += __shfl_xor_sync(0xffffffffu, contrib, d);
-                        alive_before += contrib;
-#endif
-                        if (prefix_mask) done = true; else pos -= 32u;
-                    }
-                }
-            }
-            if (done) break;
-            if (stalled) {
+            const u32 flag = hnb_state_flag(s, epoch);
+            const u32 ready_mask = __ballot_sync(0xffffffffu, flag != 0u);
+            const u32 prefix_mask = __ballot_sync(0xffffffffu, flag == u32(HNB_FLAG_PREFIX));
+            const u32 first_p = prefix_mask ? (u32)(__ffs(prefix_mask) - 1) : 32u;
+            const u32 need = first_p >= 31u ? 0xffffffffu : ((2u << first_p) - 1u);
+            if ((ready_mask & need) != need) {  // a needed predecessor has not published yet: poll again from here
 #if HNB_PROFILE
                 prof_polls++;
 #endif
-#if HNB_LOOKBACK_SLEEP_NS > 0
-                __nanosleep(HNB_LOOKBACK_SLEEP_NS);
-#endif
+                continue;
             }
+#if HNB_SLOT_ORDER
+            u64 contrib = lane <= first_p ? hnb_state_value(s) : 0ull;
+#pragma unroll
+            for (int d = 16; d > 0; d >>= 1) contrib += __shfl_xor_sync(0xffffffffu, contrib, d);
+            sum_before += contrib;
+#else
+            u32 contrib = lane <= first_p ? u32(s) : 0u;
+#pragma unroll
+            for (int d = 16; d > 0; d >>= 1) contrib += __shfl_xor_sync(0xffffffffu, contrib, d);
+            alive_before += contrib;
+#endif
+            if (prefix_mask) break;
+            pos -= 32u;
         }
 #if HNB_SLOT_ORDER
         alive_before = u32(sum_before >> 28) & 0x0fffffffu;
@@ -486,19 +454,19 @@ HNB_DI void hnb_compact_tile(const BatchParams& P, const PendingTile& pt, const 
 
 extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_update(const BatchParams P) {
     // Dynamic shared memory (size = hnb_update_smem_bytes, computed identically on the host):
-    //   tile-prefix table | per warp, HNB_PARK + 1 buffers: alive-list entries [B][R][32], survivor ballots [B][R], valid masks [B][R] |
-    //   per warp: HNB_PARK PendingTile records | per warp: Properties staging slot
+    //   tile-prefix table | per warp, 2 buffers (streamed tile, parked tile): alive-list entries [2][R][32], survivor ballots
+    //   [2][R], valid masks [2][R] | per warp: one PendingTile record | per warp: Properties staging slot
     u32* const sh_tile_prefix = (u32*)hnb_smem;
     typedef u32 PidxBuf[HNB_ROWS_PER_LANE][32];
     typedef u32 SurvBuf[HNB_ROWS_PER_LANE];
-    enum : size_t { kStash = (sizeof(PidxBuf) + 2 * sizeof(SurvBuf)) * HNB_STASH_BUFFERS * HNB_WARPS };
-    PidxBuf(*const sh_pidx)[HNB_STASH_BUFFERS] = (PidxBuf(*)[HNB_STASH_BUFFERS])(hnb_smem + HNB_SMEM_PREFIX_BYTES);
-    SurvBuf(*const sh_survivors)[HNB_STASH_BUFFERS] = (SurvBuf(*)[HNB_STASH_BUFFERS])(hnb_smem + HNB_SMEM_PREFIX_BYTES + sizeof(PidxBuf) * HNB_STASH_BUFFERS * HNB_WARPS);
-    SurvBuf(*const sh_valids)[HNB_STASH_BUFFERS] = (SurvBuf(*)[HNB_STASH_BUFFERS])(hnb_smem + HNB_SMEM_PREFIX_BYTES + (sizeof(PidxBuf) + sizeof(SurvBuf)) * HNB_STASH_BUFFERS * HNB_WARPS);  // slot order
-    PendingTile(*const sh_pending)[HNB_PARK] = (PendingTile(*)[HNB_PARK])(hnb_smem + HNB_SMEM_PREFIX_BYTES + kStash);
+    enum : size_t { kStash = (sizeof(PidxBuf) + 2 * sizeof(SurvBuf)) * 2 * HNB_WARPS };
+    PidxBuf(*const sh_pidx)[2] = (PidxBuf(*)[2])(hnb_smem + HNB_SMEM_PREFIX_BYTES);
+    SurvBuf(*const sh_survivors)[2] = (SurvBuf(*)[2])(hnb_smem + HNB_SMEM_PREFIX_BYTES + sizeof(PidxBuf) * 2 * HNB_WARPS);
+    SurvBuf(*const sh_valids)[2] = (SurvBuf(*)[2])(hnb_smem + HNB_SMEM_PREFIX_BYTES + (sizeof(PidxBuf) + sizeof(SurvBuf)) * 2 * HNB_WARPS);  // slot order
+    PendingTile* const sh_pending = (PendingTile*)(hnb_smem + HNB_SMEM_PREFIX_BYTES + kStash);
 #if HNB_HAS_PROPERTIES
     typedef unsigned char PropsBuf[(sizeof(Properties) + 15) / 16 * 16];
-    PropsBuf* const sh_props = (PropsBuf*)(hnb_smem + HNB_SMEM_PREFIX_BYTES + kStash + sizeof(PendingTile) * HNB_PARK * HNB_WARPS);
+    PropsBuf* const sh_props = (PropsBuf*)(hnb_smem + HNB_SMEM_PREFIX_BYTES + kStash + sizeof(PendingTile) * HNB_WARPS);
 #endif
     const u32 tid = threadIdx.x;
     const u32 lane = tid & 31u;
@@ -543,9 +511,11 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
     // host (and used by the bookkeeping kernel for the tile prefix), so it is a run-time value here
     const u32 tile_rows = hnb_tile_rows(P.tile_rows);
     const u32 chunks = tile_rows / (32u * HNB_TILE_K);
-    PendingTile* const parked = sh_pending[warp];  // FIFO of this warp's parked tiles: q_len records starting at q_head
-    u32 q_head = 0u, q_len = 0u;
-    u32 cur = 0u;  // buffer the tile being streamed uses
+    PendingTile* const parked = &sh_pending[warp];  // this warp's parked tile
+    // Tiles this warp has streamed so far (ordered builds): the next one uses stash buffer streamed & 1, the parked tile, if
+    // any (streamed != 0), the other one. One counter rather than a buffer index and a has-parked flag: the extra live
+    // register made the slot-order and force-field builds of hnb_update spill.
+    u32 streamed = 0u;
 
     // cached descriptor of the instance the current tile belongs to (reloaded when a tile leaves
     // [inst_first_tile, inst_end_tile))
@@ -663,8 +633,8 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
             bind_instance(effect_index, false, 0u);
         }
         const u32 row0 = (tile - inst_first_tile) * tile_rows;
-        u32* const survivors = sh_survivors[warp][cur];
-        u32(*const pidx_stash)[32] = sh_pidx[warp][cur];
+        u32* const survivors = sh_survivors[warp][streamed & 1u];
+        u32(*const pidx_stash)[32] = sh_pidx[warp][streamed & 1u];
 
         // ---- pass 1: stream the tile's rows in `chunks` sub-tiles of 32*K rows:
         //      alive-list entry -> particle record -> simulate -> write back; remember who survived.
@@ -675,7 +645,7 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
         // bitmap belongs to this warp alone: lane jk loads it now and stores the survivors' ballot back after the pass —
         // 4 bytes per 32 slots instead of 4 bytes per particle of alive-list reads, and every record access of a warp
         // falls into one contiguous span of each plane, however the population was recycled.
-        u32* const valids = sh_valids[warp][cur];
+        u32* const valids = sh_valids[warp][streamed & 1u];
         u32* const tile_bits = P.slab.alive_bits + ((base_particle + row0) >> 5u);
         const bool owns_word = lane < chunks * HNB_TILE_K && row0 + lane * 32u < inst_capacity;
         u32 my_bits = owns_word ? tile_bits[lane] : 0u;
@@ -789,6 +759,9 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
         if (prof_first) { HNB_PROF_TIME(10, false) HNB_PROF_TIME(12, true) prof_first = false; }
 #endif
 
+#if !HNB_RELAXED_ORDER
+        ++streamed;  // this tile is parked below; if it is not the warp's first, the previous one is resolved first
+#endif
         // Request the next tile now; the atomic's round trip hides behind the compaction below.
         u32 next_tile = 0u;
         if (lane == 0) next_tile = atomicAdd(P.ticket, 1u);
@@ -797,38 +770,32 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
         // to finish its pass 1 (they started at about the same time, and pass-1 durations vary). Instead the
         // tile is parked and the PREVIOUS tile of this warp is resolved: its predecessors published their
         // aggregates a whole pass 1 ago, so the look-back finds them immediately.
-#if HNB_DEFER_COMPACTION
+#if !HNB_RELAXED_ORDER
         __syncwarp();
-        if (q_len == u32(HNB_PARK)) {  // the queue is full: resolve the oldest parked tile (its stash buffer is the next one to be reused)
-            const PendingTile pt = parked[q_head];
+        if (streamed != 1u) {  // resolve the parked tile: its stash buffer is the one the next tile will reuse
+            const PendingTile pt = *parked;
             hnb_compact_tile(P, pt, sh_survivors[warp][pt.buffer], sh_valids[warp][pt.buffer], sh_pidx[warp][pt.buffer], chunks, epoch, lane, prof_polls);
-            q_head = (q_head + 1u) % u32(HNB_PARK);
-            q_len -= 1u;
         }
         __syncwarp();
         if (lane == 0) {
-            PendingTile& pending = parked[(q_head + q_len) % u32(HNB_PARK)];
-            pending.valid = 1u; pending.tile = tile; pending.row0 = row0; pending.tile_alive = tile_alive;
-            pending.base_particle = base_particle; pending.max_update = max_update; pending.write_index = write_index;
-            pending.render_index = render_index; pending.inst_first_tile = inst_first_tile; pending.inst_end_tile = inst_end_tile;
-            pending.metadata_index = metadata_index;
-            pending.buffer = cur;
-            pending.trust_r = trust_r; pending.claim_w = claim_w;
+            parked->tile = tile; parked->row0 = row0; parked->tile_alive = tile_alive;
+            parked->base_particle = base_particle; parked->max_update = max_update; parked->write_index = write_index;
+            parked->render_index = render_index; parked->inst_first_tile = inst_first_tile; parked->inst_end_tile = inst_end_tile;
+            parked->metadata_index = metadata_index;
+            parked->buffer = ~streamed & 1u;
+            parked->trust_r = trust_r; parked->claim_w = claim_w;
 #if HNB_SLOT_ORDER
-            pending.tile_valid = tile_valid;
+            parked->tile_valid = tile_valid;
 #endif
         }
-        q_len += 1u;
-        cur = (cur + 1u) % u32(HNB_STASH_BUFFERS);
         __syncwarp();
 #else
         {
             __syncwarp();
             PendingTile pt;
-            pt.valid = 1u; pt.tile = tile; pt.row0 = row0; pt.tile_alive = tile_alive; pt.base_particle = base_particle;
+            pt.tile = tile; pt.row0 = row0; pt.tile_alive = tile_alive; pt.base_particle = base_particle;
             pt.max_update = max_update; pt.write_index = write_index; pt.render_index = render_index;
             pt.inst_first_tile = inst_first_tile; pt.inst_end_tile = inst_end_tile; pt.metadata_index = metadata_index;
-            pt.buffer = cur;
             pt.trust_r = trust_r; pt.claim_w = claim_w;
 #if HNB_SLOT_ORDER
             pt.tile_valid = tile_valid;
@@ -845,12 +812,11 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
         prof_tiles++;
 #endif
     }
-#if HNB_DEFER_COMPACTION
+#if !HNB_RELAXED_ORDER
     __syncwarp();
-    for (; q_len != 0u; --q_len) {  // no more tiles: resolve what is parked, oldest first
-        const PendingTile pt = parked[q_head];
+    if (streamed != 0u) {  // no more tiles: resolve the parked one
+        const PendingTile pt = *parked;
         hnb_compact_tile(P, pt, sh_survivors[warp][pt.buffer], sh_valids[warp][pt.buffer], sh_pidx[warp][pt.buffer], chunks, epoch, lane, prof_polls);
-        q_head = (q_head + 1u) % u32(HNB_PARK);
     }
 #endif
 #if HNB_PROFILE

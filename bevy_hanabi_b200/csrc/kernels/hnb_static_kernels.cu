@@ -782,7 +782,7 @@ __global__ void __launch_bounds__(BK_THREADS) k_frame_block(u32* arena, const __
     for (u32 i = threadIdx.x; i < block_words; i += BK_THREADS) arena[i] = block.w[i];
 }
 template <int NW>
-static cudaError_t launch_frame_block_t(u32* arena, const u32* src, u32 words, bool pdl, cudaStream_t st) {
+static cudaError_t launch_frame_block_t(u32* arena, const u32* src, u32 words, cudaStream_t st) {
     FrameBlock<NW> blk;
     memcpy(blk.w, src, size_t(words) * 4);
     cudaLaunchConfig_t cfg{};
@@ -793,19 +793,19 @@ static cudaError_t launch_frame_block_t(u32* arena, const u32* src, u32 words, b
     attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr.val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = &attr;
-    cfg.numAttrs = pdl ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, k_frame_block<NW>, arena, blk, words);
 }
-cudaError_t launch_frame_block(void* device_arena, const void* frame_block, u32 block_bytes, bool pdl, cudaStream_t st) {
+cudaError_t launch_frame_block(void* device_arena, const void* frame_block, u32 block_bytes, cudaStream_t st) {
     if (!frame_block || block_bytes == 0 || (block_bytes & 3u) || block_bytes > HNB_FRAME_BLOCK_MAX_BYTES) return cudaErrorInvalidValue;
     const u32 words = block_bytes / 4u;
-    if (words <= 64u) return launch_frame_block_t<64>((u32*)device_arena, (const u32*)frame_block, words, pdl, st);
-    if (words <= HNB_FRAME_BLOCK_MID_BYTES / 4u) return launch_frame_block_t<HNB_FRAME_BLOCK_MID_BYTES / 4>((u32*)device_arena, (const u32*)frame_block, words, pdl, st);
-    return launch_frame_block_t<HNB_FRAME_BLOCK_MAX_BYTES / 4>((u32*)device_arena, (const u32*)frame_block, words, pdl, st);
+    if (words <= 64u) return launch_frame_block_t<64>((u32*)device_arena, (const u32*)frame_block, words, st);
+    if (words <= HNB_FRAME_BLOCK_MID_BYTES / 4u) return launch_frame_block_t<HNB_FRAME_BLOCK_MID_BYTES / 4>((u32*)device_arena, (const u32*)frame_block, words, st);
+    return launch_frame_block_t<HNB_FRAME_BLOCK_MAX_BYTES / 4>((u32*)device_arena, (const u32*)frame_block, words, st);
 }
 
 template <int NW>
-static cudaError_t launch_bookkeeping_t(const StaticTables& T, u32 num_batches, const u32* block_words_src, u32 block_words, bool pdl, cudaStream_t st) {
+static cudaError_t launch_bookkeeping_t(const StaticTables& T, u32 num_batches, const u32* block_words_src, u32 block_words, cudaStream_t st) {
     FrameBlock<NW> blk;
     if (block_words) memcpy(blk.w, block_words_src, size_t(block_words) * 4);
     cudaLaunchConfig_t cfg{};
@@ -816,18 +816,18 @@ static cudaError_t launch_bookkeeping_t(const StaticTables& T, u32 num_batches, 
     attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr.val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = &attr;
-    cfg.numAttrs = pdl ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, k_bookkeeping<NW>, T, blk, block_words);
 }
-cudaError_t launch_bookkeeping(const StaticTables& T, u32 num_effects, u32 num_batches, const void* frame_block, u32 block_bytes, bool pdl, cudaStream_t st) {
+cudaError_t launch_bookkeeping(const StaticTables& T, u32 num_effects, u32 num_batches, const void* frame_block, u32 block_bytes, cudaStream_t st) {
     if (num_batches == 0) return cudaSuccess;
     if (block_bytes & 3u) return cudaErrorInvalidValue;
     const u32 words = frame_block ? block_bytes / 4u : 0u;
     cudaError_t e;
-    if (words <= BK_HEADER_WORDS) e = launch_bookkeeping_t<int(sizeof(FrameHeader) / 4)>(T, num_batches, (const u32*)frame_block, words, pdl, st);
-    else if (words <= 64u) e = launch_bookkeeping_t<64>(T, num_batches, (const u32*)frame_block, words, pdl, st);
-    else if (words <= HNB_FRAME_BLOCK_MID_BYTES / 4u) e = launch_bookkeeping_t<HNB_FRAME_BLOCK_MID_BYTES / 4>(T, num_batches, (const u32*)frame_block, words, pdl, st);
-    else if (words <= HNB_FRAME_BLOCK_MAX_BYTES / 4u) e = launch_bookkeeping_t<HNB_FRAME_BLOCK_MAX_BYTES / 4>(T, num_batches, (const u32*)frame_block, words, pdl, st);
+    if (words <= BK_HEADER_WORDS) e = launch_bookkeeping_t<int(sizeof(FrameHeader) / 4)>(T, num_batches, (const u32*)frame_block, words, st);
+    else if (words <= 64u) e = launch_bookkeeping_t<64>(T, num_batches, (const u32*)frame_block, words, st);
+    else if (words <= HNB_FRAME_BLOCK_MID_BYTES / 4u) e = launch_bookkeeping_t<HNB_FRAME_BLOCK_MID_BYTES / 4>(T, num_batches, (const u32*)frame_block, words, st);
+    else if (words <= HNB_FRAME_BLOCK_MAX_BYTES / 4u) e = launch_bookkeeping_t<HNB_FRAME_BLOCK_MAX_BYTES / 4>(T, num_batches, (const u32*)frame_block, words, st);
     else return cudaErrorInvalidValue;
     if (e != cudaSuccess) return e;
     if (T.num_child_infos) k_clear_events<<<blocks_for(num_effects, 64), 64, 0, st>>>(T);

@@ -111,12 +111,12 @@ cudaError_t launch_prefix_sum(const StaticTables& T, u32 num_batches, cudaStream
 cudaError_t launch_tile_prefix(const StaticTables& T, u32 batch_index, u32 tile, cudaStream_t st);
 // `frame_block` / `block_bytes`: the first bytes of the HOST frame arena to carry in the kernel's parameter space and store into
 // T.frame from there — NULL / 0: the host copied the frame block; sizeof(FrameHeader): the header only; up to
-// HNB_FRAME_BLOCK_MAX_BYTES: header + every host-written table. `pdl`: launch with programmatic stream serialization.
+// HNB_FRAME_BLOCK_MAX_BYTES: header + every host-written table. Launched with programmatic stream serialization.
 #define HNB_FRAME_BLOCK_MID_BYTES 3840u    // fits the classic 4 KB parameter space together with the table pointers
 #define HNB_FRAME_BLOCK_MAX_BYTES 30720u   // CUDA 12.1+ on sm_70+: 32764 bytes of kernel parameters
-cudaError_t launch_bookkeeping(const StaticTables& T, u32 num_effects, u32 num_batches, const void* frame_block, u32 block_bytes, bool pdl, cudaStream_t st);
+cudaError_t launch_bookkeeping(const StaticTables& T, u32 num_effects, u32 num_batches, const void* frame_block, u32 block_bytes, cudaStream_t st);
 // the same block at the head of a frame that has an init pass (a one-CTA kernel stores it into the device arena)
-cudaError_t launch_frame_block(void* device_arena, const void* frame_block, u32 block_bytes, bool pdl, cudaStream_t st);
+cudaError_t launch_frame_block(void* device_arena, const void* frame_block, u32 block_bytes, cudaStream_t st);
 cudaError_t launch_fill_dispatch_args(const u32* src, u32* dst, u32 src_offset, u32 src_stride, u32 dst_offset,
                                       u32 dst_stride, u32 count, cudaStream_t st);
 cudaError_t launch_slab_reset(u32* ping, u32* pong, u32* dead, u32 first, u32 count, cudaStream_t st);

@@ -200,14 +200,12 @@ struct hnb_ctx {
     std::vector<cudaStream_t> side_streams;
     std::vector<cudaEvent_t> side_done;
     cudaEvent_t fork_event = nullptr;
-    uint32_t max_side_streams = 7;  // HNB_SIDE_STREAMS env (0 = everything on the context stream)
     // ribbon sort scratch (large path), sized to the largest ribbon slab seen so far
     uint64_t* d_sort_keys[2] = {nullptr, nullptr};
     uint32_t* d_sort_vals[2] = {nullptr, nullptr};
     uint32_t* d_sort_hist = nullptr;
     uint32_t sort_rows = 0;
     uint32_t tile_chunks_override = 0;  // HNB_TILE_CHUNKS env: fixed sub-tile count per tile (tuning)
-    bool pdl = true;          // HNB_PDL=0: launch the frame chain without programmatic dependent launch
     bool param_upload = true; // HNB_PARAM_UPLOAD=0: always copy the frame block with the copy engine (never as a kernel parameter)
     unsigned long long* mailbox = nullptr;  // device alias of the caller's pinned count mailbox (hnb_ctx_set_count_mailbox)
     uint32_t mailbox_rows = 0, mailbox_ring = 0;
@@ -651,7 +649,7 @@ void launch_kernel(hnb_ctx* c, CUfunction f, uint32_t blocks, hnb::BatchParams& 
     attr.id = CU_LAUNCH_ATTRIBUTE_PROGRAMMATIC_STREAM_SERIALIZATION;
     attr.value.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = &attr;
-    cfg.numAttrs = c->pdl ? 1 : 0;
+    cfg.numAttrs = 1;
     CUresult r = c->drv.LaunchKernelEx(&cfg, f, args, nullptr);
     if (r != CUDA_SUCCESS) fail(HNB_ERR_CUDA, "cuLaunchKernelEx: " + cu_error_string(c->drv, r));
     c->launches++;
@@ -676,12 +674,13 @@ void launch_update(hnb_ctx* c, LaunchPlan& lp, cudaStream_t st = nullptr) {
 // dispatch per batch into a single compute pass (mod.rs:7280-7370) and leaves the overlap to the driver; here
 // launch k goes to lane k % lanes (lane 0 = the context stream itself). Small batches are latency-bound
 // (a few microseconds of work behind ~10 of launch and pipeline ramp), so concurrency is what fills the GPU.
+constexpr uint32_t kMaxSideStreams = 7;
 struct Fork {
     hnb_ctx* c;
     uint32_t lanes = 1;
     Fork(hnb_ctx* ctx, uint32_t launches) : c(ctx) {
-        if (c->max_side_streams == 0 || launches < 2) return;
-        lanes = std::min<uint32_t>(launches, c->max_side_streams + 1);
+        if (launches < 2) return;
+        lanes = std::min<uint32_t>(launches, kMaxSideStreams + 1);
         while (c->side_streams.size() < lanes - 1) {
             cudaStream_t s = nullptr;
             cudaEvent_t e = nullptr;
@@ -829,8 +828,6 @@ int32_t hnb_ctx_create(int32_t cuda_device, uintptr_t external_stream, hnb_ctx**
         }
         if (const char* env = getenv("HNB_TILE_CHUNKS")) c->tile_chunks_override = (uint32_t)atoi(env);
         if (const char* env = getenv("HNB_EPOCH_START")) c->epoch = uint32_t(strtoul(env, nullptr, 0)) & 0x3fffffffu;  // tests: start near the wrap
-        if (const char* env = getenv("HNB_SIDE_STREAMS")) c->max_side_streams = (uint32_t)std::max(0, std::min(atoi(env), 31));
-        if (const char* env = getenv("HNB_PDL")) c->pdl = atoi(env) != 0;
         if (const char* env = getenv("HNB_PARAM_UPLOAD")) c->param_upload = atoi(env) != 0;
         ensure_arena(c.get(), 0, 0);
         CUDA_CHECK(cudaMalloc((void**)&c->d_debug, kDebugWords * 8));
@@ -1621,7 +1618,7 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
         // with an init pass the block needs a (one-CTA) kernel of its own at the head of the frame: init reads the tables first
         const bool block_kernel = param_block && any_init;
         if (block_kernel) {
-            CUDA_CHECK(hnb::launch_frame_block(c->d_arena, c->h_arena, uint32_t(c->lay.off_prefix_sum), c->pdl, c->stream));
+            CUDA_CHECK(hnb::launch_frame_block(c->d_arena, c->h_arena, uint32_t(c->lay.off_prefix_sum), c->stream));
             c->launches++;
             for (auto& lp : plans) lp.params.late_tables = 1u;
         }
@@ -1654,7 +1651,7 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
             if (param_block && !block_kernel) { block = c->h_arena; block_bytes = uint32_t(c->lay.off_prefix_sum); }
             else if (block_kernel) { /* already stored by k_frame_block, header included */ }
             else if (!copy_block) { block = c->header(); block_bytes = uint32_t(sizeof(hnb::FrameHeader)); }
-            CUDA_CHECK(hnb::launch_bookkeeping(static_tables(c), c->header()->sim.num_effects, c->B, block, block_bytes, c->pdl, c->stream));
+            CUDA_CHECK(hnb::launch_bookkeeping(static_tables(c), c->header()->sim.num_effects, c->B, block, block_bytes, c->stream));
             if (param_block && !block_kernel) { c->dirty_tables = false; c->plan_dirty = false; }  // the tables went with this launch
             c->launches += 1 + (c->child_rows ? 1 : 0);
             std::fill(c->init_pending.begin(), c->init_pending.end(), 0);

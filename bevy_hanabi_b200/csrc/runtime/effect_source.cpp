@@ -216,21 +216,12 @@ uint32_t rows_per_lane() {
     return 16;
 }
 
-uint32_t park_depth() {
-    // tiles a warp keeps parked behind the one it streams (HNB_PARK in the kernel); HNB_PARK env for tuning
-    if (const char* e = getenv("HNB_PARK")) {
-        int v = atoi(e);
-        if (v >= 1 && v <= 4) return (uint32_t)v;
-    }
-    return 1;
-}
-
 uint32_t update_smem_bytes(const hnb_effect_desc& d) {
     // must mirror the carve-up at the top of hnb_update (hnb_particle_kernels.cuh)
-    const uint32_t R = rows_per_lane(), warps = 8, park = park_depth();
+    const uint32_t R = rows_per_lane(), warps = 8;
     uint32_t bytes = (2047 + 1) * 4;
-    bytes += (R * 32 * 4 + 2 * R * 4) * (park + 1) * warps;  // alive-list entries, survivor ballots, valid masks: park + 1 buffers
-    bytes += 64 * park * warps;                              // PendingTile records
+    bytes += (R * 32 * 4 + 2 * R * 4) * 2 * warps;  // alive-list entries, survivor ballots, valid masks: streamed and parked tile
+    bytes += 64 * warps;                            // PendingTile record of the parked tile
     if (d.properties_size) bytes += ((d.properties_size + 15) / 16 * 16) * warps;
     return bytes;
 }
@@ -264,7 +255,7 @@ std::string generate_effect_source(const hnb_effect_desc& d) {
     o << kSrcWgsl << "\n" << kSrcTables << "\n";
     o << "namespace hnb {\n";
     // Tuning hook for experiments: HNB_DEFINES="NAME=VALUE;NAME2=VALUE2" prepends #defines that the
-    // kernel templates honour through #ifndef guards (tile shape, look-back back-off, cache hints).
+    // kernel templates honour through #ifndef guards (tile shape, cache hints).
     if (const char* env = getenv("HNB_DEFINES")) {
         std::string e(env);
         size_t pos = 0;
@@ -276,7 +267,7 @@ std::string generate_effect_source(const hnb_effect_desc& d) {
             // The host sizes the dynamic shared memory and the grid from its own copy of these (update_smem_bytes,
             // plan_batch): overriding them here would make the kernel's carve-up disagree with the launch. Ignored, loudly.
             static const char* const kHostMirrored[] = {"HNB_SMEM_EFFECTS", "HNB_BLOCK", "HNB_WARPS", "HNB_ROWS_PER_LANE", "HNB_TILE_K",
-                                                        "HNB_NUM_PLANES", "HNB_INIT_ITEMS", "HNB_MAX_CHUNKS", "HNB_INIT_SMEM_EFFECTS", "HNB_PARK"};
+                                                        "HNB_NUM_PLANES", "HNB_INIT_ITEMS", "HNB_MAX_CHUNKS", "HNB_INIT_SMEM_EFFECTS"};
             const std::string name = item.substr(0, eq);
             bool mirrored = false;
             for (const char* m : kHostMirrored) mirrored |= name == m;
@@ -291,7 +282,6 @@ std::string generate_effect_source(const hnb_effect_desc& d) {
     o << "#define HNB_NUM_PLANES " << planes.size() << "\n";
     o << "#define HNB_TILE_K " << choose_tile_k(d) << "\n";
     o << "#define HNB_ROWS_PER_LANE " << rows_per_lane() << "\n";
-    o << "#define HNB_PARK " << park_depth() << "\n";
     o << "#define HNB_INIT_ITEMS " << kInitItems << "\n";
     o << "#define HNB_HAS_PROPERTIES " << (d.properties_size ? 1 : 0) << "\n";
     o << "#define HNB_CONSUME_EVENTS " << (consume ? 1 : 0) << "\n";

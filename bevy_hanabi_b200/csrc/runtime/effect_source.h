@@ -38,7 +38,7 @@ constexpr uint32_t kInitSmemBytes = 1024 * 4;  // HNB_INIT_SMEM_EFFECTS spawn-pr
 uint32_t rows_per_lane();  // == HNB_ROWS_PER_LANE of the generated kernels: tile_rows <= 32 * rows_per_lane()
 uint32_t choose_tile_k(const hnb_effect_desc& d);
 // Dynamic shared memory of hnb_update for this effect (tile-prefix table + per-warp double-buffered stash +
-// pending-tile records + Properties staging).
+// parked-tile record + Properties staging).
 uint32_t update_smem_bytes(const hnb_effect_desc& d);
 
 // The complete translation unit (throws std::invalid_argument on a bad description).

@@ -213,7 +213,7 @@ def test_relaxed_order(shaped_ctx, orc, name):
 
 
 # ---- the slab-size rule ------------------------------------------------------------------------------------------------
-# The update kernel's dynamic shared memory (42.5 KiB at the default rows per lane and park depth) leaves room for at most 5
+# The update kernel's dynamic shared memory (42.5 KiB at the default rows per lane) leaves room for at most 5
 # CTAs of 8 warps on an H100's 228 KiB: from 8 waves of those warps up, plan_batch always picks the largest tile.
 MAX_CTAS_PER_SM = 5
 

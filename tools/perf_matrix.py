@@ -471,25 +471,21 @@ def fresh_sector():
 
 
 def frame_chain():
-    """Whole frames (bookkeeping + update, state resident, no table changes) back to back, with and without programmatic
-    dependent launch: what one step costs beyond its update kernel, at the shard sizes of the strong-scaling runs."""
-    import os
+    """Whole frames (bookkeeping + update, state resident, no table changes) back to back: what one step costs beyond its
+    update kernel, at the shard sizes of the strong-scaling runs."""
     for mi in (1, 2, 4, 8, 16, 64):
         P = mi << 20
-        for pdl in ("0", "1"):
-            os.environ["HNB_PDL"] = pdl
-            ctx = hb.Context(0, stream.cuda_stream)
-            slab = ctx.slab_create(P, 32)
-            ctx.slab_fill_c5(slab, 0, P, 42, 1e9, 1e9)
-            single_instance(ctx, P, 32, alive=P)
-            la = [N.BatchLaunch.make(ctx.effect_compile(recipes.c5_lowered()), slab, 0, 0)]
-            for _ in range(10):
-                ctx.simulate(la)
-            fr = min(frame_ms(ctx, la, 200) for _ in range(3))
-            k = timed_update(ctx, la, 50)
-            report(f"C5 {mi:2d}Mi frame chain, HNB_PDL={pdl}", fr, 72 * P, f"isolated update kernel {k:.4f} ms; frame - kernel = {1e3 * (fr - k):+.1f} us")
-            ctx.close()
-    os.environ.pop("HNB_PDL", None)
+        ctx = hb.Context(0, stream.cuda_stream)
+        slab = ctx.slab_create(P, 32)
+        ctx.slab_fill_c5(slab, 0, P, 42, 1e9, 1e9)
+        single_instance(ctx, P, 32, alive=P)
+        la = [N.BatchLaunch.make(ctx.effect_compile(recipes.c5_lowered()), slab, 0, 0)]
+        for _ in range(10):
+            ctx.simulate(la)
+        fr = min(frame_ms(ctx, la, 200) for _ in range(3))
+        k = timed_update(ctx, la, 50)
+        report(f"C5 {mi:2d}Mi frame chain", fr, 72 * P, f"isolated update kernel {k:.4f} ms; frame - kernel = {1e3 * (fr - k):+.1f} us")
+        ctx.close()
 
 
 def chunks_sweep():
