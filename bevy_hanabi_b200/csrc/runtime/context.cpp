@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "../kernels/hnb_static_kernels.h"
+#include "cuda_owned.h"
 #include "driver.h"
 #include "effect_source.h"
 #include "hanabi_b200.h"
@@ -86,13 +87,13 @@ struct Slab {
     uint32_t capacity = 0, stride = 0;
     bool sector_planes = false;  // HNB_SLAB_SECTOR_PLANES
     std::vector<Plane> planes;   // physical columns
-    void* d_planes[HNB_RT_MAX_PLANES] = {};
-    uint32_t *ping = nullptr, *pong = nullptr, *dead = nullptr;
-    uint32_t* alive_bits = nullptr;  // one bit per row (HNB_EFFECT_SLOT_ORDER effects keep it current)
-    unsigned long long* ident_claim = nullptr;  // [2]: identity claims of ping / pong (hnb_claim_pack)
+    DeviceArray<char> d_planes[HNB_RT_MAX_PLANES];
+    DeviceArray<uint32_t> ping, pong, dead;
+    DeviceArray<uint32_t> alive_bits;  // one bit per row (HNB_EFFECT_SLOT_ORDER effects keep it current)
+    DeviceArray<unsigned long long> ident_claim;  // [2]: identity claims of ping / pong (hnb_claim_pack)
     // HNB_EFFECT_ORDERED_EVENTS scratch, allocated on first use: per channel the per-row event counts and their block sums
-    uint32_t* event_counts[HNB_MAX_EVENT_BINDINGS] = {};
-    uint32_t* event_block_sums[HNB_MAX_EVENT_BINDINGS] = {};
+    DeviceArray<uint32_t> event_counts[HNB_MAX_EVENT_BINDINGS];
+    DeviceArray<uint32_t> event_block_sums[HNB_MAX_EVENT_BINDINGS];
 };
 
 struct KernelModule {
@@ -108,24 +109,23 @@ struct Effect {
     KernelModule* km = nullptr;
     uint32_t tile_k = 4, flags = 0, particle_stride = 0, parent_stride = 0, rows_per_lane = 16, update_smem = 0;
     int update_blocks_per_sm = 1;
-    uint32_t props_size = 0, props_stride = 0, props_rows = 0;
-    char* d_props = nullptr;
+    uint32_t props_size = 0, props_stride = 0;
+    DeviceArray<char> d_props;  // rows of props_stride bytes
     std::string name;
-};
-
-struct EventBuffer {
-    uint32_t capacity = 0;
-    uint32_t* d = nullptr;
 };
 
 // Pinned staging slot of the per-frame upload (see flush_arena).
 constexpr size_t kDebugWords = 16 + 4 * 64;
 constexpr int kStageSlots = 32;  // frames the host may queue ahead of the GPU before blocking
 struct StageSlot {
-    char* h = nullptr;
-    size_t cap = 0;
-    cudaEvent_t done = nullptr;
+    PinnedBlock h;
+    Event done;
     bool used = false;
+};
+
+struct SideStream {
+    Stream stream;
+    Event done;
 };
 
 struct ArenaLayout {
@@ -152,168 +152,119 @@ struct LaunchPlan;
 }
 
 struct hnb_ctx {
+    // Members are destroyed in reverse order: every buffer and event below goes first, then the side streams, and the
+    // context stream last.
+    Stream stream;  // created with the context, or the caller's external stream (borrowed, never destroyed)
+    // side streams: the update (and independent init) launches of a multi-batch frame run concurrently
+    std::vector<SideStream> side_streams;
+    Event fork_event;
+
     int device = 0;
     int sm_count = 132;
     std::vector<uint8_t> init_pending;   // per batch: a stand-alone hnb_pass_init whose accounting hnb_pass_indirect has not applied yet
     std::vector<LaunchPlan> frame_plans;  // hnb_simulate's per-frame launch plans (kept to avoid a heap allocation per frame)
-    cudaStream_t stream = nullptr;
-    bool own_stream = false;
     DriverApi drv;
     uint64_t launches = 0;
 
     // per-frame arena (host pinned + device mirror), exact-size layout for (E, B)
     uint32_t E = 0, B = 0;
     ArenaLayout lay = ArenaLayout::make(0, 0);
-    char* h_arena = nullptr;
-    char* d_arena = nullptr;
-    size_t arena_cap = 0;
+    PinnedBlock h_arena;
+    DeviceArray<char> d_arena;
     bool dirty_tables = true;  // spawners / batch infos / prefix sums changed since last flush
     StageSlot stage[kStageSlots];  // pinned snapshots of the frame block, one per in-flight frame
     uint32_t stage_next = 0;
     uint32_t epoch = 0;
 
     // persistent device tables
-    uint32_t md_rows = 0, draw_rows = 0, child_rows = 0;
-    hnb::EffectMetadata* d_metadata = nullptr;
-    uint32_t* d_draw_args = nullptr;
-    hnb::ChildInfo* d_child_infos = nullptr;
+    DeviceArray<hnb::EffectMetadata> d_metadata;
+    DeviceArray<hnb_draw_indexed_indirect_args> d_draw_args;
+    DeviceArray<hnb::ChildInfo> d_child_infos;  // its size is the logical array length the kernels read (num_child_infos)
     // per-instance / per-batch scratch
-    uint32_t scratch_E = 0, scratch_B = 0;
-    uint32_t *d_tile_prefix = nullptr, *d_dispatch_args = nullptr, *d_batch_tiles = nullptr, *d_tickets = nullptr;
-    std::vector<unsigned long long*> d_tile_state;  // per batch
-    std::vector<uint32_t> tile_state_cap;
+    DeviceArray<uint32_t> d_tile_prefix;
+    // per batch slot: the dispatch args (3 words), then the tile counts, then the tickets. One block, so that growing
+    // it takes one synchronisation.
+    DeviceArray<uint32_t> d_batch_scratch;
+    std::vector<DeviceArray<unsigned long long>> d_tile_state;  // per batch
     std::vector<hnb_rt::TileStateSlot> tile_state_slot;  // when the batch's states were last zeroed (tile_state_rule.h)
     uint64_t tile_state_clears = 0;  // zeroings tile_state_needs_clear asked for (hnb_ctx_tile_state_clears)
     uint64_t md_generation = 1;            // bumped by hnb_metadata_insert
 
     std::vector<Slab> slabs;
     std::vector<Effect> effects;
-    std::vector<EventBuffer> event_buffers;
+    std::vector<DeviceArray<uint32_t>> event_buffers;
     std::unordered_map<uint64_t, std::unique_ptr<KernelModule>> modules;  // ≙ ShaderCache
 
     // kernel timing
     bool timing = false;
-    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pending, ev_free;
+    std::vector<std::pair<Event, Event>> ev_pending, ev_free;
     double update_ms = 0.0;
     uint64_t update_launches = 0;
-    // side streams: the update (and independent init) launches of a multi-batch frame run concurrently
-    std::vector<cudaStream_t> side_streams;
-    std::vector<cudaEvent_t> side_done;
-    cudaEvent_t fork_event = nullptr;
-    // ribbon sort scratch (large path), sized to the largest ribbon slab seen so far
-    uint64_t* d_sort_keys[2] = {nullptr, nullptr};
-    uint32_t* d_sort_vals[2] = {nullptr, nullptr};
-    uint32_t* d_sort_hist = nullptr;
-    uint32_t sort_rows = 0;
+    // ribbon sort scratch (large path), sized to the largest ribbon slab seen so far: keys[2] (8 bytes per row), then
+    // vals[2] (4 bytes per row), so three 8-byte words per row in one block that grows with one synchronisation
+    DeviceArray<uint64_t> d_sort_scratch;
+    DeviceArray<uint32_t> d_sort_hist;
     uint32_t tile_chunks_override = 0;  // HNB_TILE_CHUNKS env: fixed sub-tile count per tile (tuning)
     bool param_upload = true; // HNB_PARAM_UPLOAD=0: always copy the frame block with the copy engine (never as a kernel parameter)
     unsigned long long* mailbox = nullptr;  // device alias of the caller's pinned count mailbox (hnb_ctx_set_count_mailbox)
     uint32_t mailbox_rows = 0, mailbox_ring = 0;
     bool plan_dirty = false;  // plan_batch changed a tile-size or range word of the host frame block since the last upload
     uint64_t frame_copies = 0, frames = 0;  // hnb_simulate calls that needed the host->device copy of the frame block / all calls
-    unsigned long long* d_debug = nullptr;  // 16 diagnostic counters + a 64-frame timeline ring of 4 words (HNB_PROFILE kernels)
+    DeviceArray<unsigned long long> d_debug;  // 16 diagnostic counters + a 64-frame timeline ring of 4 words (HNB_PROFILE kernels)
 
-    hnb::FrameHeader* header() { return reinterpret_cast<hnb::FrameHeader*>(h_arena); }
-    template <typename T> T* h_at(size_t off) { return reinterpret_cast<T*>(h_arena + off); }
-    template <typename T> T* d_at(size_t off) { return reinterpret_cast<T*>(d_arena + off); }
+    hnb::FrameHeader* header() { return reinterpret_cast<hnb::FrameHeader*>(h_arena.get()); }
+    template <typename T> T* h_at(size_t off) { return reinterpret_cast<T*>(h_arena.get() + off); }
+    template <typename T> T* d_at(size_t off) { return reinterpret_cast<T*>(d_arena.get() + off); }
+    uint32_t scratch_B() const { return uint32_t(d_batch_scratch.size() / 5); }
+    uint32_t* dispatch_args() const { return d_batch_scratch.get(); }
+    uint32_t* batch_tiles() const { return d_batch_scratch.get() + 3 * size_t(scratch_B()); }
+    uint32_t* tickets() const { return d_batch_scratch.get() + 4 * size_t(scratch_B()); }
+    uint32_t* draw_args() const { return reinterpret_cast<uint32_t*>(d_draw_args.get()); }  // as the kernels index it: 5 words per row
 };
 
 namespace {
+
+// Moves the tables of the frame block from layout `ol` (E = oE, B = oB) to layout `nl`, keeping the rows both have.
+void relocate_tables(char* dst, const ArenaLayout& nl, uint32_t E, uint32_t B, const char* src, const ArenaLayout& ol, uint32_t oE, uint32_t oB) {
+    const uint32_t mB = std::min(oB, B), mE = std::min(oE, E);
+    memcpy(dst, src, sizeof(hnb::FrameHeader));
+    memcpy(dst + nl.off_batch_infos, src + ol.off_batch_infos, size_t(mB) * sizeof(hnb_batch_info));
+    memcpy(dst + nl.off_tile_size, src + ol.off_tile_size, size_t(mB) * 4);
+    memcpy(dst + nl.off_spawners, src + ol.off_spawners, size_t(mE) * sizeof(hnb_spawner));
+    memcpy(dst + nl.off_range, src + ol.off_range, size_t(mE) * 4);
+    memcpy(dst + nl.off_spawn_prefix, src + ol.off_spawn_prefix, size_t(mE) * 4);
+    memcpy(dst + nl.off_prefix_sum, src + ol.off_prefix_sum, size_t(mE) * 4);
+}
 
 void ensure_arena(hnb_ctx* c, uint32_t E, uint32_t B) {
     if (E == c->E && B == c->B && c->h_arena) return;
     ArenaLayout nl = ArenaLayout::make(E, B);
     size_t need = std::max<size_t>(nl.total, 256);
-    char* nh = c->h_arena;
-    if (need > c->arena_cap) {
+    // the tables move to their new offsets through a copy of the old host block
+    std::vector<char> old(c->h_arena.get(), c->h_arena.get() + (c->h_arena ? c->lay.total : 0));
+    if (need > c->h_arena.size()) {
         size_t cap = std::max(need * 2, size_t(4096));
-        CUDA_CHECK(cudaMallocHost((void**)&nh, cap));
-        memset(nh, 0, cap);
-        char* nd = nullptr;
-        CUDA_CHECK(cudaMalloc((void**)&nd, cap));
-        CUDA_CHECK(cudaMemsetAsync(nd, 0, cap, c->stream));
-        // move: copy old host contents into the new buffer at the new offsets
-        std::vector<char> old(c->h_arena ? c->lay.total : 0);
-        if (c->h_arena) memcpy(old.data(), c->h_arena, c->lay.total);
-        if (c->h_arena) {
-            CUDA_CHECK(cudaStreamSynchronize(c->stream));
-            cudaFreeHost(c->h_arena);
-            cudaFree(c->d_arena);
-        }
-        const ArenaLayout ol = c->lay;
-        const uint32_t oE = c->E, oB = c->B;
-        c->h_arena = nh;
-        c->d_arena = nd;
-        c->arena_cap = cap;
-        if (!old.empty()) {
-            memcpy(nh, old.data(), sizeof(hnb::FrameHeader));
-            uint32_t mB = std::min(oB, B), mE = std::min(oE, E);
-            memcpy(nh + nl.off_batch_infos, old.data() + ol.off_batch_infos, size_t(mB) * sizeof(hnb_batch_info));
-            memcpy(nh + nl.off_tile_size, old.data() + ol.off_tile_size, size_t(mB) * 4);
-            memcpy(nh + nl.off_spawners, old.data() + ol.off_spawners, size_t(mE) * sizeof(hnb_spawner));
-            memcpy(nh + nl.off_range, old.data() + ol.off_range, size_t(mE) * 4);
-            memcpy(nh + nl.off_spawn_prefix, old.data() + ol.off_spawn_prefix, size_t(mE) * 4);
-            memcpy(nh + nl.off_prefix_sum, old.data() + ol.off_prefix_sum, size_t(mE) * 4);
-        }
+        PinnedBlock nh;
+        CUDA_CHECK(nh.alloc(cap));
+        memset(nh.get(), 0, cap);
+        CUDA_CHECK(grow(c->d_arena, cap, 0, c->stream));
+        c->h_arena = std::move(nh);
     } else if (c->h_arena) {
-        // same buffer, new offsets: repack through a temporary copy
-        std::vector<char> old(c->lay.total);
-        memcpy(old.data(), c->h_arena, c->lay.total);
-        const ArenaLayout ol = c->lay;
-        uint32_t mB = std::min(c->B, B), mE = std::min(c->E, E);
-        memset(c->h_arena + sizeof(hnb::FrameHeader), 0, nl.total - sizeof(hnb::FrameHeader));
-        memcpy(nh + nl.off_batch_infos, old.data() + ol.off_batch_infos, size_t(mB) * sizeof(hnb_batch_info));
-        memcpy(nh + nl.off_tile_size, old.data() + ol.off_tile_size, size_t(mB) * 4);
-        memcpy(nh + nl.off_spawners, old.data() + ol.off_spawners, size_t(mE) * sizeof(hnb_spawner));
-        memcpy(nh + nl.off_range, old.data() + ol.off_range, size_t(mE) * 4);
-        memcpy(nh + nl.off_spawn_prefix, old.data() + ol.off_spawn_prefix, size_t(mE) * 4);
-        memcpy(nh + nl.off_prefix_sum, old.data() + ol.off_prefix_sum, size_t(mE) * 4);
+        memset(c->h_arena.get() + sizeof(hnb::FrameHeader), 0, nl.total - sizeof(hnb::FrameHeader));
     }
+    if (!old.empty()) relocate_tables(c->h_arena.get(), nl, E, B, old.data(), c->lay, c->E, c->B);
     c->lay = nl;
     c->E = E;
     c->B = B;
     c->dirty_tables = true;
 }
 
-template <typename T> void grow_device(T*& p, uint32_t& rows, uint32_t need, cudaStream_t st) {
-    if (need <= rows) return;
-    uint32_t cap = std::max<uint32_t>(need, std::max<uint32_t>(rows * 2, 16));
-    T* np = nullptr;
-    CUDA_CHECK(cudaMalloc((void**)&np, size_t(cap) * sizeof(T)));
-    CUDA_CHECK(cudaMemsetAsync(np, 0, size_t(cap) * sizeof(T), st));
-    if (p) {
-        CUDA_CHECK(cudaMemcpyAsync(np, p, size_t(rows) * sizeof(T), cudaMemcpyDeviceToDevice, st));
-        CUDA_CHECK(cudaStreamSynchronize(st));
-        cudaFree(p);
-    }
-    p = np;
-    rows = cap;
-}
-
 void ensure_scratch(hnb_ctx* c) {
-    if (c->E > c->scratch_E) {
-        if (c->d_tile_prefix) {
-            CUDA_CHECK(cudaStreamSynchronize(c->stream));  // earlier frames may still read the old table
-            cudaFree(c->d_tile_prefix);
-        }
-        uint32_t cap = std::max<uint32_t>(c->E * 2, 64);
-        CUDA_CHECK(cudaMalloc((void**)&c->d_tile_prefix, size_t(cap) * 4));
-        CUDA_CHECK(cudaMemsetAsync(c->d_tile_prefix, 0, size_t(cap) * 4, c->stream));
-        c->scratch_E = cap;
-    }
-    if (c->B > c->scratch_B) {
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        if (c->d_dispatch_args) { cudaFree(c->d_dispatch_args); cudaFree(c->d_batch_tiles); cudaFree(c->d_tickets); }
+    if (c->E > c->d_tile_prefix.size()) CUDA_CHECK(grow(c->d_tile_prefix, std::max<uint32_t>(c->E * 2, 64), 0, c->stream));
+    if (c->B > c->scratch_B()) {
         uint32_t cap = std::max<uint32_t>(c->B * 2, 16);
-        CUDA_CHECK(cudaMalloc((void**)&c->d_dispatch_args, size_t(cap) * 12));
-        CUDA_CHECK(cudaMalloc((void**)&c->d_batch_tiles, size_t(cap) * 4));
-        CUDA_CHECK(cudaMalloc((void**)&c->d_tickets, size_t(cap) * 4));
-        CUDA_CHECK(cudaMemsetAsync(c->d_dispatch_args, 0, size_t(cap) * 12, c->stream));
-        CUDA_CHECK(cudaMemsetAsync(c->d_batch_tiles, 0, size_t(cap) * 4, c->stream));
-        CUDA_CHECK(cudaMemsetAsync(c->d_tickets, 0, size_t(cap) * 4, c->stream));
-        c->scratch_B = cap;
-        c->d_tile_state.resize(cap, nullptr);
-        c->tile_state_cap.resize(cap, 0);
+        CUDA_CHECK(grow(c->d_batch_scratch, size_t(cap) * 5, 0, c->stream));
+        c->d_tile_state.resize(cap);
         c->tile_state_slot.resize(cap);
     }
 }
@@ -324,16 +275,16 @@ hnb::StaticTables static_tables(hnb_ctx* c) {
     T.spawners = c->d_at<hnb::Spawner>(c->lay.off_spawners);
     T.spawn_range = c->d_at<uint32_t>(c->lay.off_range);
     T.prefix_sum = c->d_at<uint32_t>(c->lay.off_prefix_sum);
-    T.tile_prefix = c->d_tile_prefix;
+    T.tile_prefix = c->d_tile_prefix.get();
     T.batch_infos = c->d_at<hnb::BatchInfo>(c->lay.off_batch_infos);
     T.batch_tile_size = c->d_at<uint32_t>(c->lay.off_tile_size);
-    T.dispatch_args = c->d_dispatch_args;
-    T.batch_tiles = c->d_batch_tiles;
-    T.tickets = c->d_tickets;
-    T.metadata = c->d_metadata;
-    T.draw_args = c->d_draw_args;
-    T.child_infos = c->d_child_infos;
-    T.num_child_infos = c->child_rows;
+    T.dispatch_args = c->dispatch_args();
+    T.batch_tiles = c->batch_tiles();
+    T.tickets = c->tickets();
+    T.metadata = c->d_metadata.get();
+    T.draw_args = c->draw_args();
+    T.child_infos = c->d_child_infos.get();
+    T.num_child_infos = uint32_t(c->d_child_infos.size());
     return T;
 }
 
@@ -350,14 +301,10 @@ void flush_arena(hnb_ctx* c, bool with_ranges) {
     // a pinned staging slot that is not reused until its copy has completed.
     StageSlot& slot = c->stage[c->stage_next++ % kStageSlots];
     if (slot.used) CUDA_CHECK(cudaEventSynchronize(slot.done));
-    if (slot.cap < bytes) {
-        if (slot.h) cudaFreeHost(slot.h);
-        slot.cap = std::max(bytes * 2, size_t(4096));
-        CUDA_CHECK(cudaMallocHost((void**)&slot.h, slot.cap));
-    }
-    if (!slot.done) CUDA_CHECK(cudaEventCreateWithFlags(&slot.done, cudaEventDisableTiming));
-    memcpy(slot.h, c->h_arena, bytes);
-    CUDA_CHECK(cudaMemcpyAsync(c->d_arena, slot.h, bytes, cudaMemcpyHostToDevice, c->stream));
+    if (slot.h.size() < bytes) CUDA_CHECK(slot.h.alloc(std::max(bytes * 2, size_t(4096))));
+    if (!slot.done) CUDA_CHECK(slot.done.create(cudaEventDisableTiming));
+    memcpy(slot.h.get(), c->h_arena.get(), bytes);
+    CUDA_CHECK(cudaMemcpyAsync(c->d_arena.get(), slot.h.get(), bytes, cudaMemcpyHostToDevice, c->stream));
     CUDA_CHECK(cudaEventRecord(slot.done, c->stream));
     slot.used = true;
     c->dirty_tables = false;
@@ -370,8 +317,8 @@ void next_epoch(hnb_ctx* c) {
         // 30-bit wrap (207 days at 60 frames/s): a tile state left untouched since the same epoch of the previous
         // cycle would look current, so drop them all. 0 = "never written".
         c->epoch = 1;
-        for (size_t b = 0; b < c->d_tile_state.size(); ++b)
-            if (c->d_tile_state[b]) CUDA_CHECK(cudaMemsetAsync(c->d_tile_state[b], 0, size_t(c->tile_state_cap[b]) * 8, c->stream));
+        for (const auto& ts : c->d_tile_state)
+            if (ts) CUDA_CHECK(cudaMemsetAsync(ts.get(), 0, ts.size() * 8, c->stream));
     }
     c->header()->epoch = c->epoch;
     c->header()->num_batches = c->B;
@@ -389,7 +336,7 @@ Effect& get_effect(hnb_ctx* c, hnb_effect e) {
 hnb::PlaneSet plane_set(const Slab& s) {
     hnb::PlaneSet ps{};
     for (size_t p = 0; p < s.planes.size(); ++p) {
-        ps.ptr[p] = s.d_planes[p];
+        ps.ptr[p] = s.d_planes[p].get();
         ps.words[p] = s.planes[p].width / 4;
         ps.word_off[p] = s.planes[p].offset / 4;
         for (uint32_t w = 0; w < s.planes[p].width / 4; ++w) ps.word_to_plane[s.planes[p].offset / 4 + w] = (unsigned char)p;
@@ -399,19 +346,26 @@ hnb::PlaneSet plane_set(const Slab& s) {
 
 hnb::SlabView slab_view(const Slab& s) {
     hnb::SlabView v{};
-    for (size_t p = 0; p < s.planes.size(); ++p) v.planes[p] = s.d_planes[p];
-    v.particle_index[0] = s.ping;
-    v.particle_index[1] = s.pong;
-    v.dead_index = s.dead;
-    v.alive_bits = s.alive_bits;
-    v.ident_claim = s.ident_claim;
+    for (size_t p = 0; p < s.planes.size(); ++p) v.planes[p] = s.d_planes[p].get();
+    v.particle_index[0] = s.ping.get();
+    v.particle_index[1] = s.pong.get();
+    v.dead_index = s.dead.get();
+    v.alive_bits = s.alive_bits.get();
+    v.ident_claim = s.ident_claim.get();
     v.capacity_rows = s.capacity;
     return v;
 }
 
 // Drops both identity claims of the slab, in stream order: for writers of the index columns that do not keep them true.
 void clear_ident_claims(hnb_ctx* c, const Slab& s) {
-    CUDA_CHECK(cudaMemsetAsync(s.ident_claim, 0, 2 * sizeof(unsigned long long), c->stream));
+    CUDA_CHECK(cudaMemsetAsync(s.ident_claim.get(), 0, 2 * sizeof(unsigned long long), c->stream));
+}
+
+// Copies `bytes` from the device to the host in stream order (and then zeroes the source when `clear`), and waits.
+void read_back(hnb_ctx* c, void* out, void* d_src, size_t bytes, bool clear = false) {
+    CUDA_CHECK(cudaMemcpyAsync(out, d_src, bytes, cudaMemcpyDeviceToHost, c->stream));
+    if (clear) CUDA_CHECK(cudaMemsetAsync(d_src, 0, bytes, c->stream));
+    CUDA_CHECK(cudaStreamSynchronize(c->stream));
 }
 
 void check_rows(const Slab& s, uint32_t first, uint32_t count) {
@@ -454,15 +408,8 @@ struct LaunchPlan {
 };
 
 void ensure_tile_state(hnb_ctx* c, uint32_t batch, uint32_t tiles) {
-    if (c->tile_state_cap[batch] >= tiles) return;
-    if (c->d_tile_state[batch]) {
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        cudaFree(c->d_tile_state[batch]);
-    }
-    uint32_t cap = tiles + tiles / 2 + 64;
-    CUDA_CHECK(cudaMalloc((void**)&c->d_tile_state[batch], size_t(cap) * 8));
-    CUDA_CHECK(cudaMemsetAsync(c->d_tile_state[batch], 0, size_t(cap) * 8, c->stream));
-    c->tile_state_cap[batch] = cap;
+    if (c->d_tile_state[batch].size() >= tiles) return;
+    CUDA_CHECK(grow(c->d_tile_state[batch], tiles + tiles / 2 + 64, 0, c->stream));
     c->tile_state_slot[batch] = hnb_rt::TileStateSlot{};
 }
 
@@ -535,7 +482,7 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
         // threads of the last partial workgroup would read past the buffer when a parent over-emits (event_count is
         // unclamped, lib.rs:976-993), which WGSL's robust buffer access forgives and raw CUDA does not. The init
         // accounting in the bookkeeping kernel uses the same bound (range = capacity).
-        init_threads = c->event_buffers[bl.consume_events].capacity;
+        init_threads = uint32_t(c->event_buffers[bl.consume_events].size());
     } else {
         init_threads = ceil_div(lp.total_spawn, 64) * 64;  // dispatch_workgroups(ceil(n/64)), mod.rs:7157-7173
     }
@@ -572,7 +519,7 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
             sig |= 1;
         }
         if (hnb_rt::tile_state_needs_clear(c->tile_state_slot[lp.batch], sig, hnb_rt::tile_state_run_epoch(c->epoch))) {
-            CUDA_CHECK(cudaMemsetAsync(c->d_tile_state[lp.batch], 0, size_t(c->tile_state_cap[lp.batch]) * 8, c->stream));
+            CUDA_CHECK(cudaMemsetAsync(c->d_tile_state[lp.batch].get(), 0, c->d_tile_state[lp.batch].size() * 8, c->stream));
             c->tile_state_clears++;
         }
     }
@@ -582,15 +529,15 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
     P.spawners = c->d_at<hnb::Spawner>(c->lay.off_spawners);
     P.spawn_prefix = c->d_at<uint32_t>(c->lay.off_spawn_prefix);
     P.prefix_sum = c->d_at<uint32_t>(c->lay.off_prefix_sum);
-    P.tile_prefix = c->d_tile_prefix;
+    P.tile_prefix = c->d_tile_prefix.get();
     P.batch_info = c->d_at<hnb::BatchInfo>(c->lay.off_batch_infos) + lp.batch;
-    P.batch_tiles = c->d_batch_tiles + lp.batch;
-    P.ticket = c->d_tickets + lp.batch;
-    P.tile_state = c->d_tile_state[lp.batch];
-    P.metadata = c->d_metadata;
-    P.draw_args = c->d_draw_args;
-    P.child_infos = c->d_child_infos;
-    P.properties = lp.fx->d_props;
+    P.batch_tiles = c->batch_tiles() + lp.batch;
+    P.ticket = c->tickets() + lp.batch;
+    P.tile_state = c->d_tile_state[lp.batch].get();
+    P.metadata = c->d_metadata.get();
+    P.draw_args = c->draw_args();
+    P.child_infos = c->d_child_infos.get();
+    P.properties = lp.fx->d_props.get();
     P.properties_stride = lp.fx->props_stride;
     P.slab = slab_view(*lp.slab);
     if (bl.parent_slab != 0xFFFFFFFFu) {
@@ -598,27 +545,26 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
         if (parent.sector_planes) fail(HNB_ERR_LAYOUT, "a parent slab read by a child effect must use the default plane layout");
         P.parent_slab = slab_view(parent);
     }
-    if (consume) P.consume_events = c->event_buffers[bl.consume_events].d;
+    if (consume) P.consume_events = c->event_buffers[bl.consume_events].get();
     for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
         if (bl.emit_events[i] != 0xFFFFFFFFu) {
             if (bl.emit_events[i] >= c->event_buffers.size()) fail(HNB_ERR_INVALID_ARG, "invalid emit event buffer");
-            P.emit_events[i] = c->event_buffers[bl.emit_events[i]].d;
-            P.emit_events_capacity[i] = c->event_buffers[bl.emit_events[i]].capacity;
+            P.emit_events[i] = c->event_buffers[bl.emit_events[i]].get();
+            P.emit_events_capacity[i] = uint32_t(c->event_buffers[bl.emit_events[i]].size());
         }
     }
     if ((lp.fx->flags & HNB_EFFECT_ORDERED_EVENTS) && (lp.fx->flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS)) {
         if (bi.prefix_sum_count != 1) fail(HNB_ERR_INVALID_ARG, "HNB_EFFECT_ORDERED_EVENTS needs a batch of exactly one instance");
         for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
             if (!P.emit_events[i]) continue;
-            if (!lp.slab->event_counts[i]) {
-                CUDA_CHECK(cudaMalloc((void**)&lp.slab->event_counts[i], size_t(lp.slab->capacity) * 4));
-                CUDA_CHECK(cudaMalloc((void**)&lp.slab->event_block_sums[i], size_t(hnb::ordered_event_blocks(lp.slab->capacity) + 1) * 4));
-            }
-            P.event_counts[i] = lp.slab->event_counts[i];
+            // each allocated when missing: a frame that failed between the two allocations is completed by the next
+            if (!lp.slab->event_counts[i]) CUDA_CHECK(lp.slab->event_counts[i].alloc(lp.slab->capacity));
+            if (!lp.slab->event_block_sums[i]) CUDA_CHECK(lp.slab->event_block_sums[i].alloc(hnb::ordered_event_blocks(lp.slab->capacity) + 1));
+            P.event_counts[i] = lp.slab->event_counts[i].get();
         }
     }
     P.init_thread_count = init_threads;
-    P.debug = c->d_debug;
+    P.debug = c->d_debug.get();
     P.bi_spawner_base = bi.spawner_base;
     P.bi_prefix_sum_offset = bi.prefix_sum_offset;
     P.bi_prefix_sum_count = bi.prefix_sum_count;
@@ -657,16 +603,16 @@ void launch_kernel(hnb_ctx* c, CUfunction f, uint32_t blocks, hnb::BatchParams& 
 
 void launch_update(hnb_ctx* c, LaunchPlan& lp, cudaStream_t st = nullptr) {
     if (!st) st = c->stream;
-    std::pair<cudaEvent_t, cudaEvent_t> ev{};
+    std::pair<Event, Event> ev;
     if (c->timing) {
-        if (!c->ev_free.empty()) { ev = c->ev_free.back(); c->ev_free.pop_back(); }
-        else { CUDA_CHECK(cudaEventCreate(&ev.first)); CUDA_CHECK(cudaEventCreate(&ev.second)); }
+        if (!c->ev_free.empty()) { ev = std::move(c->ev_free.back()); c->ev_free.pop_back(); }
+        else { CUDA_CHECK(ev.first.create(cudaEventDefault)); CUDA_CHECK(ev.second.create(cudaEventDefault)); }
         CUDA_CHECK(cudaEventRecord(ev.first, st));
     }
     launch_kernel(c, lp.fx->km->update, lp.update_blocks, lp.params, lp.fx->update_smem, st);
     if (c->timing) {
         CUDA_CHECK(cudaEventRecord(ev.second, st));
-        c->ev_pending.push_back(ev);
+        c->ev_pending.push_back(std::move(ev));
     }
 }
 
@@ -682,25 +628,23 @@ struct Fork {
         if (launches < 2) return;
         lanes = std::min<uint32_t>(launches, kMaxSideStreams + 1);
         while (c->side_streams.size() < lanes - 1) {
-            cudaStream_t s = nullptr;
-            cudaEvent_t e = nullptr;
-            CUDA_CHECK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-            CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            c->side_streams.push_back(s);
-            c->side_done.push_back(e);
+            SideStream s;
+            CUDA_CHECK(s.stream.create(cudaStreamNonBlocking));
+            CUDA_CHECK(s.done.create(cudaEventDisableTiming));
+            c->side_streams.push_back(std::move(s));
         }
-        if (!c->fork_event) CUDA_CHECK(cudaEventCreateWithFlags(&c->fork_event, cudaEventDisableTiming));
+        if (!c->fork_event) CUDA_CHECK(c->fork_event.create(cudaEventDisableTiming));
         CUDA_CHECK(cudaEventRecord(c->fork_event, c->stream));
-        for (uint32_t i = 0; i + 1 < lanes; ++i) CUDA_CHECK(cudaStreamWaitEvent(c->side_streams[i], c->fork_event, 0));
+        for (uint32_t i = 0; i + 1 < lanes; ++i) CUDA_CHECK(cudaStreamWaitEvent(c->side_streams[i].stream, c->fork_event, 0));
     }
     cudaStream_t lane(uint32_t k) const {
         const uint32_t l = k % lanes;
-        return l == 0 ? c->stream : c->side_streams[l - 1];
+        return l == 0 ? c->stream : c->side_streams[l - 1].stream;
     }
     void join() {
         for (uint32_t i = 0; i + 1 < lanes; ++i) {
-            CUDA_CHECK(cudaEventRecord(c->side_done[i], c->side_streams[i]));
-            CUDA_CHECK(cudaStreamWaitEvent(c->stream, c->side_done[i], 0));
+            CUDA_CHECK(cudaEventRecord(c->side_streams[i].done, c->side_streams[i].stream));
+            CUDA_CHECK(cudaStreamWaitEvent(c->stream, c->side_streams[i].done, 0));
         }
         lanes = 1;
     }
@@ -711,33 +655,26 @@ struct Fork {
 void launch_ribbon_sort(hnb_ctx* c, const LaunchPlan& lp) {
     const hnb_batch_info& bi = c->h_at<hnb_batch_info>(c->lay.off_batch_infos)[lp.batch];
     const bool any_large = lp.slab->capacity > HNB_RIBBON_SORT_SMALL_MAX;
-    if (any_large && c->sort_rows < lp.slab->capacity) {
-        if (c->sort_rows) CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        for (int i = 0; i < 2; ++i) {
-            cudaFree(c->d_sort_keys[i]); cudaFree(c->d_sort_vals[i]);
-            c->d_sort_keys[i] = nullptr; c->d_sort_vals[i] = nullptr;
-        }
-        c->sort_rows = 0;
-        for (int i = 0; i < 2; ++i) {
-            CUDA_CHECK(cudaMalloc((void**)&c->d_sort_keys[i], size_t(lp.slab->capacity) * 8));
-            CUDA_CHECK(cudaMalloc((void**)&c->d_sort_vals[i], size_t(lp.slab->capacity) * 4));
-        }
-        if (!c->d_sort_hist) CUDA_CHECK(cudaMalloc((void**)&c->d_sort_hist, hnb::ribbon_sort_hist_words(uint32_t(c->sm_count)) * 4));
-        c->sort_rows = lp.slab->capacity;
+    if (any_large && c->d_sort_scratch.size() < size_t(lp.slab->capacity) * 3) {
+        CUDA_CHECK(grow(c->d_sort_scratch, size_t(lp.slab->capacity) * 3, 0, c->stream));
+        if (!c->d_sort_hist) CUDA_CHECK(c->d_sort_hist.alloc(hnb::ribbon_sort_hist_words(uint32_t(c->sm_count))));
     }
+    const size_t sort_rows = c->d_sort_scratch.size() / 3;
+    uint64_t* keys = c->d_sort_scratch.get();
+    uint32_t* vals = reinterpret_cast<uint32_t*>(keys + 2 * sort_rows);
     hnb::RibbonSortArgs a{};
     a.planes = plane_set(*lp.slab);
-    a.ping = lp.slab->ping;
-    a.pong = lp.slab->pong;
+    a.ping = lp.slab->ping.get();
+    a.pong = lp.slab->pong.get();
     a.spawners = c->d_at<hnb::Spawner>(c->lay.off_spawners);
-    a.metadata = c->d_metadata;
+    a.metadata = c->d_metadata.get();
     a.spawner_base = bi.spawner_base;
     a.instance_count = bi.prefix_sum_count;
-    for (int i = 0; i < 2; ++i) { a.scratch_keys[i] = (u64*)c->d_sort_keys[i]; a.scratch_vals[i] = c->d_sort_vals[i]; }
-    a.scratch_hist = c->d_sort_hist;
-    a.scratch_rows = c->sort_rows;
+    for (int i = 0; i < 2; ++i) { a.scratch_keys[i] = (u64*)(keys + i * sort_rows); a.scratch_vals[i] = vals + i * sort_rows; }
+    a.scratch_hist = c->d_sort_hist.get();
+    a.scratch_rows = uint32_t(sort_rows);
     a.scratch_grid = uint32_t(c->sm_count);
-    if (any_large) CUDA_CHECK(cudaMemsetAsync(c->d_sort_hist, 0, size_t(2 * 8 * 256) * 4, c->stream));
+    if (any_large) CUDA_CHECK(cudaMemsetAsync(c->d_sort_hist.get(), 0, size_t(2 * 8 * 256) * 4, c->stream));
     clear_ident_claims(c, *lp.slab);  // the sort permutes the column the update just wrote
     uint32_t launched = 0;
     CUDA_CHECK(hnb::launch_ribbon_sort(a, any_large, uint32_t(c->sm_count), c->stream, &launched));
@@ -773,8 +710,8 @@ void check_coverage(hnb_ctx* c, const std::vector<LaunchPlan>& plans) {
     if (c->dirty_tables) {
         const hnb_spawner* sp = c->h_at<hnb_spawner>(c->lay.off_spawners);
         for (uint32_t i = 0; i < c->header()->sim.num_effects; ++i) {
-            if (sp[i].effect_metadata_index >= c->md_rows) fail(HNB_ERR_OUT_OF_RANGE, "spawner row " + std::to_string(i) + ": effect_metadata_index outside the metadata table");
-            if (sp[i].draw_indirect_index >= c->draw_rows) fail(HNB_ERR_OUT_OF_RANGE, "spawner row " + std::to_string(i) + ": draw_indirect_index outside the draw-args table");
+            if (sp[i].effect_metadata_index >= c->d_metadata.size()) fail(HNB_ERR_OUT_OF_RANGE, "spawner row " + std::to_string(i) + ": effect_metadata_index outside the metadata table");
+            if (sp[i].draw_indirect_index >= c->d_draw_args.size()) fail(HNB_ERR_OUT_OF_RANGE, "spawner row " + std::to_string(i) + ": draw_indirect_index outside the draw-args table");
         }
     }
     std::vector<bool> seen(c->B, false);
@@ -820,18 +757,13 @@ int32_t hnb_ctx_create(int32_t cuda_device, uintptr_t external_stream, hnb_ctx**
         CUDA_CHECK(cudaGetDeviceProperties(&prop, cuda_device));
         c->sm_count = prop.multiProcessorCount;
         if (prop.major != 9 || prop.minor != 0) fail(HNB_ERR_NO_DEVICE, "hanabi_b200 kernels are built for sm_90a only; device is sm_" + std::to_string(prop.major * 10 + prop.minor));
-        if (external_stream) {
-            c->stream = (cudaStream_t)external_stream;
-        } else {
-            CUDA_CHECK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-            c->own_stream = true;
-        }
+        if (external_stream) c->stream.borrow((cudaStream_t)external_stream);
+        else CUDA_CHECK(c->stream.create(cudaStreamNonBlocking));
         if (const char* env = getenv("HNB_TILE_CHUNKS")) c->tile_chunks_override = (uint32_t)atoi(env);
         if (const char* env = getenv("HNB_EPOCH_START")) c->epoch = uint32_t(strtoul(env, nullptr, 0)) & 0x3fffffffu;  // tests: start near the wrap
         if (const char* env = getenv("HNB_PARAM_UPLOAD")) c->param_upload = atoi(env) != 0;
         ensure_arena(c.get(), 0, 0);
-        CUDA_CHECK(cudaMalloc((void**)&c->d_debug, kDebugWords * 8));
-        CUDA_CHECK(cudaMemsetAsync(c->d_debug, 0, kDebugWords * 8, c->stream));
+        CUDA_CHECK(grow(c->d_debug, kDebugWords, 0, c->stream));
         *out = c.release();
     });
 }
@@ -840,40 +772,14 @@ void hnb_ctx_destroy(hnb_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
-    for (auto& s : c->slabs) {
-        if (!s.live) continue;
-        for (auto p : s.d_planes) if (p) cudaFree(p);
-        cudaFree(s.ping); cudaFree(s.pong); cudaFree(s.dead); cudaFree(s.alive_bits); cudaFree(s.ident_claim);
-        for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) { cudaFree(s.event_counts[i]); cudaFree(s.event_block_sums[i]); }
-    }
-    for (auto& e : c->effects) if (e.d_props) cudaFree(e.d_props);
-    for (auto& b : c->event_buffers) if (b.d) cudaFree(b.d);
     for (auto& m : c->modules) if (m.second->mod) c->drv.ModuleUnload(m.second->mod);
-    for (auto p : c->d_tile_state) if (p) cudaFree(p);
-    for (auto& ev : c->ev_pending) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
-    for (auto& ev : c->ev_free) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
-    for (auto& sl : c->stage) {
-        if (sl.h) cudaFreeHost(sl.h);
-        if (sl.done) cudaEventDestroy(sl.done);
-    }
-    if (c->h_arena) cudaFreeHost(c->h_arena);
-    if (c->d_arena) cudaFree(c->d_arena);
-    cudaFree(c->d_metadata); cudaFree(c->d_draw_args); cudaFree(c->d_child_infos);
-    cudaFree(c->d_debug);
-    for (auto st : c->side_streams) cudaStreamDestroy(st);
-    for (auto e : c->side_done) cudaEventDestroy(e);
-    if (c->fork_event) cudaEventDestroy(c->fork_event);
-    for (int i = 0; i < 2; ++i) { cudaFree(c->d_sort_keys[i]); cudaFree(c->d_sort_vals[i]); }
-    cudaFree(c->d_sort_hist);
-    cudaFree(c->d_tile_prefix); cudaFree(c->d_dispatch_args); cudaFree(c->d_batch_tiles); cudaFree(c->d_tickets);
-    if (c->own_stream) cudaStreamDestroy(c->stream);
     delete c;
 }
 
 int32_t hnb_sync(hnb_ctx* c) {
     return guarded([&] { CUDA_CHECK(cudaStreamSynchronize(c->stream)); });
 }
-uintptr_t hnb_ctx_stream(hnb_ctx* c) { return (uintptr_t)c->stream; }
+uintptr_t hnb_ctx_stream(hnb_ctx* c) { return (uintptr_t)c->stream.get(); }
 uint64_t hnb_ctx_launch_count(hnb_ctx* c) { return c->launches; }
 void hnb_ctx_frame_count(hnb_ctx* c, uint64_t* frames, uint64_t* frame_block_copies) {
     if (frames) *frames = c->frames;
@@ -893,22 +799,18 @@ int32_t hnb_slab_create_ex(hnb_ctx* c, uint32_t capacity_rows, uint32_t stride, 
         s.stride = stride;
         s.sector_planes = (flags & HNB_SLAB_SECTOR_PLANES) != 0;
         s.planes = physical_planes(stride, s.sector_planes);
-        for (size_t p = 0; p < s.planes.size(); ++p) {
-            CUDA_CHECK(cudaMalloc(&s.d_planes[p], size_t(capacity_rows) * s.planes[p].width));
-            // zero-filled (debug builds of the reference poison the particle buffer instead, effect_cache.rs:284-296)
-            CUDA_CHECK(cudaMemsetAsync(s.d_planes[p], 0, size_t(capacity_rows) * s.planes[p].width, c->stream));
-        }
-        CUDA_CHECK(cudaMalloc((void**)&s.ping, size_t(capacity_rows) * 4));
-        CUDA_CHECK(cudaMalloc((void**)&s.pong, size_t(capacity_rows) * 4));
-        CUDA_CHECK(cudaMalloc((void**)&s.dead, size_t(capacity_rows) * 4));
-        CUDA_CHECK(cudaMalloc((void**)&s.alive_bits, (size_t(capacity_rows) / 32 + 2) * 4));
-        CUDA_CHECK(cudaMemsetAsync(s.alive_bits, 0, (size_t(capacity_rows) / 32 + 2) * 4, c->stream));
-        CUDA_CHECK(cudaMalloc((void**)&s.ident_claim, 2 * sizeof(unsigned long long)));
+        // planes zero-filled (debug builds of the reference poison the particle buffer instead, effect_cache.rs:284-296)
+        for (size_t p = 0; p < s.planes.size(); ++p) CUDA_CHECK(grow(s.d_planes[p], size_t(capacity_rows) * s.planes[p].width, 0, c->stream));
+        CUDA_CHECK(s.ping.alloc(capacity_rows));
+        CUDA_CHECK(s.pong.alloc(capacity_rows));
+        CUDA_CHECK(s.dead.alloc(capacity_rows));
+        CUDA_CHECK(grow(s.alive_bits, size_t(capacity_rows) / 32 + 2, 0, c->stream));
+        CUDA_CHECK(s.ident_claim.alloc(2));
         clear_ident_claims(c, s);
-        CUDA_CHECK(hnb::launch_slab_reset(s.ping, s.pong, s.dead, 0, capacity_rows, c->stream));
+        CUDA_CHECK(hnb::launch_slab_reset(s.ping.get(), s.pong.get(), s.dead.get(), 0, capacity_rows, c->stream));
         c->launches++;
         s.live = true;
-        c->slabs.push_back(s);
+        c->slabs.push_back(std::move(s));
         *out = (hnb_slab)(c->slabs.size() - 1);
     });
 }
@@ -917,15 +819,7 @@ int32_t hnb_slab_destroy(hnb_ctx* c, hnb_slab h) {
     return guarded([&] {
         Slab& s = get_slab(c, h);
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        for (auto& p : s.d_planes) if (p) { cudaFree(p); p = nullptr; }
-        cudaFree(s.ping); cudaFree(s.pong); cudaFree(s.dead); cudaFree(s.alive_bits); cudaFree(s.ident_claim);
-        s.alive_bits = nullptr;
-        s.ident_claim = nullptr;
-        for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
-            cudaFree(s.event_counts[i]); cudaFree(s.event_block_sums[i]);
-            s.event_counts[i] = s.event_block_sums[i] = nullptr;
-        }
-        s.live = false;
+        s = Slab{};  // releases its buffers; live = false, and the handle is never reused
     });
 }
 
@@ -934,8 +828,8 @@ int32_t hnb_slab_reset_rows(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t cou
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
         clear_ident_claims(c, s);
-        CUDA_CHECK(hnb::launch_slab_reset(s.ping, s.pong, s.dead, first, count, c->stream));
-        CUDA_CHECK(hnb::launch_bits_range(s.alive_bits, first, count, false, c->stream));
+        CUDA_CHECK(hnb::launch_slab_reset(s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
+        CUDA_CHECK(hnb::launch_bits_range(s.alive_bits.get(), first, count, false, c->stream));
         c->launches += 2;
     });
 }
@@ -945,50 +839,47 @@ int32_t hnb_slab_rebuild_alive_bits(hnb_ctx* c, hnb_slab h, uint32_t first, uint
         Slab& s = get_slab(c, h);
         check_rows(s, first, rows);
         if (column > 1 || alive_count > rows) fail(HNB_ERR_INVALID_ARG, "bad alive-list column or count");
-        CUDA_CHECK(hnb::launch_bits_range(s.alive_bits, first, rows, false, c->stream));
-        CUDA_CHECK(hnb::launch_bits_from_list(s.alive_bits, (column ? s.pong : s.ping) + first, first, alive_count, c->stream));
+        CUDA_CHECK(hnb::launch_bits_range(s.alive_bits.get(), first, rows, false, c->stream));
+        CUDA_CHECK(hnb::launch_bits_from_list(s.alive_bits.get(), (column ? s.pong : s.ping).get() + first, first, alive_count, c->stream));
         c->launches += rows ? 1 + (alive_count ? 1 : 0) : 0;
     });
 }
 
-int32_t hnb_slab_upload_aos(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, const void* aos) {
-    return guarded([&] {
-        Slab& s = get_slab(c, h);
-        check_rows(s, first, count);
-        if (count == 0) return;
-        const uint32_t rows_per_chunk = (uint32_t)std::max<size_t>(1, kChunkBytes / s.stride);
-        uint32_t* stage = nullptr;
-        CUDA_CHECK(cudaMalloc((void**)&stage, size_t(std::min(rows_per_chunk, count)) * s.stride));
-        hnb::PlaneSet ps = plane_set(s);
-        for (uint32_t done = 0; done < count; done += rows_per_chunk) {
-            uint32_t n = std::min(rows_per_chunk, count - done);
-            CUDA_CHECK(cudaMemcpyAsync(stage, (const char*)aos + size_t(done) * s.stride, size_t(n) * s.stride, cudaMemcpyHostToDevice, c->stream));
+namespace {
+// AoS records <-> the slab's planes through a device staging buffer, chunk by chunk: on upload the host records are
+// copied up (and only read) and transposed into the planes, on download the planes are transposed and copied down.
+void transfer_aos(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, void* host, bool upload) {
+    Slab& s = get_slab(c, h);
+    check_rows(s, first, count);
+    if (count == 0) return;
+    const uint32_t rows_per_chunk = (uint32_t)std::max<size_t>(1, kChunkBytes / s.stride);
+    DeviceArray<char> staging;
+    CUDA_CHECK(staging.alloc(size_t(std::min(rows_per_chunk, count)) * s.stride));
+    uint32_t* stage = reinterpret_cast<uint32_t*>(staging.get());
+    hnb::PlaneSet ps = plane_set(s);
+    for (uint32_t done = 0; done < count; done += rows_per_chunk) {
+        uint32_t n = std::min(rows_per_chunk, count - done);
+        const size_t at = size_t(done) * s.stride, bytes = size_t(n) * s.stride;
+        if (upload) {
+            CUDA_CHECK(cudaMemcpyAsync(stage, (const char*)host + at, bytes, cudaMemcpyHostToDevice, c->stream));
             CUDA_CHECK(hnb::launch_aos_to_planes(stage, ps, first + done, n, s.stride / 4, c->stream));
             c->launches++;
-            CUDA_CHECK(cudaStreamSynchronize(c->stream));
+        } else {
+            CUDA_CHECK(hnb::launch_planes_to_aos(stage, ps, first + done, n, s.stride / 4, c->stream));
+            c->launches++;
+            CUDA_CHECK(cudaMemcpyAsync((char*)host + at, stage, bytes, cudaMemcpyDeviceToHost, c->stream));
         }
-        cudaFree(stage);
-    });
+        CUDA_CHECK(cudaStreamSynchronize(c->stream));
+    }
+}
+}  // namespace
+
+int32_t hnb_slab_upload_aos(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, const void* aos) {
+    return guarded([&] { transfer_aos(c, h, first, count, const_cast<void*>(aos), true); });
 }
 
 int32_t hnb_slab_download_aos(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, void* aos) {
-    return guarded([&] {
-        Slab& s = get_slab(c, h);
-        check_rows(s, first, count);
-        if (count == 0) return;
-        const uint32_t rows_per_chunk = (uint32_t)std::max<size_t>(1, kChunkBytes / s.stride);
-        uint32_t* stage = nullptr;
-        CUDA_CHECK(cudaMalloc((void**)&stage, size_t(std::min(rows_per_chunk, count)) * s.stride));
-        hnb::PlaneSet ps = plane_set(s);
-        for (uint32_t done = 0; done < count; done += rows_per_chunk) {
-            uint32_t n = std::min(rows_per_chunk, count - done);
-            CUDA_CHECK(hnb::launch_planes_to_aos(stage, ps, first + done, n, s.stride / 4, c->stream));
-            c->launches++;
-            CUDA_CHECK(cudaMemcpyAsync((char*)aos + size_t(done) * s.stride, stage, size_t(n) * s.stride, cudaMemcpyDeviceToHost, c->stream));
-            CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        }
-        cudaFree(stage);
-    });
+    return guarded([&] { transfer_aos(c, h, first, count, aos, false); });
 }
 
 int32_t hnb_slab_upload_indirect(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, const hnb_indirect_index* rows) {
@@ -996,14 +887,13 @@ int32_t hnb_slab_upload_indirect(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
         if (count == 0) return;
-        uint32_t* stage = nullptr;
-        CUDA_CHECK(cudaMalloc((void**)&stage, size_t(count) * 12));
-        CUDA_CHECK(cudaMemcpyAsync(stage, rows, size_t(count) * 12, cudaMemcpyHostToDevice, c->stream));
+        DeviceArray<uint32_t> stage;
+        CUDA_CHECK(stage.alloc(size_t(count) * 3));
+        CUDA_CHECK(cudaMemcpyAsync(stage.get(), rows, size_t(count) * 12, cudaMemcpyHostToDevice, c->stream));
         clear_ident_claims(c, s);
-        CUDA_CHECK(hnb::launch_indirect_deinterleave(stage, s.ping, s.pong, s.dead, first, count, c->stream));
+        CUDA_CHECK(hnb::launch_indirect_deinterleave(stage.get(), s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
         c->launches++;
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        cudaFree(stage);
     });
 }
 
@@ -1012,13 +902,12 @@ int32_t hnb_slab_download_indirect(hnb_ctx* c, hnb_slab h, uint32_t first, uint3
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
         if (count == 0) return;
-        uint32_t* stage = nullptr;
-        CUDA_CHECK(cudaMalloc((void**)&stage, size_t(count) * 12));
-        CUDA_CHECK(hnb::launch_indirect_interleave(stage, s.ping, s.pong, s.dead, first, count, c->stream));
+        DeviceArray<uint32_t> stage;
+        CUDA_CHECK(stage.alloc(size_t(count) * 3));
+        CUDA_CHECK(hnb::launch_indirect_interleave(stage.get(), s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
         c->launches++;
-        CUDA_CHECK(cudaMemcpyAsync(rows, stage, size_t(count) * 12, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_CHECK(cudaMemcpyAsync(rows, stage.get(), size_t(count) * 12, cudaMemcpyDeviceToHost, c->stream));
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        cudaFree(stage);
     });
 }
 
@@ -1050,7 +939,7 @@ int32_t hnb_slab_export_indirect_device(hnb_ctx* c, hnb_slab h, uint32_t first, 
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
         if (count && !d_dst) fail(HNB_ERR_INVALID_ARG, "d_dst is NULL");
-        CUDA_CHECK(hnb::launch_indirect_interleave((uint32_t*)d_dst, s.ping, s.pong, s.dead, first, count, c->stream));
+        CUDA_CHECK(hnb::launch_indirect_interleave((uint32_t*)d_dst, s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
         c->launches += count ? 1 : 0;
     });
 }
@@ -1060,7 +949,7 @@ int32_t hnb_slab_import_indirect_device(hnb_ctx* c, hnb_slab h, uint32_t first, 
         check_rows(s, first, count);
         if (count && !d_src) fail(HNB_ERR_INVALID_ARG, "d_src is NULL");
         clear_ident_claims(c, s);
-        CUDA_CHECK(hnb::launch_indirect_deinterleave((const uint32_t*)d_src, s.ping, s.pong, s.dead, first, count, c->stream));
+        CUDA_CHECK(hnb::launch_indirect_deinterleave((const uint32_t*)d_src, s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
         c->launches += count ? 1 : 0;
     });
 }
@@ -1073,13 +962,13 @@ int32_t hnb_slab_device_view(hnb_ctx* c, hnb_slab h, hnb_slab_view* out) {
         out->particle_stride = s.stride;
         out->num_planes = (uint32_t)s.planes.size();
         for (size_t p = 0; p < s.planes.size(); ++p) {
-            out->planes[p] = s.d_planes[p];
+            out->planes[p] = s.d_planes[p].get();
             out->plane_offset[p] = s.planes[p].offset;
             out->plane_width[p] = s.planes[p].width;
         }
-        out->ping = s.ping;
-        out->pong = s.pong;
-        out->dead = s.dead;
+        out->ping = s.ping.get();
+        out->pong = s.pong.get();
+        out->dead = s.dead.get();
     });
 }
 void* hnb_device_alloc(hnb_ctx* c, size_t bytes) {
@@ -1119,8 +1008,9 @@ int32_t hnb_slab_fill_c5_ex(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t cou
         check_rows(s, first, count);
         if (s.stride != 32) fail(HNB_ERR_LAYOUT, "hnb_slab_fill_c5 needs the 32-byte {position,age,velocity,lifetime} layout");
         if (s.sector_planes) fail(HNB_ERR_LAYOUT, "hnb_slab_fill_c5 writes the default plane layout; spawn through the init pass or use hnb_slab_upload_aos");
-        CUDA_CHECK(hnb::launch_fill_c5(s.d_planes[0], s.d_planes[1], s.ping, s.pong, s.ident_claim, first, count, seed, lo, hi, logical_first, c->stream));
-        CUDA_CHECK(hnb::launch_bits_range(s.alive_bits, first, count, true, c->stream));
+        CUDA_CHECK(hnb::launch_fill_c5(s.d_planes[0].get(), s.d_planes[1].get(), s.ping.get(), s.pong.get(), s.ident_claim.get(), first, count, seed, lo, hi,
+                                       logical_first, c->stream));
+        CUDA_CHECK(hnb::launch_bits_range(s.alive_bits.get(), first, count, true, c->stream));
         c->launches += 2;
     });
 }
@@ -1134,13 +1024,39 @@ void check_instance_slice(hnb_ctx* c, const Slab& s, const Effect& fx, uint32_t 
                           const char* what) {
     const std::string w = what;
     if (uint64_t(first) + rows > s.capacity) fail(HNB_ERR_INVALID_ARG, w + ": rows outside the slab");
-    if (metadata_row >= c->md_rows) fail(HNB_ERR_INVALID_ARG, w + ": metadata row out of range");
+    if (metadata_row >= c->d_metadata.size()) fail(HNB_ERR_INVALID_ARG, w + ": metadata row out of range");
     if (fx.particle_stride != s.stride) fail(HNB_ERR_INVALID_ARG, w + ": effect particle stride does not match the slab");
     if (((fx.flags & HNB_EFFECT_SECTOR_PLANES) != 0) != s.sector_planes)
         fail(HNB_ERR_INVALID_ARG, w + ": effect and slab disagree on HNB_EFFECT_SECTOR_PLANES / HNB_SLAB_SECTOR_PLANES");
     if (fx.flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS)
         fail(HNB_ERR_INVALID_ARG, w + ": pending GPU spawn events name parent slots; an emitting effect cannot be " +
                                       (w == "hnb_slab_repack" ? "repacked" : "snapshot or restored"));
+}
+
+hnb::RepackArgs repack_args(hnb_ctx* c, const Slab& s, uint32_t metadata_row, uint32_t first, uint32_t rows) {
+    hnb::RepackArgs a{};
+    a.metadata = c->d_metadata.get() + metadata_row;
+    a.ping = s.ping.get();
+    a.pong = s.pong.get();
+    a.dead = s.dead.get();
+    a.alive_bits = s.alive_bits.get();
+    a.claim = s.ident_claim.get();
+    a.first = first;
+    a.rows = rows;
+    return a;
+}
+
+hnb::SnapshotArgs snapshot_args(hnb_ctx* c, const Slab& s, uint32_t metadata_row, uint32_t first, uint32_t rows) {
+    hnb::SnapshotArgs a{};
+    a.metadata = c->d_metadata.get() + metadata_row;
+    a.ping = s.ping.get();
+    a.pong = s.pong.get();
+    a.planes = plane_set(s);
+    a.num_planes = (uint32_t)s.planes.size();
+    a.stride_words = s.stride / 4;
+    a.first = first;
+    a.rows = rows;
+    return a;
 }
 }  // namespace
 
@@ -1151,15 +1067,7 @@ int32_t hnb_slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_
         check_instance_slice(c, s, fx, metadata_row, first, rows, "hnb_slab_repack");
         if (rows == 0) return;
         CUDA_CHECK(cudaSetDevice(c->device));
-        hnb::RepackArgs a{};
-        a.metadata = c->d_metadata + metadata_row;
-        a.ping = s.ping;
-        a.pong = s.pong;
-        a.dead = s.dead;
-        a.alive_bits = s.alive_bits;
-        a.claim = s.ident_claim;
-        a.first = first;
-        a.rows = rows;
+        const hnb::RepackArgs a = repack_args(c, s, metadata_row, first, rows);
         uint32_t widest = 0;
         for (const Plane& p : s.planes) widest = std::max(widest, p.width);
         void* scratch = nullptr;
@@ -1167,9 +1075,9 @@ int32_t hnb_slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_
         cudaError_t err = cudaSuccess;
         for (size_t p = 0; p < s.planes.size() && err == cudaSuccess; ++p) {
             const uint32_t width = s.planes[p].width;
-            err = hnb::launch_repack_gather(a, s.d_planes[p], scratch, width, c->stream);
+            err = hnb::launch_repack_gather(a, s.d_planes[p].get(), scratch, width, c->stream);
             if (err == cudaSuccess)
-                err = cudaMemcpyAsync((char*)s.d_planes[p] + size_t(first) * width, scratch, size_t(rows) * width, cudaMemcpyDeviceToDevice, c->stream);
+                err = cudaMemcpyAsync(s.d_planes[p].get() + size_t(first) * width, scratch, size_t(rows) * width, cudaMemcpyDeviceToDevice, c->stream);
             c->launches++;
         }
         // the lists last: every gather reads them
@@ -1188,21 +1096,6 @@ static_assert(HNB_SNAPSHOT_MAGIC == HNB_SNAPSHOT_MAGIC_WORD && HNB_SNAPSHOT_VERS
 size_t hnb_instance_snapshot_bytes(uint32_t particle_stride, uint32_t rows) {
     return sizeof(hnb_instance_snapshot_header) + size_t(rows) * particle_stride;
 }
-
-namespace {
-hnb::SnapshotArgs snapshot_args(hnb_ctx* c, const Slab& s, uint32_t metadata_row, uint32_t first, uint32_t rows) {
-    hnb::SnapshotArgs a{};
-    a.metadata = c->d_metadata + metadata_row;
-    a.ping = s.ping;
-    a.pong = s.pong;
-    a.planes = plane_set(s);
-    a.num_planes = (uint32_t)s.planes.size();
-    a.stride_words = s.stride / 4;
-    a.first = first;
-    a.rows = rows;
-    return a;
-}
-}  // namespace
 
 // One launch: the kernel reads n, W and particle_counter on the device, so the host never waits for them.
 int32_t hnb_instance_snapshot(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
@@ -1237,16 +1130,7 @@ int32_t hnb_instance_restore(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t meta
         a.src_bytes = src_bytes;
         CUDA_CHECK(hnb::launch_restore_scatter(a, (const uint32_t*)d_src, c->stream));
         c->launches++;
-        hnb::RepackArgs r{};
-        r.metadata = a.metadata;
-        r.ping = s.ping;
-        r.pong = s.pong;
-        r.dead = s.dead;
-        r.alive_bits = s.alive_bits;
-        r.claim = s.ident_claim;
-        r.first = first;
-        r.rows = rows;
-        CUDA_CHECK(hnb::launch_repack_lists(r, c->stream));
+        CUDA_CHECK(hnb::launch_repack_lists(repack_args(c, s, metadata_row, first, rows), c->stream));
         c->launches++;
     });
 }
@@ -1255,18 +1139,23 @@ int32_t hnb_slab_checksum(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count
     return hnb_slab_checksum_ex(c, h, first, count, 0, out);
 }
 
+namespace {
+// Hashes rows [first, first + count) of the columns `ps` (`words` per row) on the device into `out`, and waits.
+void checksum(hnb_ctx* c, const hnb::PlaneSet& ps, uint32_t first, uint32_t count, uint32_t words, uint64_t index_base, uint64_t* out) {
+    DeviceArray<unsigned long long> d;
+    CUDA_CHECK(d.alloc(1));
+    CUDA_CHECK(cudaMemsetAsync(d.get(), 0, 8, c->stream));
+    CUDA_CHECK(hnb::launch_checksum(ps, first, count, words, index_base, d.get(), c->stream));
+    c->launches++;
+    read_back(c, out, d.get(), 8);
+}
+}  // namespace
+
 int32_t hnb_slab_checksum_ex(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, uint64_t index_base, uint64_t* out) {
     return guarded([&] {
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
-        unsigned long long* d = nullptr;
-        CUDA_CHECK(cudaMalloc((void**)&d, 8));
-        CUDA_CHECK(cudaMemsetAsync(d, 0, 8, c->stream));
-        CUDA_CHECK(hnb::launch_checksum(plane_set(s), first, count, s.stride / 4, index_base, d, c->stream));
-        c->launches++;
-        CUDA_CHECK(cudaMemcpyAsync(out, d, 8, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        cudaFree(d);
+        checksum(c, plane_set(s), first, count, s.stride / 4, index_base, out);
     });
 }
 
@@ -1276,21 +1165,14 @@ int32_t hnb_slab_checksum_indirect(hnb_ctx* c, hnb_slab h, uint32_t first, uint3
         check_rows(s, first, count);
         // hash the rows as the reference's interleaved IndirectEntry {ping, pong, dead}
         hnb::PlaneSet ps{};
-        uint32_t* cols[3] = {s.ping, s.pong, s.dead};
+        uint32_t* cols[3] = {s.ping.get(), s.pong.get(), s.dead.get()};
         for (int p = 0; p < 3; ++p) {
             ps.ptr[p] = cols[p];
             ps.words[p] = 1;
             ps.word_off[p] = (uint32_t)p;
             ps.word_to_plane[p] = (unsigned char)p;
         }
-        unsigned long long* d = nullptr;
-        CUDA_CHECK(cudaMalloc((void**)&d, 8));
-        CUDA_CHECK(cudaMemsetAsync(d, 0, 8, c->stream));
-        CUDA_CHECK(hnb::launch_checksum(ps, first, count, 3, 0, d, c->stream));
-        c->launches++;
-        CUDA_CHECK(cudaMemcpyAsync(out, d, 8, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        cudaFree(d);
+        checksum(c, ps, first, count, 3, 0, out);
     });
 }
 
@@ -1366,7 +1248,7 @@ static hnb_effect install_effect(hnb_ctx* c, const EffectBlueprint& bp, const st
     fx.props_size = bp.props_size;
     fx.props_stride = (uint32_t)align_up(bp.props_size, 16);
     fx.live = true;
-    c->effects.push_back(fx);
+    c->effects.push_back(std::move(fx));
     return (hnb_effect)(c->effects.size() - 1);
 }
 
@@ -1439,8 +1321,7 @@ int32_t hnb_effect_destroy(hnb_ctx* c, hnb_effect h) {
     return guarded([&] {
         Effect& fx = get_effect(c, h);
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        if (fx.d_props) cudaFree(fx.d_props);
-        fx.d_props = nullptr;
+        fx.d_props.reset();
         fx.live = false;  // the compiled module stays in the cache (ShaderCache never evicts either)
     });
 }
@@ -1450,20 +1331,12 @@ int32_t hnb_upload_properties(hnb_ctx* c, hnb_effect h, uint32_t array_index, co
         Effect& fx = get_effect(c, h);
         if (fx.props_size == 0) fail(HNB_ERR_INVALID_ARG, "effect has no properties");
         if (bytes != fx.props_size) fail(HNB_ERR_LAYOUT, "property blob size does not match the effect's PropertyLayout");
-        if (array_index >= fx.props_rows) {
-            uint32_t cap = std::max<uint32_t>(array_index + 1, std::max<uint32_t>(fx.props_rows * 2, 4));
-            char* np = nullptr;
-            CUDA_CHECK(cudaMalloc((void**)&np, size_t(cap) * fx.props_stride));
-            CUDA_CHECK(cudaMemsetAsync(np, 0, size_t(cap) * fx.props_stride, c->stream));
-            if (fx.d_props) {
-                CUDA_CHECK(cudaMemcpyAsync(np, fx.d_props, size_t(fx.props_rows) * fx.props_stride, cudaMemcpyDeviceToDevice, c->stream));
-                CUDA_CHECK(cudaStreamSynchronize(c->stream));
-                cudaFree(fx.d_props);
-            }
-            fx.d_props = np;
-            fx.props_rows = cap;
+        const uint32_t rows = uint32_t(fx.d_props.size() / fx.props_stride);
+        if (array_index >= rows) {
+            uint32_t cap = std::max<uint32_t>(array_index + 1, std::max<uint32_t>(rows * 2, 4));
+            CUDA_CHECK(grow(fx.d_props, size_t(cap) * fx.props_stride, fx.d_props.size(), c->stream));
         }
-        CUDA_CHECK(cudaMemcpyAsync(fx.d_props + size_t(array_index) * fx.props_stride, blob, bytes, cudaMemcpyHostToDevice, c->stream));
+        CUDA_CHECK(cudaMemcpyAsync(fx.d_props.get() + size_t(array_index) * fx.props_stride, blob, bytes, cudaMemcpyHostToDevice, c->stream));
         CUDA_CHECK(cudaStreamSynchronize(c->stream));  // blob is pageable caller memory
     });
 }
@@ -1480,14 +1353,14 @@ int32_t hnb_upload_spawners(hnb_ctx* c, const hnb_spawner* rows, uint32_t n) {
     return guarded([&] {
         if (n && !rows) fail(HNB_ERR_INVALID_ARG, "rows is NULL");
         const uint32_t old_e = c->E, old_b = c->B;
-        const char* const old_arena = c->h_arena;
+        const char* const old_arena = c->h_arena.get();
         ensure_arena(c, n, c->B);
         // A host that uploads its tables every frame whether they changed or not (the reference does: mod.rs:4679-4705) should not
         // pay for it: identical rows over an unchanged layout leave the frame a header-only frame.
-        if (old_arena == c->h_arena && old_e == c->E && old_b == c->B && n &&
-            memcmp(c->h_arena + c->lay.off_spawners, rows, size_t(n) * sizeof(hnb_spawner)) == 0)
+        if (old_arena == c->h_arena.get() && old_e == c->E && old_b == c->B && n &&
+            memcmp(c->h_arena.get() + c->lay.off_spawners, rows, size_t(n) * sizeof(hnb_spawner)) == 0)
             return;
-        memcpy(c->h_arena + c->lay.off_spawners, rows, size_t(n) * sizeof(hnb_spawner));
+        memcpy(c->h_arena.get() + c->lay.off_spawners, rows, size_t(n) * sizeof(hnb_spawner));
         c->dirty_tables = true;
     });
 }
@@ -1496,17 +1369,17 @@ int32_t hnb_upload_batches(hnb_ctx* c, const hnb_batch_info* rows, uint32_t nb, 
     return guarded([&] {
         if ((nb && !rows) || (np && !prefix)) fail(HNB_ERR_INVALID_ARG, "NULL table");
         const uint32_t old_e = c->E, old_b = c->B;
-        const char* const old_arena = c->h_arena;
+        const char* const old_arena = c->h_arena.get();
         ensure_arena(c, std::max(c->E, np), nb);
         if (np > c->E) fail(HNB_ERR_OUT_OF_RANGE, "more prefix entries than instances");
-        if (old_arena == c->h_arena && old_e == c->E && old_b == c->B && nb &&
-            memcmp(c->h_arena + c->lay.off_batch_infos, rows, size_t(nb) * sizeof(hnb_batch_info)) == 0 &&
-            (np == 0 || memcmp(c->h_arena + c->lay.off_spawn_prefix, prefix, size_t(np) * 4) == 0))
+        if (old_arena == c->h_arena.get() && old_e == c->E && old_b == c->B && nb &&
+            memcmp(c->h_arena.get() + c->lay.off_batch_infos, rows, size_t(nb) * sizeof(hnb_batch_info)) == 0 &&
+            (np == 0 || memcmp(c->h_arena.get() + c->lay.off_spawn_prefix, prefix, size_t(np) * 4) == 0))
             return;  // unchanged (see hnb_upload_spawners); the per-frame spawn ranges are recomputed by every launch plan
-        memcpy(c->h_arena + c->lay.off_batch_infos, rows, size_t(nb) * sizeof(hnb_batch_info));
-        memcpy(c->h_arena + c->lay.off_spawn_prefix, prefix, size_t(np) * 4);
-        memcpy(c->h_arena + c->lay.off_prefix_sum, prefix, size_t(np) * 4);  // same buffer in the reference (batch.rs:194-216)
-        memset(c->h_arena + c->lay.off_range, 0, size_t(c->E) * 4);
+        memcpy(c->h_arena.get() + c->lay.off_batch_infos, rows, size_t(nb) * sizeof(hnb_batch_info));
+        memcpy(c->h_arena.get() + c->lay.off_spawn_prefix, prefix, size_t(np) * 4);
+        memcpy(c->h_arena.get() + c->lay.off_prefix_sum, prefix, size_t(np) * 4);  // same buffer in the reference (batch.rs:194-216)
+        memset(c->h_arena.get() + c->lay.off_range, 0, size_t(c->E) * 4);
         c->dirty_tables = true;
     });
 }
@@ -1515,8 +1388,9 @@ int32_t hnb_metadata_insert(hnb_ctx* c, uint32_t row, const hnb_effect_metadata*
     return guarded([&] {
         if (!md) fail(HNB_ERR_INVALID_ARG, "md is NULL");
         c->md_generation++;
-        grow_device(c->d_metadata, c->md_rows, row + 1, c->stream);
-        CUDA_CHECK(cudaMemcpyAsync(c->d_metadata + row, md, sizeof(*md), cudaMemcpyHostToDevice, c->stream));
+        const uint32_t rows = uint32_t(c->d_metadata.size());
+        if (row + 1 > rows) CUDA_CHECK(grow(c->d_metadata, std::max<uint32_t>(row + 1, std::max<uint32_t>(rows * 2, 16)), rows, c->stream));
+        CUDA_CHECK(cudaMemcpyAsync(c->d_metadata.get() + row, md, sizeof(*md), cudaMemcpyHostToDevice, c->stream));
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
     });
 }
@@ -1524,14 +1398,9 @@ int32_t hnb_metadata_insert(hnb_ctx* c, uint32_t row, const hnb_effect_metadata*
 int32_t hnb_draw_args_insert(hnb_ctx* c, uint32_t row, const hnb_draw_indexed_indirect_args* a) {
     return guarded([&] {
         if (!a) fail(HNB_ERR_INVALID_ARG, "args is NULL");
-        uint32_t words = c->draw_rows * 5;
-        if (row >= c->draw_rows) {
-            uint32_t need_rows = std::max<uint32_t>(row + 1, std::max<uint32_t>(c->draw_rows * 2, 16));
-            uint32_t need_words = need_rows * 5;
-            grow_device(c->d_draw_args, words, need_words, c->stream);
-            c->draw_rows = words / 5;
-        }
-        CUDA_CHECK(cudaMemcpyAsync(c->d_draw_args + size_t(row) * 5, a, sizeof(*a), cudaMemcpyHostToDevice, c->stream));
+        const uint32_t rows = uint32_t(c->d_draw_args.size());
+        if (row >= rows) CUDA_CHECK(grow(c->d_draw_args, std::max<uint32_t>(row + 1, std::max<uint32_t>(rows * 2, 16)), rows, c->stream));
+        CUDA_CHECK(cudaMemcpyAsync(c->d_draw_args.get() + row, a, sizeof(*a), cudaMemcpyHostToDevice, c->stream));
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
     });
 }
@@ -1539,11 +1408,9 @@ int32_t hnb_draw_args_insert(hnb_ctx* c, uint32_t row, const hnb_draw_indexed_in
 int32_t hnb_event_buffer_create(hnb_ctx* c, uint32_t capacity, hnb_event_buffer* out) {
     return guarded([&] {
         if (!out || !capacity) fail(HNB_ERR_INVALID_ARG, "bad event buffer arguments");
-        EventBuffer b;
-        b.capacity = capacity;
-        CUDA_CHECK(cudaMalloc((void**)&b.d, size_t(capacity) * 4));
-        CUDA_CHECK(cudaMemsetAsync(b.d, 0, size_t(capacity) * 4, c->stream));
-        c->event_buffers.push_back(b);
+        DeviceArray<uint32_t> b;
+        CUDA_CHECK(grow(b, capacity, 0, c->stream));
+        c->event_buffers.push_back(std::move(b));
         *out = (hnb_event_buffer)(c->event_buffers.size() - 1);
     });
 }
@@ -1551,32 +1418,18 @@ int32_t hnb_event_buffer_create(hnb_ctx* c, uint32_t capacity, hnb_event_buffer*
 int32_t hnb_child_info_insert(hnb_ctx* c, uint32_t row, const hnb_child_info* info) {
     return guarded([&] {
         if (!info) fail(HNB_ERR_INVALID_ARG, "info is NULL");
-        uint32_t rows = c->child_rows;
-        // child_rows tracks the logical array length (arrayLength() in vfx_indirect.wgsl:43)
-        uint32_t cap = c->child_rows;
-        if (row >= cap) {
-            hnb::ChildInfo* np = nullptr;
-            uint32_t ncap = row + 1;
-            CUDA_CHECK(cudaMalloc((void**)&np, size_t(ncap) * sizeof(hnb::ChildInfo)));
-            CUDA_CHECK(cudaMemsetAsync(np, 0, size_t(ncap) * sizeof(hnb::ChildInfo), c->stream));
-            if (c->d_child_infos) {
-                CUDA_CHECK(cudaMemcpyAsync(np, c->d_child_infos, size_t(rows) * sizeof(hnb::ChildInfo), cudaMemcpyDeviceToDevice, c->stream));
-                CUDA_CHECK(cudaStreamSynchronize(c->stream));
-                cudaFree(c->d_child_infos);
-            }
-            c->d_child_infos = np;
-            c->child_rows = ncap;
-        }
-        CUDA_CHECK(cudaMemcpyAsync(c->d_child_infos + row, info, sizeof(*info), cudaMemcpyHostToDevice, c->stream));
+        // the table is exactly as long as the logical array (arrayLength() in vfx_indirect.wgsl:43)
+        const uint32_t rows = uint32_t(c->d_child_infos.size());
+        if (row >= rows) CUDA_CHECK(grow(c->d_child_infos, row + 1, rows, c->stream));
+        CUDA_CHECK(cudaMemcpyAsync(c->d_child_infos.get() + row, info, sizeof(*info), cudaMemcpyHostToDevice, c->stream));
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
     });
 }
 
 int32_t hnb_read_child_info(hnb_ctx* c, uint32_t row, hnb_child_info* out) {
     return guarded([&] {
-        if (row >= c->child_rows) fail(HNB_ERR_OUT_OF_RANGE, "child info row out of range");
-        CUDA_CHECK(cudaMemcpyAsync(out, c->d_child_infos + row, sizeof(*out), cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
+        if (row >= c->d_child_infos.size()) fail(HNB_ERR_OUT_OF_RANGE, "child info row out of range");
+        read_back(c, out, c->d_child_infos.get() + row, sizeof(*out));
     });
 }
 
@@ -1584,9 +1437,8 @@ int32_t hnb_event_buffer_download(hnb_ctx* c, hnb_event_buffer h, uint32_t first
     return guarded([&] {
         if (h >= c->event_buffers.size()) fail(HNB_ERR_INVALID_ARG, "invalid event buffer");
         auto& b = c->event_buffers[h];
-        if (uint64_t(first) + count > b.capacity) fail(HNB_ERR_OUT_OF_RANGE, "event range out of bounds");
-        CUDA_CHECK(cudaMemcpyAsync(out, b.d + first, size_t(count) * 4, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
+        if (uint64_t(first) + count > b.size()) fail(HNB_ERR_OUT_OF_RANGE, "event range out of bounds");
+        read_back(c, out, b.get() + first, size_t(count) * 4);
     });
 }
 
@@ -1618,7 +1470,7 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
         // with an init pass the block needs a (one-CTA) kernel of its own at the head of the frame: init reads the tables first
         const bool block_kernel = param_block && any_init;
         if (block_kernel) {
-            CUDA_CHECK(hnb::launch_frame_block(c->d_arena, c->h_arena, uint32_t(c->lay.off_prefix_sum), c->stream));
+            CUDA_CHECK(hnb::launch_frame_block(c->d_arena.get(), c->h_arena.get(), uint32_t(c->lay.off_prefix_sum), c->stream));
             c->launches++;
             for (auto& lp : plans) lp.params.late_tables = 1u;
         }
@@ -1648,12 +1500,12 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
             PassRange range("hanabi:indirect_dispatch");  // + "hanabi:update_prefix_sum"
             const void* block = nullptr;   // what rides in the kernel's parameter space: nothing / the 64-byte header / header + tables
             uint32_t block_bytes = 0;
-            if (param_block && !block_kernel) { block = c->h_arena; block_bytes = uint32_t(c->lay.off_prefix_sum); }
+            if (param_block && !block_kernel) { block = c->h_arena.get(); block_bytes = uint32_t(c->lay.off_prefix_sum); }
             else if (block_kernel) { /* already stored by k_frame_block, header included */ }
             else if (!copy_block) { block = c->header(); block_bytes = uint32_t(sizeof(hnb::FrameHeader)); }
             CUDA_CHECK(hnb::launch_bookkeeping(static_tables(c), c->header()->sim.num_effects, c->B, block, block_bytes, c->stream));
             if (param_block && !block_kernel) { c->dirty_tables = false; c->plan_dirty = false; }  // the tables went with this launch
-            c->launches += 1 + (c->child_rows ? 1 : 0);
+            c->launches += 1 + (c->d_child_infos.size() ? 1 : 0);
             std::fill(c->init_pending.begin(), c->init_pending.end(), 0);
         }
         // pass "hanabi:update" (mod.rs:7280-7370): batches are independent (event appends are atomic)
@@ -1670,17 +1522,17 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
             if (!(lp.fx->flags & HNB_EFFECT_ORDERED_EVENTS) || !(lp.fx->flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS)) continue;
             const hnb_batch_info& bi = c->h_at<hnb_batch_info>(c->lay.off_batch_infos)[lp.batch];
             const hnb_spawner& sp = c->h_at<hnb_spawner>(c->lay.off_spawners)[bi.spawner_base];
-            if (sp.effect_metadata_index >= c->md_rows) fail(HNB_ERR_OUT_OF_RANGE, "spawner row points outside the metadata table");
+            if (sp.effect_metadata_index >= c->d_metadata.size()) fail(HNB_ERR_OUT_OF_RANGE, "spawner row points outside the metadata table");
             for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
                 if (!lp.params.event_counts[i]) continue;
                 hnb::EventAppendArgs a{};
                 a.counts = lp.params.event_counts[i];
-                a.ping = lp.slab->ping;
-                a.pong = lp.slab->pong;
+                a.ping = lp.slab->ping.get();
+                a.pong = lp.slab->pong.get();
                 a.spawner = c->d_at<hnb::Spawner>(c->lay.off_spawners) + bi.spawner_base;
-                a.metadata = c->d_metadata + sp.effect_metadata_index;
-                a.block_sums = lp.slab->event_block_sums[i];
-                a.child_infos = c->d_child_infos;
+                a.metadata = c->d_metadata.get() + sp.effect_metadata_index;
+                a.block_sums = lp.slab->event_block_sums[i].get();
+                a.child_infos = c->d_child_infos.get();
                 a.binding = uint32_t(i);
                 a.buffer = lp.params.emit_events[i];
                 a.capacity = lp.params.emit_events_capacity[i];
@@ -1742,7 +1594,7 @@ int32_t hnb_pass_indirect(hnb_ctx* c) {
         uint32_t ne = c->header()->sim.num_effects;
         if (ne > c->E) fail(HNB_ERR_NOT_READY, "sim_params.num_effects exceeds the uploaded spawner table");
         CUDA_CHECK(hnb::launch_indirect(static_tables(c), ne, c->stream));
-        c->launches += ne ? (1 + (c->child_rows ? 1 : 0)) : 0;
+        c->launches += ne ? (1 + (c->d_child_infos.size() ? 1 : 0)) : 0;
         std::fill(c->init_pending.begin(), c->init_pending.end(), 0);  // the deferred init accounting has been applied
     });
 }
@@ -1756,7 +1608,7 @@ int32_t hnb_pass_prefix_sum(hnb_ctx* c) {
         uint32_t* ts = c->h_at<uint32_t>(c->lay.off_tile_size);
         for (uint32_t b = 0; b < c->B; ++b) if (ts[b] == 0) ts[b] = 128;
         flush_arena(c, false);
-        if (c->B) CUDA_CHECK(cudaMemcpyAsync(c->d_arena + c->lay.off_tile_size, ts, size_t(c->B) * 4, cudaMemcpyHostToDevice, c->stream));
+        if (c->B) CUDA_CHECK(cudaMemcpyAsync(c->d_arena.get() + c->lay.off_tile_size, ts, size_t(c->B) * 4, cudaMemcpyHostToDevice, c->stream));
         CUDA_CHECK(hnb::launch_prefix_sum(static_tables(c), c->B, c->stream));
         c->launches += c->B ? 1 : 0;
     });
@@ -1781,67 +1633,59 @@ int32_t hnb_pass_fill_dispatch_args(hnb_ctx* c, const uint32_t* src, uint32_t sr
         if (count == 0) return;
         uint32_t src_len = src_offset + (count - 1) * src_stride + 1;
         if (dst_offset + (count - 1) * dst_stride + 3 > dst_len) fail(HNB_ERR_OUT_OF_RANGE, "dst too small");
-        uint32_t *ds = nullptr, *dd = nullptr;
-        CUDA_CHECK(cudaMalloc((void**)&ds, size_t(src_len) * 4));
-        CUDA_CHECK(cudaMalloc((void**)&dd, size_t(dst_len) * 4));
-        CUDA_CHECK(cudaMemcpyAsync(ds, src, size_t(src_len) * 4, cudaMemcpyHostToDevice, c->stream));
-        CUDA_CHECK(cudaMemcpyAsync(dd, dst, size_t(dst_len) * 4, cudaMemcpyHostToDevice, c->stream));
-        CUDA_CHECK(hnb::launch_fill_dispatch_args(ds, dd, src_offset, src_stride, dst_offset, dst_stride, count, c->stream));
+        DeviceArray<uint32_t> ds, dd;
+        CUDA_CHECK(ds.alloc(src_len));
+        CUDA_CHECK(dd.alloc(dst_len));
+        CUDA_CHECK(cudaMemcpyAsync(ds.get(), src, size_t(src_len) * 4, cudaMemcpyHostToDevice, c->stream));
+        CUDA_CHECK(cudaMemcpyAsync(dd.get(), dst, size_t(dst_len) * 4, cudaMemcpyHostToDevice, c->stream));
+        CUDA_CHECK(hnb::launch_fill_dispatch_args(ds.get(), dd.get(), src_offset, src_stride, dst_offset, dst_stride, count, c->stream));
         c->launches++;
-        CUDA_CHECK(cudaMemcpyAsync(dst, dd, size_t(dst_len) * 4, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_CHECK(cudaMemcpyAsync(dst, dd.get(), size_t(dst_len) * 4, cudaMemcpyDeviceToHost, c->stream));
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        cudaFree(ds);
-        cudaFree(dd);
     });
 }
 
 // ---- readback ---------------------------------------------------------------------------------
 int32_t hnb_read_metadata(hnb_ctx* c, uint32_t row, hnb_effect_metadata* out) {
     return guarded([&] {
-        if (row >= c->md_rows) fail(HNB_ERR_OUT_OF_RANGE, "metadata row out of range");
-        CUDA_CHECK(cudaMemcpyAsync(out, c->d_metadata + row, sizeof(*out), cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
+        if (row >= c->d_metadata.size()) fail(HNB_ERR_OUT_OF_RANGE, "metadata row out of range");
+        read_back(c, out, c->d_metadata.get() + row, sizeof(*out));
     });
 }
 int32_t hnb_read_draw_args(hnb_ctx* c, uint32_t row, hnb_draw_indexed_indirect_args* out) {
     return guarded([&] {
-        if (row >= c->draw_rows) fail(HNB_ERR_OUT_OF_RANGE, "draw args row out of range");
-        CUDA_CHECK(cudaMemcpyAsync(out, c->d_draw_args + size_t(row) * 5, sizeof(*out), cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
+        if (row >= c->d_draw_args.size()) fail(HNB_ERR_OUT_OF_RANGE, "draw args row out of range");
+        read_back(c, out, c->d_draw_args.get() + row, sizeof(*out));
     });
 }
 int32_t hnb_read_draw_args_async(hnb_ctx* c, uint32_t first, uint32_t count, hnb_draw_indexed_indirect_args* pinned_out) {
     return guarded([&] {
-        if (uint64_t(first) + count > c->draw_rows) fail(HNB_ERR_OUT_OF_RANGE, "draw args rows out of range");
-        CUDA_CHECK(cudaMemcpyAsync(pinned_out, c->d_draw_args + size_t(first) * 5, size_t(count) * 20, cudaMemcpyDeviceToHost, c->stream));
+        if (uint64_t(first) + count > c->d_draw_args.size()) fail(HNB_ERR_OUT_OF_RANGE, "draw args rows out of range");
+        CUDA_CHECK(cudaMemcpyAsync(pinned_out, c->d_draw_args.get() + first, size_t(count) * 20, cudaMemcpyDeviceToHost, c->stream));
     });
 }
 int32_t hnb_read_spawner(hnb_ctx* c, uint32_t row, hnb_spawner* out) {
     return guarded([&] {
         if (row >= c->E) fail(HNB_ERR_OUT_OF_RANGE, "spawner row out of range");
-        CUDA_CHECK(cudaMemcpyAsync(out, c->d_arena + c->lay.off_spawners + size_t(row) * 128, 128, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
+        read_back(c, out, c->d_arena.get() + c->lay.off_spawners + size_t(row) * 128, 128);
     });
 }
 int32_t hnb_read_batch_info(hnb_ctx* c, uint32_t row, hnb_batch_info* out) {
     return guarded([&] {
         if (row >= c->B) fail(HNB_ERR_OUT_OF_RANGE, "batch row out of range");
-        CUDA_CHECK(cudaMemcpyAsync(out, c->d_arena + c->lay.off_batch_infos + size_t(row) * 24, 24, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
+        read_back(c, out, c->d_arena.get() + c->lay.off_batch_infos + size_t(row) * 24, 24);
     });
 }
 int32_t hnb_read_prefix_sum(hnb_ctx* c, uint32_t first, uint32_t count, uint32_t* out) {
     return guarded([&] {
         if (uint64_t(first) + count > c->E) fail(HNB_ERR_OUT_OF_RANGE, "prefix range out of bounds");
-        CUDA_CHECK(cudaMemcpyAsync(out, c->d_arena + c->lay.off_prefix_sum + size_t(first) * 4, size_t(count) * 4, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
+        read_back(c, out, c->d_arena.get() + c->lay.off_prefix_sum + size_t(first) * 4, size_t(count) * 4);
     });
 }
 int32_t hnb_read_dispatch_args(hnb_ctx* c, uint32_t row, hnb_dispatch_indirect_args* out) {
     return guarded([&] {
-        if (row >= c->scratch_B) fail(HNB_ERR_OUT_OF_RANGE, "dispatch args row out of range");
-        CUDA_CHECK(cudaMemcpyAsync(out, c->d_dispatch_args + size_t(row) * 3, 12, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
+        if (row >= c->scratch_B()) fail(HNB_ERR_OUT_OF_RANGE, "dispatch args row out of range");
+        read_back(c, out, c->dispatch_args() + size_t(row) * 3, 12);
     });
 }
 int32_t hnb_read_tile_size(hnb_ctx* c, uint32_t row, uint32_t* out) {
@@ -1896,30 +1740,24 @@ void hnb_host_free(void* p) {
 
 int32_t hnb_ctx_read_debug(hnb_ctx* c, uint64_t* out16, int32_t clear) {
     return guarded([&] {
-        CUDA_CHECK(cudaMemcpyAsync(out16, c->d_debug, 16 * 8, cudaMemcpyDeviceToHost, c->stream));
-        if (clear) CUDA_CHECK(cudaMemsetAsync(c->d_debug, 0, 16 * 8, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
+        read_back(c, out16, c->d_debug.get(), 16 * 8, clear != 0);
     });
 }
 
 int32_t hnb_ctx_read_debug_ring(hnb_ctx* c, uint64_t* out256, int32_t clear) {
     return guarded([&] {
-        CUDA_CHECK(cudaMemcpyAsync(out256, c->d_debug + 16, 256 * 8, cudaMemcpyDeviceToHost, c->stream));
-        if (clear) CUDA_CHECK(cudaMemsetAsync(c->d_debug + 16, 0, 256 * 8, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
+        read_back(c, out256, c->d_debug.get() + 16, 256 * 8, clear != 0);
     });
 }
 
 int32_t hnb_ctx_measure_sm_mhz(hnb_ctx* c, uint32_t window_us, double* mhz) {
     return guarded([&] {
-        unsigned long long* d = nullptr;
-        CUDA_CHECK(cudaMalloc((void**)&d, 16));
-        CUDA_CHECK(hnb::launch_measure_sm_clock(d, (unsigned long long)window_us * 1000ull, c->stream));
+        DeviceArray<unsigned long long> d;
+        CUDA_CHECK(d.alloc(2));
+        CUDA_CHECK(hnb::launch_measure_sm_clock(d.get(), (unsigned long long)window_us * 1000ull, c->stream));
         c->launches++;
         unsigned long long h[2] = {0, 0};
-        CUDA_CHECK(cudaMemcpyAsync(h, d, 16, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_CHECK(cudaStreamSynchronize(c->stream));
-        cudaFree(d);
+        read_back(c, h, d.get(), 16);
         if (mhz) *mhz = h[1] ? double(h[0]) / (double(h[1]) * 1e-3) : 0.0;
     });
 }
@@ -1936,8 +1774,8 @@ int32_t hnb_ctx_kernel_time_ms(hnb_ctx* c, double* update_ms_total, uint64_t* up
             CUDA_CHECK(cudaEventElapsedTime(&ms, ev.first, ev.second));
             c->update_ms += ms;
             c->update_launches++;
-            c->ev_free.push_back(ev);
         }
+        for (auto& ev : c->ev_pending) c->ev_free.push_back(std::move(ev));
         c->ev_pending.clear();
         if (update_ms_total) *update_ms_total = c->update_ms;
         if (update_launches) *update_launches = c->update_launches;
