@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 
 from oracle import c_oracle as O
+from oracle.hanabi_oracle import pcg_hash
 
 SUB_TILE_C5 = 128  # rows of an update sub-tile for C5 records: 32 lanes x K = 4 rows in flight per lane
 
@@ -334,6 +335,40 @@ def assert_world_equal(ref: RefWorld, got: dict, float_words=None, rtol=0.0, wha
         assert_float_attributes_close(got["particles"], ref.particles, float_attrs, rtol, what)
 
 
+def float_word_mask(asset):
+    """(boolean mask over the AoS words, [(first_word, component_count)] of the fp32 attributes)"""
+    from bevy_hanabi_b200 import graph as G
+    fields, size, _ = asset.particle_layout()
+    mask = np.zeros(size // 4, dtype=bool)
+    attrs = []
+    for f in fields:
+        if not f.name.startswith("pad") and G.vt_elem(f.vt) == "f":
+            mask[f.offset // 4: f.offset // 4 + G.vt_count(f.vt)] = True
+            attrs.append((f.offset // 4, G.vt_count(f.vt)))
+    return mask, attrs
+
+
+def assert_relaxed_equal(ref: RefWorld, got: dict, what=""):
+    """RELAXED_ORDER: counts exact, lists equal as sets per segment, particles identical."""
+    np.testing.assert_array_equal(got["metadata"], ref.metadata_rows(), err_msg=f"{what}: effect metadata")
+    np.testing.assert_array_equal(got["draw"], ref.draw, err_msg=f"{what}: draw indirect args")
+    for i, inst in enumerate(ref.instances):
+        md = ref.metadata[i]
+        base, alive, W = inst.slab_offset, md.alive_count, md.indirect_write_index
+        assert sorted(got["indirect"][base:base + alive, W].tolist()) == sorted(ref.indirect[base:base + alive, W].tolist()), f"{what}: alive set"
+        assert sorted(got["indirect"][base + alive:base + inst.capacity, 2].tolist()) == sorted(ref.indirect[base + alive:base + inst.capacity, 2].tolist()), f"{what}: dead set"
+    np.testing.assert_array_equal(got["particles"], ref.particles, err_msg=f"{what}: particle buffer")
+
+
+def assert_ribbons_sorted(ref: RefWorld):
+    """Every instance's alive list is in ascending (RIBBON_ID, AGE bits) order."""
+    for i in range(len(ref.instances)):
+        md, base = ref.metadata[i], ref.spawners[i].slab_offset
+        e = ref.indirect[base:base + md.alive_count, md.indirect_write_index].astype(np.int64)
+        k = (ref.particles[base + e, md.sort_key_offset].astype(np.uint64) << np.uint64(32)) | ref.particles[base + e, md.sort_key2_offset]
+        assert np.all(k[1:] >= k[:-1])
+
+
 def assert_float_attributes_close(got_words, ref_words, float_attrs, rtol, what=""):
     """"fp32 attributes within `rtol` relative": the error of each component is measured against the magnitude of
     the ATTRIBUTE it belongs to (the largest component of that vector in that particle), so that a component that
@@ -350,3 +385,391 @@ def assert_float_attributes_close(got_words, ref_words, float_attrs, rtol, what=
             i = np.argwhere(bad)[0]
             raise AssertionError(f"{what}: float attribute at words [{first},{first + cnt}): {bad.sum()} components exceed rtol={rtol}; "
                                  f"first at row {i[0]}: got {a[i[0]]} want {b[i[0]]}")
+
+
+# ---- the lock-step runner ---------------------------------------------------------------------------------------------
+def seeds(n, f):
+    """Per-instance spawner seeds of frame `f`."""
+    return [int(s) for s in pcg_hash(np.arange(n, dtype=np.uint32) + np.uint32(100 * f + 7))]
+
+
+def is_identity(ref: RefWorld, i: int) -> bool:
+    """Whether instance i's current alive list is 0, 1, 2, ..."""
+    md, base = ref.metadata[i], ref.instances[i].slab_offset
+    lst = ref.indirect[base:base + md.alive_count, md.indirect_write_index]
+    return bool((lst == np.arange(len(lst))).all())
+
+
+class Lockstep:
+    """A GpuWorld and the oracle world it must equal, stepped frame by frame and compared after every frame.
+
+    `asset`: an authored effect, stepped by the numpy interpreter with the per-instance property records `props`. Without
+    it the world runs C5 (recipes.c5_lowered) under the C oracle's update body with ACCEL_DRAG; `init` adds the constant
+    init of c5_init(). `relaxed`: lists and dead stacks are compared as sets, then the oracle adopts the device's lists
+    (the next frame reads them in the order the device wrote them). `rtol`: fp32 attributes within `rtol` of their
+    magnitude, and the device restarts every compared frame from the oracle's records (the bound is a per-step bound:
+    libm-level differences are amplified from frame to frame by non-smooth dynamics). `seeds(n, f)`: the spawner seeds of
+    frame f, or None to keep them."""
+
+    def __init__(self, ctx, orc, ref, asset=None, *, props=None, init=False, sector=False, slot=False, relaxed=False,
+                 fast_math=False, rtol=0.0, seeds=None):
+        from bevy_hanabi_b200 import recipes
+        from oracle.hanabi_oracle import EffectOracle
+        from tests.effects import ACCEL_DRAG, c5_init
+        self.ctx, self.orc, self.ref, self.slot, self.relaxed, self.rtol, self.seeds = ctx, orc, ref, slot, relaxed, rtol, seeds
+        self.fresh, self.got = True, None
+        ref.slot_order = slot
+        blobs = None
+        if asset is None:
+            self.eo = None
+            self.c_args = [orc.orc_body_update_c5(), ACCEL_DRAG]
+            if init:
+                self.init = c5_init()  # kept alive: the oracle reads it through a pointer
+                self.c_args += [orc.orc_body_init_const(), C.byref(self.init)]
+            lowered = recipes.c5_lowered(relaxed_order=relaxed, slot_order=slot)
+            self.mask, self.float_attrs = None, None
+        else:
+            if props is not None:
+                blobs = [asset.serialize_properties(p) for p in props]
+                for i in range(len(ref.instances)):
+                    ref.metadata[i].properties_array_index = i
+            self.eo = EffectOracle(asset, dict(enumerate(props)) if props else None)
+            lowered = asset.generate(sector_planes=sector, slot_order=slot, relaxed_order=relaxed, fast_math=fast_math)
+            self.mask, self.float_attrs = float_word_mask(asset)
+        self.gpu = GpuWorld(ctx, ref, lowered, property_blobs=blobs, sector_planes=sector)
+
+    def step(self, f, spawns=None):
+        """Frame `f` on both sides, without a comparison. `spawns`: per instance, or None to keep the spawn counts."""
+        ref = self.ref
+        ref.sim.time = np.float32(f) * ref.sim.delta_time
+        ref.sim.virtual_time = ref.sim.real_time = ref.sim.time
+        if spawns is not None:
+            ref.set_spawns(spawns, self.seeds(len(spawns), f) if self.seeds else None)
+        if self.eo is not None:
+            self.eo.frame(ref, self.orc)
+        else:
+            ref.oracle_frame(self.orc, *self.c_args)
+        self.gpu.frame()
+        self.fresh = False
+
+    def run(self, schedule, start=0, what="", check_every=1):
+        """Frames start, start + 1, ... with the spawns of `schedule` (a list of per-instance lists, or a frame count to keep
+        the spawn counts), compared after every `check_every`-th and the last. Returns the last pulled state."""
+        schedule = [None] * schedule if isinstance(schedule, int) else schedule
+        for k, spawns in enumerate(schedule):
+            self.step(start + k, spawns)
+            if k % check_every == 0 or k == len(schedule) - 1:
+                self.compare(f"{what} frame {start + k}")
+        return self.got
+
+    def compare(self, what=""):
+        ctx, ref, gpu = self.ctx, self.ref, self.gpu
+        if self.fresh:  # no frame ran yet: the context has no per-frame tables of this world to read back
+            n = len(ref.instances)
+            ctx.sync()
+            got = {"particles": ctx.slab_download_aos(gpu.slab, 0, ref.slab_rows, gpu.stride),
+                   "indirect": ctx.slab_download_indirect(gpu.slab, 0, ref.slab_rows),
+                   "metadata": np.stack([np.frombuffer(bytes(ctx.read_metadata(i)), dtype=np.uint32) for i in range(n)]),
+                   "draw": np.concatenate([np.frombuffer(bytes(ctx.read_draw_args(i)), dtype=np.uint32) for i in range(n)])}
+            for k, want in (("particles", ref.particles), ("indirect", ref.indirect), ("metadata", ref.metadata_rows()), ("draw", ref.draw)):
+                np.testing.assert_array_equal(got[k], want, err_msg=f"{what}: {k}")
+        else:
+            got = gpu.pull()
+            if self.relaxed:
+                assert_relaxed_equal(ref, got, what)
+                ref.indirect[:, :] = got["indirect"]
+            else:
+                assert_world_equal(ref, got, float_words=self.mask if self.rtol else None, rtol=self.rtol, what=what,
+                                   float_attrs=self.float_attrs)
+                if self.rtol:
+                    ctx.slab_upload_aos(gpu.slab, 0, ref.particles)
+        if self.slot:
+            assert ctx.read_debug(False)[15] == 0, f"{what}: alive bitmap and counters disagree"
+        self.got = got
+        return got
+
+    def span(self, i):
+        inst = self.ref.instances[i]
+        return inst.slab_offset, inst.capacity
+
+
+# ---- worlds -----------------------------------------------------------------------------------------------------------
+def sparks_world(caps, dt=0.05, batches=None, seed=1):
+    """Instances of drifting_sparks with capacities `caps`, back to back, none alive, every dead stack shuffled."""
+    from tests.effects import drifting_sparks
+    asset = drifting_sparks(max(caps))
+    _, size, _ = asset.particle_layout()
+    insts, off = [], 0
+    for i, c in enumerate(caps):
+        insts.append(Instance(off, c, alive=0, seed=11 + 7 * i))
+        off += c
+    ref = RefWorld(off, size // 4, insts, batches=batches, dt=dt)
+    rng = np.random.default_rng(seed)
+    for inst in insts:
+        rows = slice(inst.slab_offset, inst.slab_offset + inst.capacity)
+        ref.indirect[rows, 2] = rng.permutation(ref.indirect[rows, 2])
+    return asset, ref
+
+
+def table_world(name, caps, batches=None, align=1, dead_perm_seed=None):
+    """A slab of instances of tests.effects.EFFECTS[name] with the given capacities, none alive, every dead stack
+    shuffled, per-instance emitter translations."""
+    from tests.effects import EFFECTS
+    _, size, dt, _ = EFFECTS[name]
+    insts, off = [], 0
+    for i, c in enumerate(caps):
+        insts.append(Instance(off, c, alive=0, seed=17 + 31 * i))
+        off += (c + align - 1) // align * align
+    ref = RefWorld(max(off, 1), size // 4, insts, batches=batches, dt=dt)
+    rng = np.random.default_rng(dead_perm_seed if dead_perm_seed is not None else sum(caps))
+    for inst in insts:
+        rows = slice(inst.slab_offset, inst.slab_offset + inst.capacity)
+        ref.indirect[rows, 2] = rng.permutation(ref.indirect[rows, 2])
+    for i in range(len(insts)):  # per-instance emitter translations (Global simulation space adds them at init)
+        tr = list(ref.spawners[i].transform)
+        tr[3], tr[7], tr[11] = 0.5 * i, -0.25 * i, 1.0 + i
+        for k in range(12):
+            ref.spawners[i].transform[k] = tr[k]
+    return ref
+
+
+def filled_c5(ctx, orc, insts, fills, batches=None, dead_perm_seed=None, parities=None):
+    """A Lockstep of C5 with its init over `insts`. `fills`: (first, count, seed, lifetime_lo, lifetime_hi) ranges filled
+    by hnb_slab_fill_c5 on the device and orc_fill_c5 in the oracle, after the world was uploaded; the last fill holds the
+    claim. `parities`: the alive-list column each instance's first frame appends to (metadata indirect_write_index)."""
+    ref = RefWorld(sum(i.capacity for i in insts), 8, insts, batches=batches)
+    for i, parity in enumerate(parities or []):
+        ref.metadata[i].indirect_write_index = parity
+    if dead_perm_seed is not None:  # a dead stack whose slots are not in row order: spawns then append non-identity entries
+        rng = np.random.default_rng(dead_perm_seed)
+        for inst in insts:
+            rows = slice(inst.slab_offset + inst.alive, inst.slab_offset + inst.capacity)
+            ref.indirect[rows, 2] = rng.permutation(ref.indirect[rows, 2])
+    lock = Lockstep(ctx, orc, ref, init=True)
+    for first, count, seed, lo, hi in fills:
+        orc.orc_fill_c5(O.ptr(ref.particles), O.ptr(ref.indirect), first, count, seed, lo, hi)
+        ctx.slab_fill_c5(lock.gpu.slab, first, count, seed, lo, hi)
+    return lock
+
+
+# Where an identity claim ends, with S = rows per tile: inside or at the end of a warp's 32 rows, of a 128-row sub-tile,
+# of a tile.
+CLAIM_ENDS = [0, 1, 31, 32, 33, 127, 128, 129, "S-1", "S", "S+1", "3S+17"]
+# Spawns per frame: a frame that keeps the claim, a burst that shrinks it to the alive count L, the frame whose write
+# column is claimed only up to L (particle L-1 dies in it), two frames without deaths, four frames in which every other
+# filled particle dies, and a burst into the freed slots.
+CLAIM_EDGE_SPAWNS = [0, 600, 0, 0, 0, 0, 0, 0, 0, 400, 0]
+
+
+def claim_end(end, S):
+    return {"S-1": S - 1, "S": S, "S+1": S + 1, "3S+17": 3 * S + 17}.get(end, end)
+
+
+def claim_edge_world(L, cap):
+    """One C5 instance of `cap` rows, L of them alive, with both alive lists the identity over the whole capacity (as
+    hnb_slab_fill_c5 leaves them, with a claim on all `cap` rows). The dead stack hands out slot L+1 first and slot L
+    second, the rest shuffled: after the burst, list rows L and L+1 hold slots L+1 and L. Particle L-1 dies in the frame
+    after the burst, so the survivor at rank L is slot L while the write column's claim ends at L and its row L still holds
+    L+1; every other filled particle dies in frames 5-8 (dt = 1/60)."""
+    rng = np.random.default_rng(L)
+    ref = RefWorld(cap, 8, [Instance(0, cap, alive=L, seed=31)])
+    dt = float(ref.sim.delta_time)
+    ref.indirect[:, 0] = ref.indirect[:, 1] = np.arange(cap, dtype=np.uint32)
+    ref.indirect[L:, 2] = np.concatenate([[L + 1, L], rng.permutation(np.arange(L + 2, cap))]).astype(np.uint32)
+    p = np.zeros((cap, 8), dtype=np.float32)
+    p[:, 0:3] = rng.uniform(-1, 1, (cap, 3))
+    p[:, 4:7] = rng.uniform(-1, 1, (cap, 3))
+    p[:, 7] = rng.uniform(5.5 * dt, 9.0 * dt, cap)
+    if L:
+        p[L - 1, 7] = 2.5 * dt
+    ref.particles[:] = p.view(np.uint32)
+    return ref
+
+
+def claim_edge_lockstep(ctx, orc, L, cap):
+    """claim_edge_world on the device: identity lists with a claim on all rows under the scenario's records (writing
+    records keeps the claim)."""
+    lock = Lockstep(ctx, orc, claim_edge_world(L, cap), init=True)
+    ctx.slab_fill_c5(lock.gpu.slab, 0, cap, 1, 1e9, 1e9)
+    ctx.slab_upload_aos(lock.gpu.slab, 0, lock.ref.particles)
+    return lock
+
+
+def assert_claims_trusted(lock, n, f):
+    """While both alive-list columns of instance 0 are claimed over [0, n), overwrite those rows through the device view
+    with two different permutations (in range: a load of them stays in bounds and shows up as a mismatch) and run frame f
+    without spawns. The claimed rows must be read as their own index and the stores skipped: both permutations survive,
+    and with the identity put back where they stand, every buffer equals the oracle."""
+    ctx, ref, gpu = lock.ctx, lock.ref, lock.gpu
+    rng = np.random.default_rng(77)
+    poison = [rng.permutation(n).astype(np.uint32) for _ in range(2)]
+    view = ctx.slab_device_view(gpu.slab)
+    ctx.sync()
+    for col, ptr in enumerate((view.ping, view.pong)):
+        ctx.device_upload(ptr, poison[col])  # not supported for users: done here to observe the claim
+    read = ref.metadata[0].indirect_write_index  # the column the next frame reads
+    lock.step(f, [0])
+    got = gpu.pull()
+    np.testing.assert_array_equal(got["indirect"][:n, 1 - read], poison[1 - read], err_msg="claimed stores were not skipped")
+    np.testing.assert_array_equal(got["indirect"][:n, read], poison[read], err_msg="the read column was written")
+    got["indirect"][:n, :2] = ref.indirect[:n, :2]
+    assert_world_equal(ref, got, what="claimed entries were loaded")
+
+
+# ---- GPU spawn events -------------------------------------------------------------------------------------------------
+def oracle_child_init(child, co, cw, po, pw, events, n_valid, seed_c):
+    """Child init from GPU spawn events (vfx_init.wgsl:123-171): one thread per event, capped by max_spawn; reads
+    the parent particle the event names. Returns the number of children spawned."""
+    from oracle.hanabi_oracle import Env, Rng, Writer, apply_modifier
+    md = cw.metadata[0]
+    n = min(n_valid, md.max_spawn)
+    if not n:
+        return 0
+    k = np.arange(n, dtype=np.int64)
+    alive_index = md.alive_count + k
+    slots = cw.indirect[alive_index, 2].astype(np.int64)
+    pidx = slots.astype(np.uint32)
+    parent_idx = events[:n].astype(np.uint32)
+    parent_rec = po.unpack(pw.particles[parent_idx.astype(np.int64)].copy())
+    rec = np.zeros((n, co.stride_words), dtype=np.uint32)
+    P = co.unpack(rec)
+    env = Env(n, P, cw.sim, Rng(pcg_hash(pidx ^ np.uint32(seed_c))), {}, pidx, (md.particle_counter + k).astype(np.uint32),
+              np.array(list(cw.spawners[0].transform), dtype=np.float32).reshape(3, 4), parent=parent_rec, parent_particle_index=parent_idx)
+    wr = Writer()
+    for m in child.init_modifiers:
+        apply_modifier(m, child.module, env, wr)
+    co.pack(P, rec)
+    cw.indirect[alive_index, md.indirect_write_index] = pidx
+    cw.particles[pidx.astype(np.int64)] = rec
+    md.alive_count += n
+    md.particle_counter += n
+    return n
+
+
+def oracle_append_events(pw, counts, events, event_count):
+    """append_spawn_events_N in serial thread order (lib.rs:976-993); returns the new event_count."""
+    from tests.effects import EVENT_CAP
+    pidx_rows = pw.indirect[:pw.metadata[0].max_update, 1 - pw.metadata[0].indirect_write_index]
+    for row in np.nonzero(counts)[0]:
+        c = int(counts[row])
+        base = min(event_count, EVENT_CAP)
+        event_count += c
+        capped = min(c, EVENT_CAP - base)
+        events[base:base + capped] = pidx_rows[row]
+    return event_count
+
+
+def emitter_scene(ctx, orc, pcap, ordered):
+    """tests.effects.emitter_assets(pcap) for 20 frames: each child consumes its own buffer the frame after. Children come
+    BEFORE the parent in batch order, as EffectSorter places them (batch.rs:599-603), so a child's init reads the parent's
+    records before the parent's init recycles slots. Without `ordered`, the order in which events land depends on atomic
+    scheduling: the buffers are compared as multisets (sub-multisets of what was emitted on overflow) and the oracle
+    consumes them in the device's order. With HNB_EFFECT_ORDERED_EVENTS the buffers must hold exactly the canonical
+    sequence, overflow included. Every other buffer is compared exactly after every frame."""
+    from collections import Counter
+
+    from bevy_hanabi_b200 import _native as N
+    from bevy_hanabi_b200 import runtime as R
+    from oracle.hanabi_oracle import EffectOracle
+    from tests.effects import EVENT_CAP, emitter_assets
+    parent, children = emitter_assets(pcap)
+    p_fx = parent.generate(num_event_bindings=2, ordered_events=ordered)
+    c_fx = [c.generate(parent=parent) for c in children]
+    p_stride, c_stride = p_fx.particle_stride, c_fx[0].particle_stride
+    dt = 1.0 / 30.0
+    pw = RefWorld(pcap, p_stride // 4, [Instance(0, pcap, alive=0, seed=1)], dt=dt)
+    cw = [RefWorld(4096, c_stride // 4, [Instance(0, 4096, alive=0, seed=2 + k)], dt=dt) for k in (0, 1)]
+    po, co = EffectOracle(parent), [EffectOracle(c) for c in children]
+    events = [np.zeros(EVENT_CAP, dtype=np.uint32) for _ in (0, 1)]
+    event_count = [0, 0]
+
+    # GPU tables: rows 0, 1 = children (batches 0, 1), row 2 = parent (batch 2); child infos 0, 1 = channels 0, 1
+    p_slab = ctx.slab_create(pcap, p_stride)
+    c_slab = [ctx.slab_create(4096, c_stride) for _ in (0, 1)]
+    p_eff = ctx.effect_compile(p_fx)
+    c_eff = [ctx.effect_compile(fx) for fx in c_fx]
+    evbuf = [ctx.event_buffer_create(EVENT_CAP) for _ in (0, 1)]
+    for k in (0, 1):
+        ctx.child_info_insert(k, 0, 0)
+        md_c = R.initial_metadata(4096, k, c_stride // 4)
+        md_c.global_child_index, md_c.local_child_index = k, k
+        ctx.metadata_insert(k, md_c)
+        ctx.draw_args_insert(k)
+    md_p = R.initial_metadata(pcap, 2, p_stride // 4)
+    md_p.base_child_index = 0
+    ctx.metadata_insert(2, md_p)
+    ctx.draw_args_insert(2)
+
+    spawn_sched = [s * pcap // 1024 for s in [700, 0, 0, 150, 0, 0, 0, 800, 0, 0, 0, 0, 100, 0, 0, 0, 0, 0, 0, 0]]
+    spawned = [0, 0]
+    overflowed = False
+    seen_counts = []
+    all_emitted = [[], []]
+    for f, spawn in enumerate(spawn_sched):
+        seed_p = int(pcg_hash(np.array([5000 + f], dtype=np.uint32))[0])
+        seed_c = [int(pcg_hash(np.array([6000 + 10 * f + k], dtype=np.uint32))[0]) for k in (0, 1)]
+        ctx.upload_spawners([R.make_spawner(spawn=0, seed=seed_c[k], effect_metadata_index=k, draw_indirect_index=k, slab_offset=0, parent_slab_offset=0)
+                             for k in (0, 1)]
+                            + [R.make_spawner(spawn=spawn, seed=seed_p, effect_metadata_index=2, draw_indirect_index=2, slab_offset=0)])
+        ctx.upload_batches([N.BatchInfo(0, 0, 0, 0, 0, 1), N.BatchInfo(0, 0, 1, 0, 1, 1), N.BatchInfo(0, 0, 2, 0, 2, 1)], [0, 0, 0])
+        ctx.set_sim_params(dt, f * dt, 3)
+        # what the previous frame's update left in the two buffers
+        n_valid = []
+        for k in (0, 1):
+            assert ctx.read_child_info(k).event_count == event_count[k], f"frame {f} channel {k}"
+            nv = min(event_count[k], EVENT_CAP)
+            overflowed |= event_count[k] > EVENT_CAP
+            seen_counts.append(event_count[k])
+            got = ctx.event_buffer_download(evbuf[k], 0, EVENT_CAP)
+            if ordered:
+                np.testing.assert_array_equal(got[:nv], events[k][:nv], err_msg=f"frame {f} channel {k}: event order")
+            elif event_count[k] <= EVENT_CAP:
+                assert sorted(got[:nv].tolist()) == sorted(events[k][:nv].tolist())
+            else:
+                # overflow: WHICH appends hit the cap depends on atomic order (lib.rs:980-986), on the reference too;
+                # what is defined is that the buffer is full of events that were really emitted
+                emitted, kept = Counter(all_emitted[k]), Counter(got.tolist())
+                assert all(kept[p] <= emitted[p] for p in kept), f"frame {f} channel {k}: event that nobody emitted"
+            events[k][:nv] = got[:nv]   # consume in the GPU buffer's order (the reference's order is unspecified)
+            n_valid.append(nv)
+        ctx.simulate([N.BatchLaunch.make(c_eff[0], c_slab[0], 0, 0, parent_slab=p_slab, consume_events=evbuf[0]),
+                      N.BatchLaunch.make(c_eff[1], c_slab[1], 1, 0, parent_slab=p_slab, consume_events=evbuf[1]),
+                      N.BatchLaunch.make(p_eff, p_slab, 2, spawn, emit_events=evbuf)])
+
+        # ----- oracle frame: inits (children read the parent's records as the previous frame left them), ...
+        t = np.float32(f * dt)
+        pw.sim.time = t
+        for k in (0, 1):
+            cw[k].sim.time = t
+            cw[k].set_spawns([0], [seed_c[k]])
+            spawned[k] += oracle_child_init(children[k], co[k], cw[k], po, pw, events[k], n_valid[k], seed_c[k])
+        pw.set_spawns([spawn], [seed_p])
+        po.init_pass(pw)
+        # ... indirect (clears the event counts, vfx_indirect.wgsl:38-46) + prefix sums, updates, event appends
+        event_count = [0, 0]
+        for w in (cw[0], cw[1], pw):
+            w.oracle_indirect(orc)
+            w.oracle_prefix_sum(orc)
+        for k in (0, 1):
+            co[k].update_pass(cw[k])
+        po.update_pass(pw)
+        assert [ch for ch, _ in po.last_emitted] == [0, 1]
+        for channel, counts in po.last_emitted:
+            event_count[channel] = oracle_append_events(pw, counts, events[channel], event_count[channel])
+            rows_read = pw.indirect[:pw.metadata[0].max_update, 1 - pw.metadata[0].indirect_write_index]
+            all_emitted[channel] = np.repeat(rows_read, counts[:len(rows_read)]).tolist()
+
+        # ----- compare
+        ctx.sync()
+        for world, slab, row, stride, rows in ((cw[0], c_slab[0], 0, c_stride, 4096), (cw[1], c_slab[1], 1, c_stride, 4096), (pw, p_slab, 2, p_stride, pcap)):
+            m_gpu = np.frombuffer(bytes(ctx.read_metadata(row)), dtype=np.uint32)
+            m_ref = world.metadata_rows()[0].copy()
+            m_ref[5] = row
+            for fld in (7, 8, 9, 10):
+                m_ref[fld] = m_gpu[fld]
+            np.testing.assert_array_equal(m_gpu, m_ref, err_msg=f"frame {f} metadata row {row}")
+            assert ctx.read_draw_args(row).instance_count == world.draw[1]
+            np.testing.assert_array_equal(ctx.slab_download_indirect(slab, 0, rows), world.indirect, err_msg=f"frame {f} row {row}: lists")
+            np.testing.assert_array_equal(ctx.slab_download_aos(slab, 0, rows, stride), world.particles, err_msg=f"frame {f} row {row}: particles")
+    assert spawned[0] > 100 and spawned[1] > 100, spawned
+    assert overflowed and min(seen_counts[2:]) < EVENT_CAP, f"the scenario must both overflow an event buffer (capped appends) and not: {seen_counts}"

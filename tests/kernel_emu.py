@@ -217,6 +217,26 @@ extern "C" uint32_t emu_init_items(void) { return HNB_INIT_ITEMS; }
 """
 
 
+# The same driver whose init and update launchers pass the slab's identity claims (SlabView::ident_claim; DRIVER passes
+# none), set with emu_set_ident_claim.
+_PLAIN_INIT = 'extern "C" void emu_init(const EmuBatch* b, uint32_t blocks) { emu_launch(hnb::hnb_init, make_params(b), blocks, HNB_INIT_SMEM_EFFECTS * 4, 8); }'
+_PLAIN_UPDATE = 'extern "C" void emu_update(const EmuBatch* b, uint32_t blocks, uint32_t smem) { emu_launch(hnb::hnb_update, make_params(b), blocks, smem); }'
+_CLAIMED_INIT = r"""static unsigned long long* g_ident_claim = nullptr;  // [2]: identity claims of ping / pong
+extern "C" void emu_set_ident_claim(unsigned long long* claim) { g_ident_claim = claim; }
+extern "C" void emu_init(const EmuBatch* b, uint32_t blocks) {
+    hnb::BatchParams P = make_params(b);
+    P.slab.ident_claim = g_ident_claim;
+    emu_launch(hnb::hnb_init, P, blocks, HNB_INIT_SMEM_EFFECTS * 4, 8);
+}"""
+_CLAIMED_UPDATE = r"""extern "C" void emu_update(const EmuBatch* b, uint32_t blocks, uint32_t smem) {
+    hnb::BatchParams P = make_params(b);
+    P.slab.ident_claim = g_ident_claim;
+    emu_launch(hnb::hnb_update, P, blocks, smem);
+}"""
+assert DRIVER.count(_PLAIN_INIT) == 1 and DRIVER.count(_PLAIN_UPDATE) == 1
+CLAIMED_DRIVER = DRIVER.replace(_PLAIN_INIT, _CLAIMED_INIT).replace(_PLAIN_UPDATE, _CLAIMED_UPDATE)
+
+
 class EmuBatch(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("frame", "spawners", "spawn_prefix", "prefix_sum", "tile_prefix", "batch_info", "batch_tiles", "ticket",
                                           "tile_state", "metadata", "draw_args", "properties")] + \
@@ -226,7 +246,8 @@ class EmuBatch(C.Structure):
                 ("parent_planes", C.c_void_p * 16), ("event_counts", C.c_void_p * 4)]
 
 
-def build_emulated_effect(lowered, allow_events: bool = False) -> C.CDLL:
+def build_emulated_effect(lowered, allow_events: bool = False, driver: str = DRIVER) -> C.CDLL:
+    """`driver`: the host entry points compiled after the kernels (CLAIMED_DRIVER: launches under identity claims)."""
     src = lowered.generate_source()
     if not allow_events and ("#define HNB_EMIT_EVENTS 1" in src or "#define HNB_READ_PARENT 1" in src or "#define HNB_CONSUME_EVENTS 1" in src):
         raise NotImplementedError("EmuWorld covers effects without GPU spawn events; use EmuScene")
@@ -234,7 +255,7 @@ def build_emulated_effect(lowered, allow_events: bool = False) -> C.CDLL:
         assert src.count(old) == 1, f"kernel source changed, update tests/kernel_emu.py: {old!r}"
         src = src.replace(old, new)
     # the remaining `asm` statements sit in #if HNB_PROFILE blocks, which are compiled out (HNB_PROFILE is 0)
-    text = PRELUDE + src + DRIVER
+    text = PRELUDE + src + driver
     OUT.mkdir(parents=True, exist_ok=True)
     tag = hashlib.sha1(text.encode()).hexdigest()[:16]
     cpp, so = OUT / f"emu_{tag}.{os.getpid()}.cpp", OUT / f"emu_{tag}.so"  # per process: workers may build the same tag at once
@@ -273,10 +294,10 @@ def tile_count(rows, word: int):
 class EmuWorld:
     """One batch (all instances of `ref`) simulated by the emulated kernels, starting from `ref`'s current state."""
 
-    def __init__(self, ref, lowered, chunks: int = 1, update_ctas: int = 2, property_blobs=None, static_lib=None):
+    def __init__(self, ref, lowered, chunks: int = 1, update_ctas: int = 2, property_blobs=None, static_lib=None, driver=DRIVER):
         """`static_lib` (tests/static_emu.build()): run the real bookkeeping and ribbon-sort kernels too instead of their
         restatements."""
-        self.ref, self.lib = ref, build_emulated_effect(lowered)
+        self.ref, self.lib = ref, build_emulated_effect(lowered, driver=driver)
         self.static_lib = static_lib
         self.ribbons = bool(lowered.flags & (1 << 5))  # HNB_EFFECT_RIBBONS
         self.stride = ref.stride_words * 4
@@ -556,3 +577,143 @@ class EmuScene:
         slab["lib"].emu_planes_to_aos(C.byref(slab["b"]), aos.ctypes.data, 0, slab["rows"], slab["stride"])
         return {"particles": aos, "indirect": np.stack(slab["cols"], axis=1), "metadata": np.frombuffer(bytes(self.metadata[b]), dtype=np.uint32).copy(),
                 "instance_count": int(self.draw[5 * b + 1])}
+
+
+# ---- shared by the emulation tests ------------------------------------------------------------------------------------
+def assert_same(ref, got, what):
+    """Every buffer of an EmuWorld bit for bit against the oracle world."""
+    np.testing.assert_array_equal(got["metadata"], ref.metadata_rows(), err_msg=f"{what}: metadata")
+    np.testing.assert_array_equal(got["draw"], ref.draw, err_msg=f"{what}: draw args")
+    np.testing.assert_array_equal(got["prefix"], ref.prefix, err_msg=f"{what}: prefix sums")
+    assert got["total_update"] == ref.batch_infos[0].total_update_count
+    np.testing.assert_array_equal(got["indirect"], ref.indirect, err_msg=f"{what}: ping / pong / dead")
+    np.testing.assert_array_equal(got["particles"], ref.particles, err_msg=f"{what}: particles")
+
+
+def c5_world(rng, insts):
+    """A C5 world of `insts`, back to back, their alive rows with random motion and lifetimes of 0.02 to 0.15 s."""
+    from tests.helpers import RefWorld
+    ref = RefWorld(sum(i.capacity for i in insts), 8, insts)
+    for inst in ref.instances:
+        n = inst.alive
+        p = np.zeros((n, 8), dtype=np.float32)
+        p[:, 0:3] = rng.uniform(-1, 1, (n, 3)); p[:, 4:7] = rng.uniform(-1, 1, (n, 3)); p[:, 7] = rng.uniform(0.02, 0.15, n)
+        ref.particles[inst.slab_offset:inst.slab_offset + n] = p.view(np.uint32)
+    return ref
+
+
+def claim(base, length):
+    """An identity-claim word: rows [0, length) of the column starting at slab row `base` hold their own index."""
+    return np.uint64((base << 32) | length)
+
+
+def claimed(ref, chunks, claim_len):
+    """The emulated C5 world of `ref` with a claim of `claim_len` rows on both alive-list columns; returns (EmuWorld, the
+    two claim words, which the kernels update in place)."""
+    from bevy_hanabi_b200 import recipes
+    emu = EmuWorld(ref, recipes.c5_lowered(), chunks=chunks, update_ctas=2, driver=CLAIMED_DRIVER)
+    claims = np.array([claim(0, claim_len)] * 2, dtype=np.uint64)
+    emu.lib.emu_set_ident_claim.argtypes = [C.c_void_p]
+    emu.lib.emu_set_ident_claim.restype = None
+    emu.lib.emu_set_ident_claim(claims.ctypes.data)
+    return emu, claims
+
+
+def c5_frame(orc, ref, emu, spawn=0):
+    """One frame of the single-instance C5 world `ref` with its constant init, in the oracle and in `emu`."""
+    from tests.effects import ACCEL_DRAG, c5_init
+    ref.set_spawns([spawn])
+    ref.oracle_frame(orc, orc.orc_body_update_c5(), ACCEL_DRAG, orc.orc_body_init_const(), C.byref(c5_init()))
+    emu.frame_step(orc, ref.sim, [spawn], [42])
+
+
+def random_event_scene(orc, ordered, seed):
+    """A randomised parent / two-children scene (emission probability, events per death, lifetimes, spawn schedule,
+    tile size, grid). Default mode: event buffers as multisets (sub-multisets on overflow), the oracle adopts the
+    buffer's order; ordered mode: exact buffers. Everything else exact in both."""
+    from collections import Counter
+
+    from bevy_hanabi_b200 import graph as G
+    from oracle.hanabi_oracle import EffectOracle, pcg_hash
+    from tests import static_emu
+    from tests.effects import EVENT_CAP
+    from tests.helpers import Instance, RefWorld, oracle_append_events, oracle_child_init
+    A = G.Attribute
+    rng = np.random.default_rng(700 + seed)
+    p_cap, c_cap = int(rng.choice([300, 1024, 1500])), 4096
+    wp = G.ExprWriter()
+    parent = (G.EffectAsset(p_cap, wp.module, name="emitter")
+              .init(G.SetAttributeModifier(A.POSITION, wp.rand(G.VEC3) * wp.lit(2.) - wp.lit(1.)))
+              .init(G.SetAttributeModifier(A.VELOCITY, wp.rand(G.VEC3) - wp.lit(0.5)))
+              .init(G.SetAttributeModifier(A.AGE, wp.lit(0.)))
+              .init(G.SetAttributeModifier(A.LIFETIME, wp.lit(float(rng.choice([0.05, 0.1]))).uniform(wp.lit(float(rng.choice([0.3, 0.6]))))))
+              .update(G.EmitSpawnEventModifier(G.ALWAYS, (wp.rand(G.FLOAT) * wp.lit(float(rng.choice([1.0625, 1.25, 1.5])))).cast(G.UINT), 0))
+              .update(G.EmitSpawnEventModifier(G.ON_DIE, wp.lit(G.U32(int(rng.integers(1, 6)))), 1)))
+    children = []
+    for tag in (0, 1):
+        wc = G.ExprWriter()
+        children.append(G.EffectAsset(c_cap, wc.module, name=f"child{tag}")
+                        .init(G.InheritAttributeModifier(A.POSITION))
+                        .init(G.SetAttributeModifier(A.VELOCITY, wc.parent_attr(A.VELOCITY) * wc.lit(0.5 + tag) + (wc.rand(G.VEC3) - wc.lit(0.5))))
+                        .init(G.SetAttributeModifier(A.AGE, wc.lit(0.)))
+                        .init(G.SetAttributeModifier(A.LIFETIME, wc.lit(0.15 + 0.1 * tag)))
+                        .init(G.SetAttributeModifier(A.U32_0, wc.parent_attr(A.ID))))
+    p_fx = parent.generate(num_event_bindings=2, ordered_events=ordered)
+    c_fx = [c.generate(parent=parent) for c in children]
+    dt = 1.0 / 30.0
+    pw = RefWorld(p_cap, p_fx.particle_stride // 4, [Instance(0, p_cap, alive=0, seed=1)], dt=dt)
+    cw = [RefWorld(c_cap, c_fx[0].particle_stride // 4, [Instance(0, c_cap, alive=0, seed=2 + k)], dt=dt) for k in (0, 1)]
+    po, co = EffectOracle(parent), [EffectOracle(c) for c in children]
+    scene = EmuScene([dict(ref=cw[0], lowered=c_fx[0], parent=2, consume=0, child_row=0),
+                      dict(ref=cw[1], lowered=c_fx[1], parent=2, consume=1, child_row=1),
+                      dict(ref=pw, lowered=p_fx, emit=[0, 1], base_child_row=0, ordered=ordered)], [EVENT_CAP, EVENT_CAP], static_emu.build(),
+                     chunks=int(rng.choice([1, 2])), update_ctas=int(rng.integers(1, 4)))
+    events = [np.zeros(EVENT_CAP, dtype=np.uint32) for _ in (0, 1)]
+    event_count, all_emitted = [0, 0], [[], []]
+    for f in range(10):
+        spawn = int(rng.integers(0, p_cap)) if rng.random() < 0.4 else 0
+        seed_p = int(pcg_hash(np.array([seed * 1000 + f], dtype=np.uint32))[0])
+        seed_c = [int(pcg_hash(np.array([seed * 1000 + 500 + 10 * f + k], dtype=np.uint32))[0]) for k in (0, 1)]
+        n_valid = []
+        for k in (0, 1):
+            assert int(scene.child_infos[k, 1]) == event_count[k]
+            nv = min(event_count[k], EVENT_CAP)
+            got = scene.events[k].copy()
+            if ordered:
+                np.testing.assert_array_equal(got[:nv], events[k][:nv], err_msg=f"frame {f} channel {k}: event order")
+            elif event_count[k] <= EVENT_CAP:
+                assert sorted(got[:nv].tolist()) == sorted(events[k][:nv].tolist())
+            else:
+                emitted, kept = Counter(all_emitted[k]), Counter(got.tolist())
+                assert all(kept[p] <= emitted[p] for p in kept)
+            events[k][:nv] = got[:nv]
+            n_valid.append(nv)
+        t = np.float32(f * dt)
+        pw.sim.time = t
+        for k in (0, 1):
+            cw[k].sim.time = t
+            cw[k].set_spawns([0], [seed_c[k]])
+            oracle_child_init(children[k], co[k], cw[k], po, pw, events[k], n_valid[k], seed_c[k])
+        pw.set_spawns([spawn], [seed_p])
+        po.init_pass(pw)
+        event_count = [0, 0]
+        for w in (cw[0], cw[1], pw):
+            w.oracle_indirect(orc)
+            w.oracle_prefix_sum(orc)
+        for k in (0, 1):
+            co[k].update_pass(cw[k])
+        po.update_pass(pw)
+        for channel, counts in po.last_emitted:
+            event_count[channel] = oracle_append_events(pw, counts, events[channel], event_count[channel])
+            rows_read = pw.indirect[:pw.metadata[0].max_update, 1 - pw.metadata[0].indirect_write_index]
+            all_emitted[channel] = np.repeat(rows_read, counts[:len(rows_read)]).tolist()
+        scene.frame_step(pw.sim, [0, 0, spawn], [seed_c[0], seed_c[1], seed_p])
+        for b, world in enumerate((cw[0], cw[1], pw)):
+            got = scene.pull(b)
+            want_md = world.metadata_rows()[0].copy()
+            want_md[5] = b
+            for fld in (7, 8, 9, 10):
+                want_md[fld] = got["metadata"][fld]
+            np.testing.assert_array_equal(got["metadata"], want_md, err_msg=f"frame {f} member {b}: metadata")
+            np.testing.assert_array_equal(got["indirect"], world.indirect, err_msg=f"frame {f} member {b}: lists")
+            np.testing.assert_array_equal(got["particles"], world.particles, err_msg=f"frame {f} member {b}: particles")

@@ -15,7 +15,10 @@ import os
 import subprocess
 from pathlib import Path
 
-from tests.kernel_emu import PRELUDE
+import numpy as np
+
+from oracle import c_oracle as O
+from tests.kernel_emu import PRELUDE, claim
 
 ROOT = Path(__file__).resolve().parent.parent
 KERNELS = ROOT / "bevy_hanabi_b200" / "csrc" / "kernels"
@@ -149,7 +152,8 @@ def _rewrite_shared(text: str) -> str:
     return new
 
 
-def build() -> C.CDLL:
+def build(extra_driver: str = "") -> C.CDLL:
+    """`extra_driver`: more host entry points, compiled after DRIVER (e.g. REPACK_DRIVER)."""
     wgsl = _strip_includes((KERNELS / "hnb_wgsl.cuh").read_text())
     tables = _strip_includes((KERNELS / "hnb_tables.cuh").read_text())
     header = _strip_includes((KERNELS / "hnb_static_kernels.h").read_text())
@@ -163,7 +167,7 @@ def build() -> C.CDLL:
     # k_measure_sm_clock reads %globaltimer: not needed here
     static = re.sub(r"__global__ void k_measure_sm_clock.*?\n}\n", "", static, flags=re.S)
     body = _rewrite_shared(static + "\n" + ribbon)
-    text = PRELUDE + EXTRA_PRELUDE + wgsl + "\n" + tables + "\n" + header + "\n" + body + DRIVER
+    text = PRELUDE + EXTRA_PRELUDE + wgsl + "\n" + tables + "\n" + header + "\n" + body + DRIVER + extra_driver
     OUT.mkdir(parents=True, exist_ok=True)
     tag = hashlib.sha1(text.encode()).hexdigest()[:16]
     cpp, so = OUT / f"static_{tag}.{os.getpid()}.cpp", OUT / f"static_{tag}.so"  # per process: workers may build the same tag at once
@@ -202,3 +206,105 @@ class EventAppendArgs(C.Structure):
     """hnb::EventAppendArgs (hnb_static_kernels.h)"""
     _fields_ = [("counts", C.c_void_p), ("ping", C.c_void_p), ("pong", C.c_void_p), ("spawner", C.c_void_p), ("metadata", C.c_void_p),
                 ("block_sums", C.c_void_p), ("child_infos", C.c_void_p), ("binding", C.c_uint32), ("buffer", C.c_void_p), ("capacity", C.c_uint32)]
+
+
+# ---- hnb_slab_repack ---------------------------------------------------------------------------------------------------
+# Entry points of the repack kernels (build(REPACK_DRIVER))
+REPACK_DRIVER = r"""
+extern "C" void semu_repack_gather(const RepackArgs* a, const void* col, void* scratch, uint32_t width) {
+    RepackArgs r = *a;
+    const unsigned blocks = (r.rows + RP_ROWS_PER_BLOCK - 1) / RP_ROWS_PER_BLOCK;
+    switch (width) {
+    case 4: emu_run([&] { k_repack_gather<1>(r, (const RepackPiece<1>*)col, (RepackPiece<1>*)scratch); }, blocks, RP_THREADS, 8); break;
+    case 8: emu_run([&] { k_repack_gather<2>(r, (const RepackPiece<2>*)col, (RepackPiece<2>*)scratch); }, blocks, RP_THREADS, 8); break;
+    case 16: emu_run([&] { k_repack_gather<4>(r, (const RepackPiece<4>*)col, (RepackPiece<4>*)scratch); }, blocks, RP_THREADS, 8); break;
+    case 32: emu_run([&] { k_repack_gather<8>(r, (const RepackPiece<8>*)col, (RepackPiece<8>*)scratch); }, blocks, RP_THREADS, 8); break;
+    }
+}
+extern "C" void semu_repack_lists(const RepackArgs* a) { RepackArgs r = *a; emu_run([&] { k_repack_lists(r); }, (r.rows + RP_THREADS - 1) / RP_THREADS, RP_THREADS, 8); }
+extern "C" uint32_t semu_sizeof_repack_args(void) { return sizeof(RepackArgs); }
+"""
+
+
+class RepackArgs(C.Structure):
+    """hnb::RepackArgs (hnb_static_kernels.h)"""
+    _fields_ = [("metadata", C.c_void_p), ("ping", C.c_void_p), ("pong", C.c_void_p), ("dead", C.c_void_p), ("alive_bits", C.c_void_p),
+                ("claim", C.c_void_p), ("first", C.c_uint32), ("rows", C.c_uint32)]
+
+
+def physical_widths(stride: int, sector: bool):
+    """Byte widths of a slab's physical columns (effect_source.cpp physical_planes)."""
+    pieces, off = [], 0
+    while off < stride:
+        w = 16 if stride - off >= 16 else (8 if stride - off >= 8 else 4)
+        pieces.append(w)
+        off += w
+    if not sector:
+        return pieces
+    out, p = [], 0
+    while p < len(pieces):
+        if p + 1 < len(pieces) and pieces[p] == pieces[p + 1] == 16:
+            out.append(32)
+            p += 2
+        else:
+            out.append(pieces[p])
+            p += 1
+    return out
+
+
+class SoaSlab:
+    """A slab in the device's layout (one array per physical column, ping / pong / dead, alive bitmap, claim words),
+    made from and read back into a RefWorld's reference layouts."""
+
+    def __init__(self, ref: RefWorld, sector: bool, rng):
+        self.widths = physical_widths(ref.stride_words * 4, sector)
+        self.planes, off = [], 0
+        for w in self.widths:
+            self.planes.append(np.ascontiguousarray(ref.particles[:, off:off + w // 4]).reshape(-1).copy())
+            off += w // 4
+        self.cols = [np.ascontiguousarray(ref.indirect[:, c]).copy() for c in range(3)]
+        self.bits = rng.integers(0, 1 << 32, ref.slab_rows // 32 + 2, dtype=np.uint64).astype(np.uint32)
+        self.claims = np.array([claim(5, 7), claim(9, 11)], dtype=np.uint64)
+        self.metadata = (O.EffectMetadata * len(ref.instances)).from_buffer_copy(bytes(ref.metadata))
+
+    def repack(self, lib, i: int, first: int, rows: int):
+        emulate_repack(lib, self.planes, self.widths, self.cols, self.bits, self.claims, self.metadata, i, first, rows)
+
+    def particles(self):
+        return np.concatenate([p.reshape(-1, w // 4) for p, w in zip(self.planes, self.widths)], axis=1)
+
+    def indirect(self):
+        return np.stack(self.cols, axis=1)
+
+
+def emulate_repack(lib, planes, widths, cols, bits, claims, metadata, i, first, rows):
+    """hnb_slab_repack's device work, in its order."""
+    a = RepackArgs(C.addressof(metadata[i]), cols[0].ctypes.data, cols[1].ctypes.data, cols[2].ctypes.data, bits.ctypes.data,
+                   claims.ctypes.data, first, rows)
+    scratch = np.zeros(rows * 8 + 8, dtype=np.uint32)
+    for plane, w in zip(planes, widths):
+        k = w // 4
+        lib.semu_repack_gather(C.byref(a), plane.ctypes.data, scratch.ctypes.data, w)
+        plane[first * k:(first + rows) * k] = scratch[:rows * k]
+    lib.semu_repack_lists(C.byref(a))
+
+
+def expected_bits(bits, first, rows, n):
+    b = np.unpackbits(bits.view(np.uint8), bitorder="little").copy()
+    b[first:first + n] = 1
+    b[first + n:first + rows] = 0
+    return np.packbits(b, bitorder="little").view(np.uint32)
+
+
+def churned(rng, ref, i, n, w):
+    """Instance `i` in a state the update invariant allows: column `w` lists n distinct local slots, the dead stack holds
+    the other slots (global values) in a shuffled order from row n up; every other index word is garbage."""
+    inst = ref.instances[i]
+    first, rows = inst.slab_offset, inst.capacity
+    perm = rng.permutation(rows).astype(np.uint32)
+    garbage = lambda k: rng.integers(0, 1 << 32, k, dtype=np.uint64).astype(np.uint32)  # noqa: E731
+    ref.indirect[first:first + rows, w] = np.concatenate([perm[:n], garbage(rows - n)])
+    ref.indirect[first:first + rows, 1 - w] = garbage(rows)
+    ref.indirect[first:first + rows, 2] = np.concatenate([garbage(n), perm[n:] + np.uint32(first)])
+    md = ref.metadata[i]
+    md.alive_count, md.max_spawn, md.indirect_write_index = n, rows - n, w

@@ -513,8 +513,8 @@ def test_matrix_property_layout_limits():
 
 
 def test_matrix_effect_compiles_for_sm100a():
-    from tests.test_host_exec_cpu import _matrix_asset
-    src = _matrix_asset(1024).generate().generate_source()
+    from tests.effects import matrix_asset
+    src = matrix_asset(1024).generate().generate_source()
     assert "mat2x3f(1.f,0.5f,0.25f,-0.5f,1.f,2.f)" in src
     size, log = R.nvrtc_check(src)
     assert size > 0 and "error" not in log.lower() and " 0 bytes spill stores" in log

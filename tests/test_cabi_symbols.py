@@ -76,3 +76,12 @@ def test_product_does_not_import_oracle():
     for src in (ROOT / "bevy_hanabi_b200" / "csrc").rglob("*"):
         if src.is_file() and src.suffix in (".cpp", ".cu", ".cuh", ".h"):
             assert "vfx_oracle" not in src.read_text(), src
+
+
+def test_no_module_imports_a_test_module():
+    """Shared test code lives in tests/helpers.py, tests/effects.py and the emulation modules: a test or tool that imports
+    a test module changes whenever that module's private helpers do."""
+    pattern = re.compile(r"^\s*(from\s+(tests)?\.test_\w*\s+import|import\s+tests\.test_|from\s+(tests|\.)\s+import\s+\(?[\w\s,]*\btest_)", re.M)
+    for py in [*(ROOT / "tests").rglob("*.py"), *(ROOT / "tools").rglob("*.py")]:
+        m = pattern.search(py.read_text())
+        assert m is None, f"{py.relative_to(ROOT)}: {m.group(0).strip()}"

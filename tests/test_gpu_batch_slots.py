@@ -24,8 +24,8 @@ import pytest
 from bevy_hanabi_b200 import _native as N, graph as G, recipes
 from oracle import c_oracle as O
 from oracle.hanabi_oracle import EffectOracle
+from tests.effects import ACCEL_DRAG, drifting_sparks
 from tests.helpers import RefWorld
-from tests.test_gpu_update_c5 import ACCEL_DRAG
 
 pytestmark = pytest.mark.gpu
 A = G.Attribute
@@ -33,17 +33,6 @@ EPOCH_MASK = 0x3FFFFFFF
 ORDERS = ["default", "slot", "relaxed"]
 # relaxed order hands out recycled slots in a scheduling-dependent order, so the spawning effect runs in the other two
 ORDER_KIND = [(o, "c5") for o in ORDERS] + [("default", "sparks"), ("slot", "sparks")]
-
-
-def _sparks(capacity):
-    w = G.ExprWriter()
-    return (G.EffectAsset(capacity, w.module, name="sparks_batch_slots")
-            .init(G.SetAttributeModifier(A.POSITION, w.rand(G.VEC3) * w.lit(2.) - w.lit(1.)))
-            .init(G.SetAttributeModifier(A.VELOCITY, w.rand(G.VEC3) * w.lit(2.) - w.lit(1.)))
-            .init(G.SetAttributeModifier(A.AGE, w.lit(0.)))
-            .init(G.SetAttributeModifier(A.LIFETIME, w.lit(0.05).uniform(w.lit(0.4))))
-            .update(G.AccelModifier(w.lit(G.Vec3(0., -9.8, 0.))))
-            .update(G.LinearDragModifier(w.lit(0.5))))
 
 
 class Scene:
@@ -73,7 +62,7 @@ class Scene:
             lowered = recipes.c5_lowered(relaxed_order=order == "relaxed", slot_order=order == "slot")
             eo = None
         else:
-            asset = _sparks(4096)
+            asset = drifting_sparks(4096, name="sparks_batch_slots", lifetime=(0.05, 0.4))
             lowered = asset.generate(relaxed_order=order == "relaxed", slot_order=order == "slot")
             eo = EffectOracle(asset)
         self.effects[name] = dict(kind=kind, order=order, handle=self.ctx.effect_compile(lowered), oracle=eo, stride=lowered.particle_stride)

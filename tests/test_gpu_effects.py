@@ -11,65 +11,12 @@ import numpy as np
 import pytest
 
 from bevy_hanabi_b200 import graph as G
-from oracle.hanabi_oracle import EffectOracle
-from tests.helpers import GpuWorld, Instance, RefWorld, assert_world_equal
+from oracle.hanabi_oracle import pcg_hash
+from tests.effects import firework_trails, force_field
+from tests.helpers import Instance, Lockstep, RefWorld
 
 pytestmark = pytest.mark.gpu
 A = G.Attribute
-
-
-def _float_word_mask(asset):
-    """(boolean mask over the AoS words, [(first_word, component_count)] of the fp32 attributes)"""
-    fields, size, _ = asset.particle_layout()
-    mask = np.zeros(size // 4, dtype=bool)
-    attrs = []
-    for f in fields:
-        if not f.name.startswith("pad") and G.vt_elem(f.vt) == "f":
-            mask[f.offset // 4: f.offset // 4 + G.vt_count(f.vt)] = True
-            attrs.append((f.offset // 4, G.vt_count(f.vt)))
-    return mask, attrs
-
-
-def _run(ctx, orc, asset, ref, frames, spawns, rtol=0.0, props=None, seeds=None, check_every=1, relaxed=False, fast_math=False):
-    """spawns: callable frame -> list of per-instance spawn counts. props: per-instance dict of property values."""
-    blobs = None
-    if props is not None:
-        blobs = [asset.serialize_properties(p) for p in props]
-        for i in range(len(ref.instances)):
-            ref.metadata[i].properties_array_index = i
-    eo = EffectOracle(asset, {i: p for i, p in enumerate(props)} if props else None)
-    gpu = GpuWorld(ctx, ref, asset.generate(relaxed_order=relaxed, fast_math=fast_math), property_blobs=blobs)
-    mask, fattrs = _float_word_mask(asset)
-    for f in range(frames):
-        ref.sim.time = np.float32(f) * ref.sim.delta_time
-        ref.sim.virtual_time = ref.sim.time
-        ref.sim.real_time = ref.sim.time
-        ref.set_spawns(spawns(f), seeds(f) if seeds else None)
-        eo.frame(ref, orc)
-        gpu.frame()
-        if f % check_every == 0 or f == frames - 1:
-            got = gpu.pull()
-            if relaxed:
-                _assert_relaxed_equal(ref, got, mask, rtol)
-            else:
-                assert_world_equal(ref, got, float_words=mask if rtol else None, rtol=rtol, what=f"frame {f}", float_attrs=fattrs)
-                if rtol:
-                    # the 1e-5 bound is a PER-STEP bound: libm-level differences are amplified from frame to frame by
-                    # non-smooth dynamics (sign / min / kill thresholds), so restart every frame from identical state
-                    ctx.slab_upload_aos(gpu.slab, 0, ref.particles)
-    return gpu, eo
-
-
-def _assert_relaxed_equal(ref, got, mask, rtol):
-    """RELAXED_ORDER: counts exact, lists equal as sets per segment, particles identical."""
-    np.testing.assert_array_equal(got["metadata"], ref.metadata_rows())
-    np.testing.assert_array_equal(got["draw"], ref.draw)
-    for i, inst in enumerate(ref.instances):
-        md = ref.metadata[i]
-        base, alive, W = inst.slab_offset, md.alive_count, md.indirect_write_index
-        assert sorted(got["indirect"][base:base + alive, W].tolist()) == sorted(ref.indirect[base:base + alive, W].tolist())
-        assert sorted(got["indirect"][base + alive:base + inst.capacity, 2].tolist()) == sorted(ref.indirect[base + alive:base + inst.capacity, 2].tolist())
-    np.testing.assert_array_equal(got["particles"], ref.particles)
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -82,84 +29,51 @@ def test_c1_single_particle_plumbing(ctx, orc):
              .init(G.SetAttributeModifier(A.SIZE3, w.lit(G.Vec3(10., 10., 10.)))))
     fields, size, _ = asset.particle_layout()
     ref = RefWorld(16, size // 4, [Instance(0, 16, alive=0, seed=0)])
-    _run(ctx, orc, asset, ref, 40, lambda f: [17 if f % 2 else 3])
+    Lockstep(ctx, orc, ref, asset).run([[17 if f % 2 else 3] for f in range(40)])
     assert ref.metadata[0].alive_count == 16 and ref.metadata[0].max_spawn == 0
     assert ref.metadata[0].particle_counter == 16
-
-
-def _firework_trails(capacity):
-    """BASELINE config C2 (examples/firework.rs:184-251 made parent-less, SURVEY §8d)."""
-    w = G.ExprWriter()
-    vel = (w.rand(G.VEC3) * w.lit(2.) - w.lit(1.)).normalize() * w.lit(40.).uniform(w.lit(60.))
-    return (G.EffectAsset(capacity, w.module, name="firework_trails")
-            .init(G.SetAttributeModifier(A.POSITION, w.lit(G.Vec3(0, 0, 0))))
-            .init(G.SetAttributeModifier(A.VELOCITY, vel))
-            .init(G.SetAttributeModifier(A.AGE, w.lit(0.)))
-            .init(G.SetAttributeModifier(A.LIFETIME, w.lit(0.8).uniform(w.lit(1.2))))
-            .init(G.SetAttributeModifier(A.COLOR, w.lit(G.U32(0xFFFFFFFF))))
-            .update(G.LinearDragModifier(w.lit(4.)))
-            .update(G.AccelModifier(w.lit(G.Vec3(0., -16., 0.)))))
 
 
 def test_c2_firework_bursts_with_recycling(ctx, orc):
     """Bursts of 1000 every 20 frames at dt=1/20: particles live 16-24 frames, so dead slots are recycled by later
     bursts and the dead stack / alive lists are permuted. Every operation is IEEE-exact: zero tolerance."""
-    asset = _firework_trails(4096)
+    asset = firework_trails(4096)
     _, size, _ = asset.particle_layout()
     assert size == 48
     ref = RefWorld(4096, size // 4, [Instance(0, 4096, alive=0)], dt=1.0 / 20.0)
-    from oracle.hanabi_oracle import pcg_hash
-    seeds = lambda f: [int(pcg_hash(np.array([0x1234 + f], dtype=np.uint32))[0])]
-    _run(ctx, orc, asset, ref, 70, lambda f: [1000 if f % 20 == 0 else 0], seeds=seeds)
+    seeds = lambda n, f: [int(pcg_hash(np.array([0x1234 + f], dtype=np.uint32))[0])]
+    Lockstep(ctx, orc, ref, asset, seeds=seeds).run([[1000 if f % 20 == 0 else 0] for f in range(70)])
     assert ref.metadata[0].particle_counter == 4000
 
 
 def test_c2_relaxed_order_same_sets(ctx, orc):
     """HNB_EFFECT_RELAXED_ORDER (reference-style atomics): counts and per-segment index SETS must be identical."""
-    asset = _firework_trails(2048)
+    asset = firework_trails(2048)
     ref = RefWorld(2048, 12, [Instance(0, 2048, alive=0)], dt=1.0 / 20.0)
-    _run(ctx, orc, asset, ref, 24, lambda f: [700 if f % 12 == 0 else 0], relaxed=True, check_every=3)
-
-
-def _force_field(capacity, aabb_half=(3., 2., 3.), kill_center=(-2., 1., 0.), kill_r2=0.36):
-    """BASELINE config C3 (examples/force_field.rs:126-203 scaled): sphere spawn, two ConformToSphere, two kills.
-    (The kill volumes are parameters so that a test can make them bite within a few frames.)"""
-    w = G.ExprWriter()
-    attractor = w.add_property("attraction_accel", 20.0)
-    repulsor = w.add_property("repulsor_position", G.Vec3(0.2, 0.6, 0.))
-    m = (G.EffectAsset(capacity, w.module, name="force_field")
-         .init(G.SetPositionSphereModifier(w.lit(G.Vec3(0, 0, 0)), w.lit(0.05), G.SURFACE))
-         .init(G.SetVelocitySphereModifier(w.lit(G.Vec3(0, 0, 0)), w.rand() * w.lit(0.2) + w.lit(0.1)))
-         .init(G.SetAttributeModifier(A.AGE, w.lit(0.)))
-         .init(G.SetAttributeModifier(A.LIFETIME, w.lit(10.)))
-         .update(G.ConformToSphereModifier(w.prop(repulsor), w.lit(0.2), w.lit(0.4), w.lit(-10.), w.lit(-2.), w.lit(0.1), w.lit(2.)))
-         .update(G.ConformToSphereModifier(w.lit(G.Vec3(0.6, -0.2, 0.)), w.lit(0.3), w.lit(30.), w.prop(attractor), w.lit(5.)))
-         .update(G.KillAabbModifier(w.lit(G.Vec3(0, 0, 0)), w.lit(G.Vec3(*aabb_half))))
-         .update(G.KillSphereModifier(w.lit(G.Vec3(*kill_center)), w.lit(kill_r2), True)))
-    return m
+    Lockstep(ctx, orc, ref, asset, relaxed=True).run([[700 if f % 12 == 0 else 0] for f in range(24)], check_every=3)
 
 
 def test_c3_force_field(ctx, orc):
-    asset = _force_field(8192)
+    asset = force_field(8192)
     _, size, _ = asset.particle_layout()
     ref = RefWorld(8192, size // 4, [Instance(0, 8192, alive=0, seed=77)])
     props = [{"attraction_accel": 18.0, "repulsor_position": G.Vec3(0.25, 0.5, 0.1)}]
-    _run(ctx, orc, asset, ref, 25, lambda f: [5000 if f == 0 else (30 if f % 5 == 0 else 0)], rtol=1e-5, props=props)
+    Lockstep(ctx, orc, ref, asset, rtol=1e-5, props=props).run([[5000 if f == 0 else (30 if f % 5 == 0 else 0)] for f in range(25)])
 
 
 def test_fast_math_effects_stay_within_tolerance(ctx, orc):
     """HNB_EFFECT_FAST_MATH (FMA contraction, approximate division / square root): fp32 attributes within the 1e-5
     per-step bound of BASELINE.json, every integer structure still exact."""
     from bevy_hanabi_b200 import _native as N
-    asset = _force_field(8192)
+    asset = force_field(8192)
     assert asset.generate(fast_math=True).flags & N.EFFECT_FAST_MATH
     _, size, _ = asset.particle_layout()
     ref = RefWorld(8192, size // 4, [Instance(0, 8192, alive=0, seed=77)])
     props = [{"attraction_accel": 18.0, "repulsor_position": G.Vec3(0.25, 0.5, 0.1)}]
-    _run(ctx, orc, asset, ref, 25, lambda f: [5000 if f == 0 else (30 if f % 5 == 0 else 0)], rtol=1e-5, props=props, fast_math=True)
-    asset = _firework_trails(4096)
+    Lockstep(ctx, orc, ref, asset, rtol=1e-5, props=props, fast_math=True).run([[5000 if f == 0 else (30 if f % 5 == 0 else 0)] for f in range(25)])
+    asset = firework_trails(4096)
     ref = RefWorld(4096, 12, [Instance(0, 4096, alive=0)], dt=1.0 / 20.0)
-    _run(ctx, orc, asset, ref, 30, lambda f: [1000 if f % 20 == 0 else 0], rtol=1e-5, fast_math=True)
+    Lockstep(ctx, orc, ref, asset, rtol=1e-5, fast_math=True).run([[1000 if f % 20 == 0 else 0] for f in range(30)])
 
 
 def test_many_instances_properties_transforms(ctx, orc):
@@ -189,7 +103,7 @@ def test_many_instances_properties_transforms(ctx, orc):
     props = [{"speed": 0.5 + 0.25 * i, "tint": G.U32(0x01010101 * (i % 200))} for i in range(n_inst)]
     rng = np.random.default_rng(4)
     sched = [[int(x) for x in rng.integers(0, 40, n_inst)] for _ in range(45)]
-    _run(ctx, orc, asset, ref, 45, lambda f: sched[f], props=props, check_every=3)
+    Lockstep(ctx, orc, ref, asset, props=props).run(sched, check_every=3)
     assert all(ref.metadata[i].particle_counter > 0 for i in range(n_inst))
 
 
@@ -219,7 +133,7 @@ def test_shapes_and_transformed_velocities(ctx, orc):
         rows = [1.5 * c, -1.5 * s, 0., 4.,   1.5 * s, 1.5 * c, 0., -1.,   0., 0., 0.5, 2.]
         for k in range(12):
             ref.spawners[0].transform[k] = rows[k]
-        _run(ctx, orc, a, ref, 6, lambda f: [2000 if f == 0 else 100], rtol=1e-5)
+        Lockstep(ctx, orc, ref, a, rtol=1e-5).run([[2000 if f == 0 else 100] for f in range(6)])
 
 
 def test_expression_operators_end_to_end(ctx, orc):
@@ -243,7 +157,7 @@ def test_expression_operators_end_to_end(ctx, orc):
              .update(G.SetAttributeModifier(A.F32X2_0, pos.x().vec2(pos.z()).sign() * w.lit(G.Vec2(2., 3.)))))
     _, size, _ = asset.particle_layout()
     ref = RefWorld(2000, size // 4, [Instance(0, 2000, alive=0, seed=5)])
-    _run(ctx, orc, asset, ref, 4, lambda f: [1500 if f == 0 else 0])
+    Lockstep(ctx, orc, ref, asset).run([[1500 if f == 0 else 0] for f in range(4)])
 
 
 def test_transcendental_operators(ctx, orc):
@@ -257,4 +171,4 @@ def test_transcendental_operators(ctx, orc):
              .update(G.SetAttributeModifier(A.F32_3, x.atan2(w.lit(2.)) + w.lit(0.).normal(w.lit(1.)) + x.inverse_sqrt() + x.round() + x.ceil())))
     _, size, _ = asset.particle_layout()
     ref = RefWorld(1500, size // 4, [Instance(0, 1500, alive=0, seed=99)])
-    _run(ctx, orc, asset, ref, 3, lambda f: [1500 if f == 0 else 0], rtol=1e-5)
+    Lockstep(ctx, orc, ref, asset, rtol=1e-5).run([[1500 if f == 0 else 0] for f in range(3)])

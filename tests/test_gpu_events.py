@@ -6,79 +6,16 @@ parent particle (InheritAttributeModifier, src/modifier/attr.rs:173-186).
 Like in the reference, the ORDER in which events land in the buffer depends on atomic scheduling, so the event
 buffer — and therefore which child slot receives which event — is compared as a multiset; counts are exact.
 """
-from collections import Counter
-
 import numpy as np
 import pytest
 
 from bevy_hanabi_b200 import _native as N
-from bevy_hanabi_b200 import graph as G
 from bevy_hanabi_b200 import runtime as R
-from oracle.hanabi_oracle import EffectOracle, Env, Rng, Writer, apply_modifier, pcg_hash
-from tests.helpers import Instance, RefWorld
+from oracle.hanabi_oracle import EffectOracle, pcg_hash
+from tests.effects import EVENT_CAP, event_assets
+from tests.helpers import Instance, RefWorld, emitter_scene, oracle_append_events, oracle_child_init
 
 pytestmark = pytest.mark.gpu
-A = G.Attribute
-EVENT_CAP = 256  # the reference hard-codes 256 events per child (event.rs:266-267)
-
-
-def _assets():
-    wp = G.ExprWriter()
-    parent = (G.EffectAsset(512, wp.module, name="rocket")
-              .init(G.SetAttributeModifier(A.POSITION, wp.rand(G.VEC3) * wp.lit(8.) - wp.lit(4.)))
-              .init(G.SetAttributeModifier(A.VELOCITY, wp.lit(G.Vec3(0., 3., 0.))))
-              .init(G.SetAttributeModifier(A.AGE, wp.lit(0.)))
-              .init(G.SetAttributeModifier(A.LIFETIME, wp.lit(0.05).uniform(wp.lit(0.4))))
-              .update(G.EmitSpawnEventModifier(G.ON_DIE, wp.lit(G.U32(3)), 0)))
-    wc = G.ExprWriter()
-    child = (G.EffectAsset(2048, wc.module, name="sparks")
-             .init(G.InheritAttributeModifier(A.POSITION))
-             .init(G.SetAttributeModifier(A.VELOCITY, wc.parent_attr(A.VELOCITY) * wc.lit(-0.5) + (wc.rand(G.VEC3) - wc.lit(0.5))))
-             .init(G.SetAttributeModifier(A.AGE, wc.lit(0.)))
-             .init(G.SetAttributeModifier(A.LIFETIME, wc.lit(0.3)))
-             .init(G.SetAttributeModifier(A.U32_0, wc.parent_attr(A.ID))))
-    return parent, child
-
-
-
-def _oracle_child_init(child, co, cw, po, pw, events, n_valid, seed_c):
-    """Child init from GPU spawn events (vfx_init.wgsl:123-171): one thread per event, capped by max_spawn; reads
-    the parent particle the event names. Returns the number of children spawned."""
-    md = cw.metadata[0]
-    n = min(n_valid, md.max_spawn)
-    if not n:
-        return 0
-    k = np.arange(n, dtype=np.int64)
-    alive_index = md.alive_count + k
-    slots = cw.indirect[alive_index, 2].astype(np.int64)
-    pidx = slots.astype(np.uint32)
-    parent_idx = events[:n].astype(np.uint32)
-    parent_rec = po.unpack(pw.particles[parent_idx.astype(np.int64)].copy())
-    rec = np.zeros((n, co.stride_words), dtype=np.uint32)
-    P = co.unpack(rec)
-    env = Env(n, P, cw.sim, Rng(pcg_hash(pidx ^ np.uint32(seed_c))), {}, pidx, (md.particle_counter + k).astype(np.uint32),
-              np.array(list(cw.spawners[0].transform), dtype=np.float32).reshape(3, 4), parent=parent_rec, parent_particle_index=parent_idx)
-    wr = Writer()
-    for m in child.init_modifiers:
-        apply_modifier(m, child.module, env, wr)
-    co.pack(P, rec)
-    cw.indirect[alive_index, md.indirect_write_index] = pidx
-    cw.particles[pidx.astype(np.int64)] = rec
-    md.alive_count += n
-    md.particle_counter += n
-    return n
-
-
-def _oracle_append_events(pw, counts, events, event_count):
-    """append_spawn_events_N in serial thread order (lib.rs:976-993); returns the new event_count."""
-    pidx_rows = pw.indirect[:pw.metadata[0].max_update, 1 - pw.metadata[0].indirect_write_index]
-    for row in np.nonzero(counts)[0]:
-        c = int(counts[row])
-        base = min(event_count, EVENT_CAP)
-        event_count += c
-        capped = min(c, EVENT_CAP - base)
-        events[base:base + capped] = pidx_rows[row]
-    return event_count
 
 
 def _sorted_rows(a):
@@ -86,7 +23,7 @@ def _sorted_rows(a):
 
 
 def test_parent_emits_child_consumes(ctx, orc):
-    parent, child = _assets()
+    parent, child = event_assets()
     p_fx = parent.generate(num_event_bindings=1)
     c_fx = child.generate(parent=parent)
     assert p_fx.flags & N.EFFECT_EMIT_GPU_SPAWN_EVENTS
@@ -145,7 +82,7 @@ def test_parent_emits_child_consumes(ctx, orc):
         pw.set_spawns([spawn], [seed_p])
         cw.set_spawns([0], [seed_c])
         po.init_pass(pw)
-        total_child_spawned += _oracle_child_init(child, co, cw, po, pw, events, n_valid, seed_c)
+        total_child_spawned += oracle_child_init(child, co, cw, po, pw, events, n_valid, seed_c)
         # indirect + prefix for both worlds, events cleared (vfx_indirect.wgsl:38-46)
         event_count = 0
         for w in (pw, cw):
@@ -155,7 +92,7 @@ def test_parent_emits_child_consumes(ctx, orc):
         co.update_pass(cw)
         for channel, counts in po.last_emitted:
             assert channel == 0
-            event_count = _oracle_append_events(pw, counts, events, event_count)
+            event_count = oracle_append_events(pw, counts, events, event_count)
 
         # ----- compare
         ctx.sync()
@@ -182,118 +119,4 @@ def test_two_children_two_conditions(ctx, orc):
     count 0 or 1 drawn per particle), channel 1 by dying particles (OnDie, 4 events each). Each child consumes its
     own buffer the frame after. Children come BEFORE the parent in batch order, as EffectSorter places them
     (batch.rs:599-603), so a child's init reads the parent's records before the parent's init recycles slots."""
-    wp = G.ExprWriter()
-    parent = (G.EffectAsset(1024, wp.module, name="emitter")
-              .init(G.SetAttributeModifier(A.POSITION, wp.rand(G.VEC3) * wp.lit(2.) - wp.lit(1.)))
-              .init(G.SetAttributeModifier(A.VELOCITY, wp.rand(G.VEC3) - wp.lit(0.5)))
-              .init(G.SetAttributeModifier(A.AGE, wp.lit(0.)))
-              .init(G.SetAttributeModifier(A.LIFETIME, wp.lit(0.1).uniform(wp.lit(0.5))))
-              .update(G.EmitSpawnEventModifier(G.ALWAYS, (wp.rand(G.FLOAT) * wp.lit(1.25)).cast(G.UINT), 0))
-              .update(G.EmitSpawnEventModifier(G.ON_DIE, wp.lit(G.U32(4)), 1)))
-    children = []
-    for tag in (0, 1):
-        wc = G.ExprWriter()
-        children.append(G.EffectAsset(4096, wc.module, name=f"child{tag}")
-                        .init(G.InheritAttributeModifier(A.POSITION))
-                        .init(G.SetAttributeModifier(A.VELOCITY, wc.parent_attr(A.VELOCITY) * wc.lit(0.25 + tag) + (wc.rand(G.VEC3) - wc.lit(0.5))))
-                        .init(G.SetAttributeModifier(A.AGE, wc.lit(0.)))
-                        .init(G.SetAttributeModifier(A.LIFETIME, wc.lit(0.2 + 0.1 * tag)))
-                        .init(G.SetAttributeModifier(A.U32_0, wc.parent_attr(A.ID))))
-    p_fx = parent.generate(num_event_bindings=2)
-    c_fx = [c.generate(parent=parent) for c in children]
-    p_stride, c_stride = p_fx.particle_stride, c_fx[0].particle_stride
-    dt = 1.0 / 30.0
-    pw = RefWorld(1024, p_stride // 4, [Instance(0, 1024, alive=0, seed=1)], dt=dt)
-    cw = [RefWorld(4096, c_stride // 4, [Instance(0, 4096, alive=0, seed=2 + k)], dt=dt) for k in (0, 1)]
-    po, co = EffectOracle(parent), [EffectOracle(c) for c in children]
-    events = [np.zeros(EVENT_CAP, dtype=np.uint32) for _ in (0, 1)]
-    event_count = [0, 0]
-
-    # GPU tables: rows 0, 1 = children (batches 0, 1), row 2 = parent (batch 2); child infos 0, 1 = channels 0, 1
-    p_slab = ctx.slab_create(1024, p_stride)
-    c_slab = [ctx.slab_create(4096, c_stride) for _ in (0, 1)]
-    p_eff = ctx.effect_compile(p_fx)
-    c_eff = [ctx.effect_compile(fx) for fx in c_fx]
-    evbuf = [ctx.event_buffer_create(EVENT_CAP) for _ in (0, 1)]
-    for k in (0, 1):
-        ctx.child_info_insert(k, 0, 0)
-        md_c = R.initial_metadata(4096, k, c_stride // 4)
-        md_c.global_child_index, md_c.local_child_index = k, k
-        ctx.metadata_insert(k, md_c)
-        ctx.draw_args_insert(k)
-    md_p = R.initial_metadata(1024, 2, p_stride // 4)
-    md_p.base_child_index = 0
-    ctx.metadata_insert(2, md_p)
-    ctx.draw_args_insert(2)
-
-    spawn_sched = [700, 0, 0, 150, 0, 0, 0, 800, 0, 0, 0, 0, 100, 0, 0, 0, 0, 0, 0, 0]
-    spawned = [0, 0]
-    overflowed = False
-    seen_counts = []
-    all_emitted = [[], []]
-    for f, spawn in enumerate(spawn_sched):
-        seed_p = int(pcg_hash(np.array([5000 + f], dtype=np.uint32))[0])
-        seed_c = [int(pcg_hash(np.array([6000 + 10 * f + k], dtype=np.uint32))[0]) for k in (0, 1)]
-        ctx.upload_spawners([R.make_spawner(spawn=0, seed=seed_c[k], effect_metadata_index=k, draw_indirect_index=k, slab_offset=0, parent_slab_offset=0)
-                             for k in (0, 1)]
-                            + [R.make_spawner(spawn=spawn, seed=seed_p, effect_metadata_index=2, draw_indirect_index=2, slab_offset=0)])
-        ctx.upload_batches([N.BatchInfo(0, 0, 0, 0, 0, 1), N.BatchInfo(0, 0, 1, 0, 1, 1), N.BatchInfo(0, 0, 2, 0, 2, 1)], [0, 0, 0])
-        ctx.set_sim_params(dt, f * dt, 3)
-        # what the previous frame's update left in the two buffers
-        n_valid = []
-        for k in (0, 1):
-            assert ctx.read_child_info(k).event_count == event_count[k], f"frame {f} channel {k}"
-            nv = min(event_count[k], EVENT_CAP)
-            overflowed |= event_count[k] > EVENT_CAP
-            seen_counts.append(event_count[k])
-            got = ctx.event_buffer_download(evbuf[k], 0, EVENT_CAP)
-            if event_count[k] <= EVENT_CAP:
-                assert sorted(got[:nv].tolist()) == sorted(events[k][:nv].tolist())
-            else:
-                # overflow: WHICH appends hit the cap depends on atomic order (lib.rs:980-986), on the reference too;
-                # what is defined is that the buffer is full of events that were really emitted
-                emitted, kept = Counter(all_emitted[k]), Counter(got.tolist())
-                assert all(kept[p] <= emitted[p] for p in kept), f"frame {f} channel {k}: event that nobody emitted"
-            events[k][:nv] = got[:nv]   # consume in the GPU buffer's order (the reference's order is unspecified)
-            n_valid.append(nv)
-        ctx.simulate([N.BatchLaunch.make(c_eff[0], c_slab[0], 0, 0, parent_slab=p_slab, consume_events=evbuf[0]),
-                      N.BatchLaunch.make(c_eff[1], c_slab[1], 1, 0, parent_slab=p_slab, consume_events=evbuf[1]),
-                      N.BatchLaunch.make(p_eff, p_slab, 2, spawn, emit_events=evbuf)])
-
-        # ----- oracle frame: inits (children read the parent's records as the previous frame left them), ...
-        t = np.float32(f * dt)
-        pw.sim.time = t
-        for k in (0, 1):
-            cw[k].sim.time = t
-            cw[k].set_spawns([0], [seed_c[k]])
-            spawned[k] += _oracle_child_init(children[k], co[k], cw[k], po, pw, events[k], n_valid[k], seed_c[k])
-        pw.set_spawns([spawn], [seed_p])
-        po.init_pass(pw)
-        # ... indirect (clears the event counts, vfx_indirect.wgsl:38-46) + prefix sums, updates, event appends
-        event_count = [0, 0]
-        for w in (cw[0], cw[1], pw):
-            w.oracle_indirect(orc)
-            w.oracle_prefix_sum(orc)
-        for k in (0, 1):
-            co[k].update_pass(cw[k])
-        po.update_pass(pw)
-        assert [ch for ch, _ in po.last_emitted] == [0, 1]
-        for channel, counts in po.last_emitted:
-            event_count[channel] = _oracle_append_events(pw, counts, events[channel], event_count[channel])
-            rows_read = pw.indirect[:pw.metadata[0].max_update, 1 - pw.metadata[0].indirect_write_index]
-            all_emitted[channel] = np.repeat(rows_read, counts[:len(rows_read)]).tolist()
-
-        # ----- compare
-        ctx.sync()
-        for world, slab, row, stride, rows in ((cw[0], c_slab[0], 0, c_stride, 4096), (cw[1], c_slab[1], 1, c_stride, 4096), (pw, p_slab, 2, p_stride, 1024)):
-            m_gpu = np.frombuffer(bytes(ctx.read_metadata(row)), dtype=np.uint32)
-            m_ref = world.metadata_rows()[0].copy()
-            m_ref[5] = row
-            for fld in (7, 8, 9, 10):
-                m_ref[fld] = m_gpu[fld]
-            np.testing.assert_array_equal(m_gpu, m_ref, err_msg=f"frame {f} metadata row {row}")
-            assert ctx.read_draw_args(row).instance_count == world.draw[1]
-            np.testing.assert_array_equal(ctx.slab_download_indirect(slab, 0, rows), world.indirect, err_msg=f"frame {f} row {row}: lists")
-            np.testing.assert_array_equal(ctx.slab_download_aos(slab, 0, rows, stride), world.particles, err_msg=f"frame {f} row {row}: particles")
-    assert spawned[0] > 100 and spawned[1] > 100, spawned
-    assert overflowed and min(seen_counts[2:]) < EVENT_CAP, f"the scenario must both overflow an event buffer (capped appends) and not: {seen_counts}"
+    emitter_scene(ctx, orc, 1024, ordered=False)

@@ -8,15 +8,16 @@ import numpy as np
 import pytest
 
 from bevy_hanabi_b200 import recipes
-from tests.helpers import GpuWorld, Instance, RefWorld, assert_world_equal
-from tests.test_gpu_update_c5 import ACCEL_DRAG, _fill
+from oracle.hanabi_oracle import pcg_hash
+from tests.effects import ACCEL_DRAG, fill_c5, firework_trails
+from tests.helpers import GpuWorld, Instance, Lockstep, RefWorld, assert_world_equal
 
 pytestmark = pytest.mark.gpu
 
 
 def _world(batches=None):
     ref = RefWorld(3 * 4096, 8, [Instance(0, 4096, alive=4000, seed=1), Instance(4096, 4096, alive=1, seed=2), Instance(8192, 4096, alive=4096, seed=3)], batches=batches)
-    _fill(ref, np.random.default_rng(5), 0.02, 0.6)
+    fill_c5(ref, np.random.default_rng(5), 0.02, 0.6)
     return ref
 
 
@@ -78,15 +79,13 @@ def test_count_mailbox(ctx, orc):
 def test_spawns_every_frame(native, orc, monkeypatch, param_upload):
     """Frames WITH an init pass: the block is stored by a one-CTA kernel at the head of the frame (init reads the tables after its
     dependency wait then) — the firework recipe spawning every frame into recycled slots, zero tolerance, on both upload paths."""
-    from oracle.hanabi_oracle import pcg_hash
-    from tests.test_gpu_effects import _firework_trails, _run
     monkeypatch.setenv("HNB_PARAM_UPLOAD", param_upload)
     ctx = native.Context(0)
-    asset = _firework_trails(4096)
+    asset = firework_trails(4096)
     ref = RefWorld(4096, 12, [Instance(0, 4096, alive=0)], dt=1.0 / 20.0)
-    seeds = lambda f: [int(pcg_hash(np.array([0x777 + f], dtype=np.uint32))[0])]
+    seeds = lambda n, f: [int(pcg_hash(np.array([0x777 + f], dtype=np.uint32))[0])]
     copies0 = ctx.frame_block_copies
-    _run(ctx, orc, asset, ref, 60, lambda f: [300 if f % 7 else 900], seeds=seeds, check_every=3)
+    Lockstep(ctx, orc, ref, asset, seeds=seeds).run([[300 if f % 7 else 900] for f in range(60)], check_every=3)
     copies = ctx.frame_block_copies - copies0
     assert (copies == 0) if param_upload == "1" else (copies >= 60)
     assert ref.metadata[0].particle_counter > 3 * 4096, "slots were recycled"
@@ -99,7 +98,7 @@ def test_large_parameter_blocks(ctx, orc, n_inst):
     many-instance path; 200: 27 KB) still travel with the launch (CUDA 12.1+: 32 KB of kernel parameters)."""
     cap = 256
     ref = RefWorld(n_inst * cap, 8, [Instance(i * cap, cap, alive=200 + (i % 50), seed=i) for i in range(n_inst)])
-    _fill(ref, np.random.default_rng(n_inst), 0.02, 0.4)
+    fill_c5(ref, np.random.default_rng(n_inst), 0.02, 0.4)
     gpu = GpuWorld(ctx, ref, recipes.c5_lowered())
     copies0 = ctx.frame_block_copies
     for f in range(8):

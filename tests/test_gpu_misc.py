@@ -13,6 +13,7 @@ from bevy_hanabi_b200 import recipes
 from bevy_hanabi_b200 import runtime as R
 from bevy_hanabi_b200._native import HanabiError
 from oracle.hanabi_oracle import EffectOracle
+from tests.effects import exact_expr
 from tests.helpers import GpuWorld, Instance, RefWorld, assert_world_equal
 
 pytestmark = pytest.mark.gpu
@@ -223,52 +224,13 @@ hypothesis = pytest.importorskip("hypothesis")
 from hypothesis import HealthCheck, Phase, given, settings, strategies as st  # noqa: E402
 
 
-def _build(draw, w, depth, kind):
-    """Draw an expression of `kind` ('f' scalar / 'v' vec3) using only IEEE-exact operators."""
-    lit_f = lambda: w.lit(float(np.float32(draw(st.floats(-4, 4, allow_nan=False, width=32)))))
-    if depth == 0:
-        if kind == "f":
-            c = draw(st.integers(0, 4))
-            return [lit_f, lambda: w.attr(A.AGE), lambda: w.attr(A.F32_1), lambda: w.attr(A.POSITION).y(), lambda: w.time()][c]()
-        c = draw(st.integers(0, 2))
-        if c == 0:
-            return w.lit(G.Vec3(*[float(np.float32(draw(st.floats(-3, 3, allow_nan=False, width=32)))) for _ in range(3)]))
-        return [None, lambda: w.attr(A.POSITION), lambda: w.attr(A.VELOCITY)][c]()
-    sub = lambda k: _build(draw, w, depth - 1, k)
-    if kind == "f":
-        c = draw(st.integers(0, 13))
-        if c == 0: return sub("f") + sub("f")
-        if c == 1: return sub("f") - sub("f")
-        if c == 2: return sub("f") * sub("f")
-        if c == 3: return sub("f") / (sub("f").abs() + w.lit(1.))
-        if c == 4: return sub("f").min(sub("f"))
-        if c == 5: return sub("f").max(sub("f"))
-        if c == 6: return sub("f").abs().sqrt()
-        if c == 7: return sub("f").floor() + sub("f").fract()
-        if c == 8: return sub("f").sign() * sub("f").ceil()
-        if c == 9: return sub("v").dot(sub("v"))
-        if c == 10: return sub("f").clamp(w.lit(-1.), w.lit(2.))
-        if c == 11: return sub("f").mix(sub("f"), w.lit(0.25))
-        if c == 12: return sub("f").step(sub("f")) + sub("v").x()
-        return sub("v").length()
-    c = draw(st.integers(0, 7))
-    if c == 0: return sub("v") + sub("v")
-    if c == 1: return sub("v") * sub("f")
-    if c == 2: return sub("v").cross(sub("v"))
-    if c == 3: return sub("f").vec3(sub("f"), sub("f"))
-    if c == 4: return sub("v").abs().min(sub("v"))
-    if c == 5: return sub("f").cast(G.VEC3) - sub("v")
-    if c == 6: return sub("v") / (sub("v").abs() + w.lit(G.Vec3(1., 1., 1.)))
-    return sub("v").max(sub("v")) * w.lit(0.5)
-
-
 # no shrinking: every example costs an NVRTC compile and a few GPU frames
 @settings(max_examples=20, deadline=None, suppress_health_check=list(HealthCheck), phases=[Phase.generate], derandomize=True)
 @given(st.data())
 def test_random_expression_graphs_bit_exact(ctx, orc, data):
     w = G.ExprWriter()
-    f_expr = _build(data.draw, w, data.draw(st.integers(1, 3)), "f")
-    v_expr = _build(data.draw, w, data.draw(st.integers(1, 3)), "v")
+    f_expr = exact_expr(data.draw, w, data.draw(st.integers(1, 3)), "f")
+    v_expr = exact_expr(data.draw, w, data.draw(st.integers(1, 3)), "v")
     asset = (G.EffectAsset(600, w.module, name="fuzz")
              .init(G.SetAttributeModifier(A.POSITION, w.rand(G.VEC3) * w.lit(4.) - w.lit(2.)))
              .init(G.SetAttributeModifier(A.VELOCITY, w.rand(G.VEC3) - w.lit(0.5)))

@@ -7,36 +7,17 @@ import numpy as np
 import pytest
 
 from bevy_hanabi_b200 import _native as N
-from bevy_hanabi_b200 import graph as G
 from bevy_hanabi_b200 import runtime as R
 from oracle.hanabi_oracle import EffectOracle
-from tests.helpers import GpuWorld, Instance, RefWorld, assert_world_equal
+from tests.effects import ribbon_asset
+from tests.helpers import GpuWorld, Instance, RefWorld, assert_ribbons_sorted, assert_world_equal
 
 pytestmark = pytest.mark.gpu
-A = G.Attribute
-
-
-def _ribbon_asset(capacity, ribbons=5.0, lifetime=(0.15, 0.6)):
-    w = G.ExprWriter()
-    return (G.EffectAsset(capacity, w.module, name="ribbons")
-            .init(G.SetAttributeModifier(A.POSITION, w.rand(G.VEC3) * w.lit(2.) - w.lit(1.)))
-            .init(G.SetAttributeModifier(A.VELOCITY, w.rand(G.VEC3) - w.lit(0.5)))
-            .init(G.SetAttributeModifier(A.AGE, w.rand(G.FLOAT) * w.lit(0.1)))
-            .init(G.SetAttributeModifier(A.LIFETIME, w.lit(lifetime[0]).uniform(w.lit(lifetime[1]))))
-            .init(G.SetAttributeModifier(A.RIBBON_ID, (w.rand(G.FLOAT) * w.lit(ribbons)).cast(G.UINT))))
-
-
-def _assert_sorted(ref):
-    for i in range(len(ref.instances)):
-        md, base = ref.metadata[i], ref.spawners[i].slab_offset
-        e = ref.indirect[base:base + md.alive_count, md.indirect_write_index].astype(np.int64)
-        k = (ref.particles[base + e, md.sort_key_offset].astype(np.uint64) << np.uint64(32)) | ref.particles[base + e, md.sort_key2_offset]
-        assert np.all(k[1:] >= k[:-1])
 
 
 def test_ribbon_effect_frames(ctx, orc):
     """Whole frames through hnb_simulate: spawns, deaths, slot recycling, and the sorted alive list every frame."""
-    asset = _ribbon_asset(4096)
+    asset = ribbon_asset(4096)
     fx = asset.generate()
     assert fx.flags & N.EFFECT_RIBBONS
     fields, size, _ = asset.particle_layout()
@@ -50,7 +31,7 @@ def test_ribbon_effect_frames(ctx, orc):
         ref.set_spawns([900 if f % 4 == 0 else 23])
         eo.frame(ref, orc)
         gpu.frame()
-        _assert_sorted(ref)
+        assert_ribbons_sorted(ref)
         assert_world_equal(ref, gpu.pull(), what=f"frame {f}")
         grew_past_small |= ref.metadata[0].alive_count > 2048
     assert grew_past_small, "the scenario must cross from the shared-memory path to the radix path"
@@ -61,7 +42,7 @@ def test_many_ribbon_instances_in_one_batch(ctx, orc):
     small ones, the cooperative kernel loops over the large ones."""
     caps = [64, 5000, 1, 300, 2048, 7000, 2, 2100]
     spawn0 = [0, 4200, 1, 250, 2048, 6500, 2, 2100]
-    asset = _ribbon_asset(sum(caps), ribbons=40.0, lifetime=(0.1, 1.0))
+    asset = ribbon_asset(sum(caps), ribbons=40.0, lifetime=(0.1, 1.0))
     fx = asset.generate()
     fields, size, _ = asset.particle_layout()
     insts, off = [], 0
@@ -77,7 +58,7 @@ def test_many_ribbon_instances_in_one_batch(ctx, orc):
         ref.set_spawns(spawn0 if f == 0 else [3, 40, 0, 5, 9, 80, 0, 11])
         eo.frame(ref, orc)
         gpu.frame()
-        _assert_sorted(ref)
+        assert_ribbons_sorted(ref)
         assert_world_equal(ref, gpu.pull(), what=f"frame {f}")
 
 
@@ -87,7 +68,7 @@ def test_sort_pass_alone(ctx, n, wide_keys):
     """hnb_pass_sort on hand-made state. `wide_keys`: ribbon ids use all 32 bits and ages all exponents, so that
     all eight radix passes run; otherwise few distinct keys, i.e. many ties (stability) and skipped passes."""
     rng = np.random.default_rng(n * 2 + int(wide_keys))
-    asset = _ribbon_asset(max(n, 1))
+    asset = ribbon_asset(max(n, 1))
     fx = asset.generate()
     fields, size, _ = asset.particle_layout()
     off = {f.name: f.offset // 4 for f in fields}

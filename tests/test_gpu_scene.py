@@ -10,38 +10,13 @@ import numpy as np
 import pytest
 
 from bevy_hanabi_b200 import _native as N
-from bevy_hanabi_b200 import graph as G
 from bevy_hanabi_b200 import runtime as R
 from bevy_hanabi_b200 import spawn as S
 from oracle.hanabi_oracle import EffectOracle, pcg_hash
+from tests.effects import drifting_sparks, firework_trails, growing_dust, ribbon_asset
 from tests.helpers import Instance, RefWorld
-from tests.test_gpu_effects import _firework_trails
-from tests.test_gpu_ribbons import _ribbon_asset
 
 pytestmark = pytest.mark.gpu
-A = G.Attribute
-
-
-def _drifting_sparks(capacity):
-    w = G.ExprWriter()
-    return (G.EffectAsset(capacity, w.module, name="sparks")
-            .init(G.SetAttributeModifier(A.POSITION, w.rand(G.VEC3) * w.lit(2.) - w.lit(1.)))
-            .init(G.SetAttributeModifier(A.VELOCITY, w.rand(G.VEC3) * w.lit(2.) - w.lit(1.)))
-            .init(G.SetAttributeModifier(A.AGE, w.lit(0.)))
-            .init(G.SetAttributeModifier(A.LIFETIME, w.lit(0.2).uniform(w.lit(0.9))))
-            .update(G.AccelModifier(w.lit(G.Vec3(0., -9.8, 0.))))
-            .update(G.LinearDragModifier(w.lit(0.5))))
-
-
-def _growing_dust(capacity):
-    """No age / lifetime: particles never die (like C1), a size attribute grows, a kill box culls."""
-    w = G.ExprWriter()
-    return (G.EffectAsset(capacity, w.module, name="dust")
-            .init(G.SetAttributeModifier(A.POSITION, w.rand(G.VEC3) - w.lit(0.5)))
-            .init(G.SetAttributeModifier(A.VELOCITY, (w.rand(G.VEC3) - w.lit(0.5)) * w.lit(3.)))
-            .init(G.SetAttributeModifier(A.SIZE, w.lit(0.01)))
-            .update(G.SetAttributeModifier(A.SIZE, w.attr(A.SIZE) * w.lit(1.0625) + w.time() * w.lit(0.001)))
-            .update(G.KillAabbModifier(w.lit(G.Vec3(0., 0., 0.)), w.lit(G.Vec3(1.5, 1.0, 1.25)))))
 
 
 class SceneEffect:
@@ -72,10 +47,10 @@ class SceneEffect:
 def test_scene_of_four_assets(ctx, orc):
     dt = 1.0 / 60.0
     plan = [
-        (_firework_trails(1), [3000, 500, 1200], [S.SpawnerSettings.burst(400, 0.25), S.SpawnerSettings.once(450), S.SpawnerSettings.rate(900.)]),
-        (_drifting_sparks(1), [4096, 70, 9000], [S.SpawnerSettings.rate(6000.), S.SpawnerSettings.rate(120.), S.SpawnerSettings.burst((500, 1500), (0.1, 0.3))]),
-        (_ribbon_asset(1), [2500, 6000], [S.SpawnerSettings.rate(3000.), S.SpawnerSettings.burst(2500, 0.5)]),
-        (_growing_dust(1), [800, 800, 800, 64], [S.SpawnerSettings.rate(400.), S.SpawnerSettings.once(800), S.SpawnerSettings.rate(1000.), S.SpawnerSettings.rate(30.)]),
+        (firework_trails(1), [3000, 500, 1200], [S.SpawnerSettings.burst(400, 0.25), S.SpawnerSettings.once(450), S.SpawnerSettings.rate(900.)]),
+        (drifting_sparks(1), [4096, 70, 9000], [S.SpawnerSettings.rate(6000.), S.SpawnerSettings.rate(120.), S.SpawnerSettings.burst((500, 1500), (0.1, 0.3))]),
+        (ribbon_asset(1), [2500, 6000], [S.SpawnerSettings.rate(3000.), S.SpawnerSettings.burst(2500, 0.5)]),
+        (growing_dust(1), [800, 800, 800, 64], [S.SpawnerSettings.rate(400.), S.SpawnerSettings.once(800), S.SpawnerSettings.rate(1000.), S.SpawnerSettings.rate(30.)]),
     ]
     effects, row = [], 0
     for asset, caps, settings in plan:

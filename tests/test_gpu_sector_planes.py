@@ -2,12 +2,9 @@
 import numpy as np
 import pytest
 
-from bevy_hanabi_b200 import graph as G
-from oracle.hanabi_oracle import EffectOracle, pcg_hash
-from tests.helpers import GpuWorld, Instance, RefWorld, assert_world_equal
-from tests.test_gpu_effects import _firework_trails
-from tests.test_gpu_ribbons import _ribbon_asset
-from tests.test_gpu_scene import _drifting_sparks
+from oracle.hanabi_oracle import pcg_hash
+from tests.effects import drifting_sparks, firework_trails, ribbon_asset
+from tests.helpers import Instance, Lockstep, RefWorld
 
 pytestmark = pytest.mark.gpu
 
@@ -16,16 +13,10 @@ pytestmark = pytest.mark.gpu
 def test_sector_planes_on_the_device(ctx, orc, name):
     """HNB_SLAB_SECTOR_PLANES + HNB_EFFECT_SECTOR_PLANES: same results as the default layout (32-, 48-byte records, and a
     ribbon effect through the sort's key gathers), including AoS upload / download of the interleaved columns."""
-    asset = {"sparks": _drifting_sparks, "trails": _firework_trails, "ribbons": _ribbon_asset}[name](6000)
+    asset = {"sparks": drifting_sparks, "trails": firework_trails, "ribbons": ribbon_asset}[name](6000)
     fields, size, _ = asset.particle_layout()
     ref = RefWorld(6000, size // 4, [Instance(0, 6000, alive=0, seed=4)], dt=1 / 10)
     if name == "ribbons":
         ref.set_sort_keys(fields)
-    eo = EffectOracle(asset)
-    gpu = GpuWorld(ctx, ref, asset.generate(sector_planes=True), sector_planes=True)
-    for f in range(8):
-        ref.sim.time = np.float32(f) * ref.sim.delta_time
-        ref.set_spawns([2500 if f % 3 == 0 else 120], [int(pcg_hash(np.array([f + 300], dtype=np.uint32))[0])])
-        eo.frame(ref, orc)
-        gpu.frame()
-        assert_world_equal(ref, gpu.pull(), what=f"{name} frame {f}")
+    seeds = lambda n, f: [int(pcg_hash(np.array([f + 300], dtype=np.uint32))[0])]
+    Lockstep(ctx, orc, ref, asset, sector=True, seeds=seeds).run([[2500 if f % 3 == 0 else 120] for f in range(8)], what=name)

@@ -11,64 +11,13 @@ import pytest
 from bevy_hanabi_b200 import _native as N
 from bevy_hanabi_b200 import recipes
 from bevy_hanabi_b200 import runtime as R
-from oracle.hanabi_oracle import EffectOracle, pcg_hash
-from tests.helpers import GpuWorld, Instance, RefWorld, assert_world_equal
+from tests.effects import EFFECTS, event_assets, ribbon_asset, table_asset, table_props
+from tests.helpers import Instance, Lockstep, RefWorld, is_identity, seeds, sparks_world, table_world
 from tests.snapshot_ref import HEADER_WORDS, SNAPSHOT_MAGIC, ref_restore, ref_snapshot
-from tests.test_gpu_events import _assets as _event_assets
-from tests.test_gpu_ribbons import _ribbon_asset
-from tests.test_gpu_scene import _drifting_sparks
-from tests.test_gpu_tile_shapes import EFFECTS, _asset, _world
 
 pytestmark = pytest.mark.gpu
 
 SENTINEL = np.uint32(0xA5A5A5A5)
-
-
-def _seeds(n, f):
-    return [int(s) for s in pcg_hash(np.arange(n, dtype=np.uint32) + np.uint32(100 * f + 7))]
-
-
-class Side:
-    """A GpuWorld and the oracle world it must equal."""
-
-    def __init__(self, ctx, asset, ref, *, props=None, sector=False, slot=False):
-        blobs = None
-        if props is not None:
-            blobs = [asset.serialize_properties(props(i)) for i in range(len(ref.instances))]
-            for i in range(len(ref.instances)):
-                ref.metadata[i].properties_array_index = i
-        ref.slot_order = slot
-        self.ctx, self.ref, self.slot, self.fresh = ctx, ref, slot, True
-        self.eo = EffectOracle(asset, {i: props(i) for i in range(len(ref.instances))} if props else None)
-        self.gpu = GpuWorld(ctx, ref, asset.generate(sector_planes=sector, slot_order=slot), property_blobs=blobs, sector_planes=sector)
-
-    def compare(self, what):
-        if self.fresh:  # no frame ran yet: the context has no per-frame tables of this world to read back
-            ctx, ref, n = self.ctx, self.ref, len(self.ref.instances)
-            ctx.sync()
-            got = {"particles": ctx.slab_download_aos(self.gpu.slab, 0, ref.slab_rows, self.gpu.stride),
-                   "indirect": ctx.slab_download_indirect(self.gpu.slab, 0, ref.slab_rows),
-                   "metadata": np.stack([np.frombuffer(bytes(ctx.read_metadata(i)), dtype=np.uint32) for i in range(n)]),
-                   "draw": np.concatenate([np.frombuffer(bytes(ctx.read_draw_args(i)), dtype=np.uint32) for i in range(n)])}
-            for k, want in (("particles", ref.particles), ("indirect", ref.indirect), ("metadata", ref.metadata_rows()), ("draw", ref.draw)):
-                np.testing.assert_array_equal(got[k], want, err_msg=f"{what}: {k}")
-        else:
-            assert_world_equal(self.ref, self.gpu.pull(), what=what)
-        if self.slot:
-            assert self.ctx.read_debug(False)[15] == 0, f"{what}: alive bitmap and counters disagree"
-
-    def frames(self, orc, schedule, start=0, what=""):
-        for f, spawns in enumerate(schedule, start=start):
-            self.ref.sim.time = np.float32(f) * self.ref.sim.delta_time
-            self.ref.set_spawns(spawns, _seeds(len(spawns), f))
-            self.eo.frame(self.ref, orc)
-            self.gpu.frame()
-            self.fresh = False
-            self.compare(f"{what} frame {f}")
-
-    def span(self, i):
-        inst = self.ref.instances[i]
-        return inst.slab_offset, inst.capacity
 
 
 class Buffers:
@@ -125,35 +74,15 @@ def restore(side, i, buf, nbytes, words):
     return m
 
 
-def _sparks_ref(caps, dt=0.05, seed=1):
-    _, size, _ = _drifting_sparks(max(caps)).particle_layout()
-    insts, off = [], 0
-    for i, c in enumerate(caps):
-        insts.append(Instance(off, c, alive=0, seed=11 + 7 * i))
-        off += c
-    ref = RefWorld(off, size // 4, insts, dt=dt)
-    rng = np.random.default_rng(seed)
-    for inst in insts:
-        rows = slice(inst.slab_offset, inst.slab_offset + inst.capacity)
-        ref.indirect[rows, 2] = rng.permutation(ref.indirect[rows, 2])
-    return ref
-
-
-def _is_identity(ref, i):
-    md, base = ref.metadata[i], ref.instances[i].slab_offset
-    lst = ref.indirect[base:base + md.alive_count, md.indirect_write_index]
-    return bool((lst == np.arange(len(lst))).all())
-
-
 # frames after a restore; _churned_sparks runs 24 frames at 300 spawns (lifetimes of 4 to 18 frames) before a snapshot
 AFTER = [[300]] * 8
 
 
 def _churned_sparks(ctx, orc, caps=(4096,), **kw):
-    asset = _drifting_sparks(max(caps))
-    side = Side(ctx, asset, _sparks_ref(list(caps)), **kw)
-    side.frames(orc, [[300] + [0] * (len(caps) - 1)] * 24, what="churn")
-    assert not _is_identity(side.ref, 0) and side.ref.metadata[0].alive_count > min(2000, caps[0] // 2)
+    asset, ref = sparks_world(list(caps))
+    side = Lockstep(ctx, orc, ref, asset, seeds=seeds, **kw)
+    side.run([[300] + [0] * (len(caps) - 1)] * 24, what="churn")
+    assert not is_identity(side.ref, 0) and side.ref.metadata[0].alive_count > min(2000, caps[0] // 2)
     return asset, side
 
 
@@ -163,8 +92,8 @@ def test_churned_sparks_into_their_own_slice(ctx, orc, bufs, mode):
     asset, side = _churned_sparks(ctx, orc, **kw)
     buf, nbytes, words = snapshot(side, 0, bufs)
     assert restore(side, 0, buf, nbytes, words) == side.ref.metadata[0].alive_count
-    assert _is_identity(side.ref, 0)
-    side.frames(orc, AFTER, start=24, what="after the restore")
+    assert is_identity(side.ref, 0)
+    side.run(AFTER, start=24, what="after the restore")
 
 
 @pytest.mark.parametrize("target", ["other_offset", "other_slab", "larger", "smaller", "other_context"])
@@ -181,10 +110,10 @@ def test_churned_sparks_moved(ctx, orc, bufs, native, target):
             dst, i = src, 1
         else:
             cap = {"larger": 6000, "smaller": 1500}.get(target, 4096)
-            dst, i = Side(ctx2, asset, _sparks_ref([777, cap, 500], seed=2)), 1
+            dst, i = Lockstep(ctx2, orc, sparks_world([777, cap, 500], seed=2)[1], asset, seeds=seeds), 1
         assert restore(dst, i, buf, nbytes, words) == min(n, dst.span(i)[1])
         spawns = [[300, 300]] * 8 if target == "other_offset" else [[50, 300, 40]] * 8
-        dst.frames(orc, spawns, start=24, what=f"{target}, after the restore")
+        dst.run(spawns, start=24, what=f"{target}, after the restore")
     finally:
         if ctx2 is not ctx:
             ctx2.close()
@@ -192,7 +121,7 @@ def test_churned_sparks_moved(ctx, orc, bufs, native, target):
 
 def test_churned_ribbons(ctx, orc, bufs):
     """Snapshot in sorted order, restored into another slab; the next frames sort again."""
-    asset = _ribbon_asset(4096)
+    asset = ribbon_asset(4096)
     fields, size, _ = asset.particle_layout()
 
     def world(caps, seed):
@@ -204,24 +133,24 @@ def test_churned_ribbons(ctx, orc, bufs):
         ref.set_sort_keys(fields)
         return ref
 
-    src = Side(ctx, asset, world([4096], 3))
-    src.frames(orc, [[900 if f % 4 == 0 else 23] for f in range(16)], what="churn")
+    src = Lockstep(ctx, orc, world([4096], 3), asset, seeds=seeds)
+    src.run([[900 if f % 4 == 0 else 23] for f in range(16)], what="churn")
     buf, nbytes, words = snapshot(src, 0, bufs)
-    dst = Side(ctx, asset, world([300, 4096], 9))
+    dst = Lockstep(ctx, orc, world([300, 4096], 9), asset, seeds=seeds)
     restore(dst, 1, buf, nbytes, words)
-    dst.frames(orc, [[0, 900 if f % 4 == 0 else 23] for f in range(16, 26)], start=16, what="ribbons, after the restore")
+    dst.run([[0, 900 if f % 4 == 0 else 23] for f in range(16, 26)], start=16, what="ribbons, after the restore")
 
 
 @pytest.mark.parametrize("name", list(EFFECTS))
 def test_churned_wide_records(ctx, orc, bufs, name):
     """48 and 64-byte records (K = 2), 96 and 144 bytes (K = 1), with per-instance properties where the effect has them:
     instance 0 churns, its snapshot goes to instance 1 of the same slab."""
-    ref = _world(name, [3000, 3000])
-    side = Side(ctx, _asset(name, 3000), ref, props=EFFECTS[name][3])
-    side.frames(orc, [[500, 0]] * 12, what="churn")
+    ref = table_world(name, [3000, 3000])
+    side = Lockstep(ctx, orc, ref, table_asset(name, 3000), props=table_props(name, 2), seeds=seeds)
+    side.run([[500, 0]] * 12, what="churn")
     buf, nbytes, words = snapshot(side, 0, bufs)
     restore(side, 1, buf, nbytes, words)
-    side.frames(orc, [[300, 300]] * 8, start=12, what="after the restore")
+    side.run([[300, 300]] * 8, start=12, what="after the restore")
 
 
 def test_host_round_trip_of_the_prefix(ctx, orc, bufs):
@@ -234,11 +163,11 @@ def test_host_round_trip_of_the_prefix(ctx, orc, bufs):
     assert not header[6:].any(), "reserved words are zero"
     prefix_bytes = 64 + int(header[3]) * int(header[2])
     host = ctx.device_download(buf, prefix_bytes)
-    dst = Side(ctx, asset, _sparks_ref([4096], seed=5))
+    dst = Lockstep(ctx, orc, sparks_world([4096], seed=5)[1], asset, seeds=seeds)
     copy = bufs.alloc(ctx, prefix_bytes)
     ctx.device_upload(copy, host)
     assert restore(dst, 0, copy, prefix_bytes, host) == header[3]
-    dst.frames(orc, AFTER, start=24, what="after the host round trip")
+    dst.run(AFTER, start=24, what="after the host round trip")
 
 
 def test_two_restores_stay_identical(ctx, orc, bufs, native):
@@ -249,20 +178,16 @@ def test_two_restores_stay_identical(ctx, orc, bufs, native):
     buf, nbytes, words = snapshot(src, 0, bufs)
     ctxs = [native.Context(0) for _ in range(2)]
     try:
-        sides = [Side(c, asset, _sparks_ref([4096], seed=7)) for c in ctxs]
+        sides = [Lockstep(c, orc, sparks_world([4096], seed=7)[1], asset, seeds=seeds) for c in ctxs]
         for side in sides:
             restore(side, 0, buf, nbytes, words)
         for f in range(24, 54):
             pulled = []
             for side in sides:
-                side.ref.sim.time = np.float32(f) * side.ref.sim.delta_time
-                side.ref.set_spawns([300], _seeds(1, f))
-                side.eo.frame(side.ref, orc)
-                side.gpu.frame()
+                side.step(f, [300])
                 pulled.append(side.gpu.pull())
             _pull_equal(pulled[0], pulled[1], f"frame {f}: the two restored instances")
         for side in sides:
-            side.fresh = False
             side.compare("after 30 frames")
     finally:
         for c in ctxs:
@@ -309,9 +234,9 @@ def test_refusals_leave_the_state_untouched(ctx, orc, bufs):
     ctx.instance_snapshot(gpu.slab, gpu.effect, 0, 0, 2000, buf, nbytes)
     ctx.sync()
     snap = ctx.device_download(buf, nbytes + 16)
-    other_stride = ctx.effect_compile(_asset("vec4x2_64", 2000).generate())
+    other_stride = ctx.effect_compile(table_asset("vec4x2_64", 2000).generate())
     sector = ctx.effect_compile(asset.generate(sector_planes=True))
-    parent = _event_assets()[0]
+    parent = event_assets()[0]
     emitting = ctx.effect_compile(parent.generate(num_event_bindings=1))
     assert parent.particle_layout()[1] == 32, "the emitting effect differs from the slab in its flag only"
     common = [("rows outside the slab", gpu.effect, 0, 1, 2000), ("rows outside the slab", gpu.effect, 0, 0, 2001),

@@ -7,11 +7,9 @@ import pytest
 
 from bevy_hanabi_b200 import graph as G
 from oracle.hanabi_oracle import EffectOracle, pcg_hash
-from tests.helpers import Instance, RefWorld, assert_float_attributes_close
+from tests.effects import MATRIX_PROPS, drifting_sparks, firework_trails, force_field, growing_dust, matrix_asset, ribbon_asset
+from tests.helpers import Instance, RefWorld, assert_float_attributes_close, float_word_mask
 from tests.host_exec import HostEffect, replay_frame
-from tests.test_gpu_effects import _firework_trails, _float_word_mask, _force_field
-from tests.test_gpu_ribbons import _ribbon_asset
-from tests.test_gpu_scene import _drifting_sparks, _growing_dust
 
 A = G.Attribute
 
@@ -30,7 +28,7 @@ def _run(orc, asset, frames, spawns, exact=True, props=None, capacity=2048):
         blob = asset.serialize_properties(props)
         ref.metadata[0].properties_array_index = 0
     eo = EffectOracle(asset, {0: props} if props else None)
-    mask, fattrs = _float_word_mask(asset)
+    mask, fattrs = float_word_mask(asset)
     checked_init = checked_update = deaths = 0
     for f in range(frames):
         ref.sim.time = np.float32(f) * ref.sim.delta_time
@@ -54,14 +52,14 @@ def _run(orc, asset, frames, spawns, exact=True, props=None, capacity=2048):
 
 
 def test_trails_generated_code_equals_interpreter(orc):
-    ci, cu, deaths = _run(orc, _firework_trails(2048), 30, lambda f: 700 if f % 10 == 0 else 0)
+    ci, cu, deaths = _run(orc, firework_trails(2048), 30, lambda f: 700 if f % 10 == 0 else 0)
     assert ci > 1500
     assert cu > 10_000 and deaths > 100
 
 
 @pytest.mark.parametrize("name", ["sparks", "dust", "ribbons"])
 def test_scene_assets_generated_code_equals_interpreter(orc, name):
-    asset = {"sparks": _drifting_sparks, "dust": _growing_dust, "ribbons": _ribbon_asset}[name](2048)
+    asset = {"sparks": drifting_sparks, "dust": growing_dust, "ribbons": ribbon_asset}[name](2048)
     ci, cu, deaths = _run(orc, asset, 20, lambda f: 300 if f % 4 == 0 else 11)
     assert ci > 800 and cu > 5000
     if name != "ribbons":
@@ -70,7 +68,7 @@ def test_scene_assets_generated_code_equals_interpreter(orc, name):
 
 def test_force_field_generated_code_within_tolerance(orc):
     props = {"attraction_accel": 18.0, "repulsor_position": G.Vec3(0.25, 0.5, 0.1)}
-    ci, cu, _ = _run(orc, _force_field(4096), 6, lambda f: 3000 if f == 0 else 20, exact=False, props=props, capacity=4096)
+    ci, cu, _ = _run(orc, force_field(4096), 6, lambda f: 3000 if f == 0 else 20, exact=False, props=props, capacity=4096)
     assert ci > 3000 and cu > 15_000
 
 
@@ -96,49 +94,12 @@ def test_operator_table_generated_code(orc):
     assert ci > 400 and cu > 2000 and deaths > 50
 
 
-def _matrix_asset(capacity):
-    """Matrix values (reference src/graph/mod.rs MatrixValue, src/attributes.rs MatrixType) in literals and
-    properties, through every WGSL matrix product and sum. Also used by the pending GPU test."""
-    w = G.ExprWriter()
-    rot = w.lit(G.Mat3((0., 1., 0.), (-1., 0., 0.), (0., 0., 1.)))            # quarter turn about z
-    lift = w.lit(G.Mat(2, 3, [1., 0.5, 0.25, -0.5, 1., 2.]))                   # mat2x3: vec2 -> vec3
-    squash = w.lit(G.Mat(3, 2, [0.5, 0.125, -0.25, 1., 0.75, -1.5]))           # mat3x2: vec3 -> vec2
-    twist = w.prop(w.add_property("twist", G.Mat2(0.8, 0.6, -0.6, 0.8)))       # 16 bytes: laid out like a vec4
-    gain = w.prop(w.add_property("gain", G.Vec4(1.5, 0., 0., 0.))).x()
-    # 64 bytes: must be the last entry of the layout (PropertyLayout::new advances 16 bytes per property of 16 bytes or
-    # more and places smaller properties after them, properties.rs:572-580), so no scalar / vec2 / vec3 property here
-    basis = w.prop(w.add_property("basis", G.Mat4(*[float(i) for i in range(16)])))
-    wide = w.lit(G.Mat(2, 4, [0.5, -1., 2., 0.25, 1.5, 0.75, -0.5, 1.]))     # mat2x4: vec2 -> vec4
-    tall = w.lit(G.Mat(4, 2, [1., -2., 0.5, 0.25, -0.75, 1.25, 2., -0.125]))  # mat4x2: vec4 -> vec2
-    m34 = w.lit(G.Mat(3, 4, [0.1 * (i - 5) for i in range(12)]))              # mat3x4: vec3 -> vec4 (literals rounded to 1e-6)
-    m43 = w.lit(G.Mat(4, 3, [0.3 * (7 - i) for i in range(12)]))              # mat4x3: vec4 -> vec3
-    v, p = w.attr(A.VELOCITY), w.attr(A.POSITION)
-    q = w.attr(A.F32X4_1)
-    return (G.EffectAsset(capacity, w.module, name="matrices")
-            .init(G.SetAttributeModifier(A.POSITION, w.rand(G.VEC3) * w.lit(4.) - w.lit(2.)))
-            .init(G.SetAttributeModifier(A.VELOCITY, w.rand(G.VEC3) - w.lit(0.5)))
-            .init(G.SetAttributeModifier(A.AGE, w.lit(0.)))
-            .init(G.SetAttributeModifier(A.LIFETIME, w.lit(0.3).uniform(w.lit(0.9))))
-            .init(G.SetAttributeModifier(A.F32X2_0, squash * (rot * (w.rand(G.VEC3) * gain))))                  # m*v twice, at init
-            .update(G.SetAttributeModifier(A.F32X3_0, (rot * v) * w.lit(0.875) + lift * (twist * v.x().vec2(v.y()))))    # m*v, prop m*v
-            .update(G.SetAttributeModifier(A.F32X3_1, v * (rot * rot + rot * w.lit(0.5)) - p * (w.lit(2.) * rot - rot)))  # v*m, m*m, m+m, m-m, m*s, s*m
-            .update(G.SetAttributeModifier(A.F32X4_1, wide * v.x().vec2(v.y()) + m34 * p + v * m43))           # the other four shapes, m*v and v*m
-            .update(G.SetAttributeModifier(A.F32X3_2, (lift * squash) * p + m43 * q + q * m34))                 # mat2x3 * mat3x2 -> mat3x3
-            .update(G.SetAttributeModifier(A.F32X2_1, (squash * lift) * w.attr(A.F32X2_0) + p * lift))          # -> mat2x2; vec3 * mat2x3 -> vec2
-            .update(G.SetAttributeModifier(A.F32X4_0, basis * p.vec4_xyz_w(gain) + v.vec4_xyz_w(w.lit(1.)) * basis))
-            .update(G.SetAttributeModifier(A.F32X2_2, tall * q + q * wide)))
-
-
-_MATRIX_PROPS = {"twist": G.Mat2(0.28, 0.96, -0.96, 0.28), "gain": G.Vec4(0.75, 9., 9., 9.),
-                 "basis": G.Mat4((1., 0., 0., 0.), (0., 2., 0., 0.), (0., 0., -1., 0.), (0.5, -0.25, 3., 1.))}
-
-
 def test_matrix_values_generated_code_equals_interpreter(orc):
     """Every product only multiplies and adds in a fixed order, so the lowered text and the interpreter agree bit for bit."""
-    ci, cu, deaths = _run(orc, _matrix_asset(1024), 10, lambda f: 500 if f == 0 else 25, props=_MATRIX_PROPS, capacity=1024)
+    ci, cu, deaths = _run(orc, matrix_asset(1024), 10, lambda f: 500 if f == 0 else 25, props=MATRIX_PROPS, capacity=1024)
     assert ci > 500 and cu > 3000 and deaths > 20
     # and with the default property values
-    ci, cu, _ = _run(orc, _matrix_asset(1024), 3, lambda f: 200, props={}, capacity=1024)
+    ci, cu, _ = _run(orc, matrix_asset(1024), 3, lambda f: 200, props={}, capacity=1024)
     assert ci == 600
 
 

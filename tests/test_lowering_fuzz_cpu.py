@@ -143,10 +143,10 @@ def test_random_exact_graphs_generated_code_equals_interpreter(orc, data):
     """Values, not just syntax: random graphs over the IEEE-exact operators (the generator of the GPU fuzz test), with
     the generated code executed on the CPU (tests/host_exec.py) and compared bit for bit with the interpreter."""
     from tests.host_exec import HostEffect, replay_frame
-    from tests.test_gpu_misc import _build as build_exact
+    from tests.effects import exact_expr
     w = G.ExprWriter()
-    f_expr = build_exact(data.draw, w, data.draw(st.integers(1, 3)), "f")
-    v_expr = build_exact(data.draw, w, data.draw(st.integers(1, 3)), "v")
+    f_expr = exact_expr(data.draw, w, data.draw(st.integers(1, 3)), "f")
+    v_expr = exact_expr(data.draw, w, data.draw(st.integers(1, 3)), "v")
     asset = (G.EffectAsset(256, w.module, name="exact_fuzz")
              .init(G.SetAttributeModifier(A.POSITION, w.rand(G.VEC3) * w.lit(4.) - w.lit(2.)))
              .init(G.SetAttributeModifier(A.VELOCITY, w.rand(G.VEC3) - w.lit(0.5)))

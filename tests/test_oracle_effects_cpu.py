@@ -5,7 +5,7 @@ import pytest
 
 from bevy_hanabi_b200 import graph as G
 from oracle.hanabi_oracle import EffectOracle, pcg_hash
-from tests import test_gpu_effects as E
+from tests.effects import firework_trails, force_field, ribbon_asset
 from tests.helpers import Instance, RefWorld
 
 
@@ -24,12 +24,12 @@ def _check_invariants(ref):
 @pytest.mark.parametrize("name", ["firework", "force_field"])
 def test_oracle_invariants(orc, name):
     if name == "firework":
-        asset = E._firework_trails(2048)
+        asset = firework_trails(2048)
         ref = RefWorld(2048, 12, [Instance(0, 2048, alive=0)], dt=1.0 / 20.0)
         spawns = lambda f: [700 if f % 12 == 0 else 0]
         props = None
     else:
-        asset = E._force_field(4096)
+        asset = force_field(4096)
         _, size, _ = asset.particle_layout()
         ref = RefWorld(4096, size // 4, [Instance(0, 4096, alive=0, seed=77)])
         spawns = lambda f: [3000 if f == 0 else 10]
@@ -119,6 +119,5 @@ def test_ribbon_sort_restatement_equals_stable_sort(orc):
 
 def test_ribbon_layout_sets_the_ribbons_flag():
     from bevy_hanabi_b200 import _native as N
-    from tests.test_gpu_ribbons import _ribbon_asset
-    assert _ribbon_asset(16).generate().flags & N.EFFECT_RIBBONS
-    assert not E._firework_trails(16).generate().flags & N.EFFECT_RIBBONS
+    assert ribbon_asset(16).generate().flags & N.EFFECT_RIBBONS
+    assert not firework_trails(16).generate().flags & N.EFFECT_RIBBONS

@@ -11,13 +11,12 @@ from tests import static_emu as S
 from tests.helpers import Instance, RefWorld
 from tests.repack_ref import ref_repack
 from tests.snapshot_ref import HEADER_WORDS, SNAPSHOT_MAGIC, ref_restore, ref_snapshot, restore_count, snapshot_bytes
-from tests.test_identity_claim_emu_cpu import _claim, _claimed, _frame, claimed_driver  # noqa: F401
-from tests.test_kernel_emu_cpu import _assert_same, _c5_world
-from tests.test_repack_emu_cpu import REPACK_DRIVER, RepackArgs, SoaSlab, churned, expected_bits
+from tests.kernel_emu import assert_same, c5_frame, c5_world, claim, claimed
+from tests.static_emu import REPACK_DRIVER, RepackArgs, SoaSlab, churned, expected_bits
 
 pytestmark = pytest.mark.timeout(600)
 
-# Entry points of the snapshot kernels, appended (with the repack ones) to the static emulation's driver for this module
+# Entry points of the snapshot kernels, built with the repack ones (static_emu.build)
 SNAPSHOT_DRIVER = r"""
 extern "C" void semu_snapshot_gather(const SnapshotArgs* a, uint32_t* dst) {
     SnapshotArgs s = *a;
@@ -40,9 +39,7 @@ class SnapshotArgs(C.Structure):
 
 @pytest.fixture(scope="module")
 def slib():
-    with pytest.MonkeyPatch.context() as mp:
-        mp.setattr(S, "DRIVER", S.DRIVER + REPACK_DRIVER + SNAPSHOT_DRIVER)
-        lib = S.build()
+    lib = S.build(REPACK_DRIVER + SNAPSHOT_DRIVER)
     lib.semu_snapshot_gather.argtypes = [C.c_void_p, C.c_void_p]
     lib.semu_restore_scatter.argtypes = [C.c_void_p, C.c_void_p]
     lib.semu_repack_lists.argtypes = [C.c_void_p]
@@ -194,7 +191,7 @@ def test_restore_matches_the_oracle(slib, stride_words, sector, n, target):
     assert m == min(n, ref.instances[1].capacity)
     _assert_soa(soa, ref, target)
     np.testing.assert_array_equal(soa.bits, expected_bits(bits0, first, ref.instances[1].capacity, m), err_msg="alive bitmap")
-    assert soa.claims[0] == soa.claims[1] == _claim(first, m), "claim words"
+    assert soa.claims[0] == soa.claims[1] == claim(first, m), "claim words"
 
 
 @pytest.mark.parametrize("first", [0, 32, 45])
@@ -217,7 +214,7 @@ def test_small_slices_and_word_edges(slib, first):
             what = f"first {first}, rows {rows}, n {n}"
             _assert_soa(soa, ref, what)
             np.testing.assert_array_equal(soa.bits, expected_bits(bits0, first, rows, m), err_msg=what)
-            assert soa.claims[0] == soa.claims[1] == _claim(first, m), what
+            assert soa.claims[0] == soa.claims[1] == claim(first, m), what
 
 
 @pytest.mark.parametrize("corruption", ["magic", "version", "stride", "short", "very_short", "header_only"])
@@ -248,7 +245,7 @@ def test_corrupt_or_short_snapshots(slib, corruption):
     _assert_soa(soa, ref, corruption)
     if corruption in ("magic", "version", "stride"):
         assert ref.metadata[1].particle_counter == counter
-    assert soa.claims[0] == soa.claims[1] == _claim(100, m)
+    assert soa.claims[0] == soa.claims[1] == claim(100, m)
 
 
 def test_round_trip_equals_repack(slib):
@@ -266,36 +263,36 @@ def test_round_trip_equals_repack(slib):
     np.testing.assert_array_equal(ref.indirect, repacked.indirect)
     np.testing.assert_array_equal(ref.metadata_rows(), repacked.metadata_rows())
     np.testing.assert_array_equal(ref.particles[37:37 + n], repacked.particles[37:37 + n])
-    assert soa.claims[0] == soa.claims[1] == _claim(37, n)
+    assert soa.claims[0] == soa.claims[1] == claim(37, n)
 
 
-def test_restore_between_emulated_frames(orc, slib, claimed_driver):  # noqa: F811
+def test_restore_between_emulated_frames(orc, slib):
     """C5 through the emulated init and update kernels: frames with deaths and bursts into recycled slots, a snapshot,
     then a restore into a fresh 1200-row world (fewer rows than are alive) and more frames there. Every buffer equals
     the oracle after every frame; the frames after the restore run under the claims the restore wrote."""
     rng = np.random.default_rng(3)
-    ref = _c5_world(rng, [Instance(0, 3000, alive=2500, seed=42)])
-    emu, _ = _claimed(ref, 2, 0)
+    ref = c5_world(rng, [Instance(0, 3000, alive=2500, seed=42)])
+    emu, _ = claimed(ref, 2, 0)
     for f, spawn in enumerate([0, 400, 0, 300, 0, 0, 250]):
         ref.sim.time = np.float32(f) * ref.sim.delta_time
-        _frame(orc, ref, emu, spawn)
-        _assert_same(ref, emu.pull(), f"frame {f}")
+        c5_frame(orc, ref, emu, spawn)
+        assert_same(ref, emu.pull(), f"frame {f}")
     assert ref.metadata[0].alive_count > 1200
     snap = np.full(snapshot_bytes(32, 3000) // 4, 0xA5A5A5A5, dtype=np.uint32)
     emulate_snapshot(slib, emu.planes, [16, 16], emu.cols, emu.metadata, 0, 0, 3000, 8, snap)
     np.testing.assert_array_equal(snap[:HEADER_WORDS + 8 * ref.metadata[0].alive_count], ref_snapshot(ref, 0))
 
-    dst = _c5_world(rng, [Instance(0, 1200, alive=0, seed=42)])
+    dst = c5_world(rng, [Instance(0, 1200, alive=0, seed=42)])
     dst.indirect[:, 2] = rng.permutation(1200).astype(np.uint32)
-    demu, claims = _claimed(dst, 2, 0)
+    demu, claims = claimed(dst, 2, 0)
     bits = np.zeros(1200 // 32 + 2, dtype=np.uint32)
     emulate_restore(slib, demu.planes, [16, 16], demu.cols, bits, claims, demu.metadata, 0, 0, 1200, 8, snap)
     m = ref_restore(dst, 0, snap)
     assert m == 1200
-    _assert_same(dst, demu.pull(), "after the restore")
-    assert claims[0] == claims[1] == _claim(0, m)
+    assert_same(dst, demu.pull(), "after the restore")
+    assert claims[0] == claims[1] == claim(0, m)
     for f, spawn in enumerate([0, 0, 200, 0, 0], start=7):
         dst.sim.time = np.float32(f) * dst.sim.delta_time
-        _frame(orc, dst, demu, spawn)
-        _assert_same(dst, demu.pull(), f"frame {f}, after the restore")
+        c5_frame(orc, dst, demu, spawn)
+        assert_same(dst, demu.pull(), f"frame {f}, after the restore")
     assert dst.metadata[0].alive_count < 1200

@@ -11,11 +11,11 @@ sys.path.insert(0, str(ROOT))
 from oracle import c_oracle  # noqa: E402
 from oracle.hanabi_oracle import EffectOracle  # noqa: E402
 from tests.helpers import Instance, RefWorld  # noqa: E402
-from tests.test_gpu_scene import _drifting_sparks  # noqa: E402
+from tests.effects import drifting_sparks  # noqa: E402
 
 orc = c_oracle.load()
 P = 1 << 16
-asset = _drifting_sparks(P)
+asset = drifting_sparks(P)
 _, size, _ = asset.particle_layout()
 ref = RefWorld(P, size // 4, [Instance(0, P, alive=0, seed=1)], dt=1 / 60)
 eo = EffectOracle(asset)

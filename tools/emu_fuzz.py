@@ -15,18 +15,15 @@ sys.path.insert(0, str(ROOT))
 from oracle import c_oracle  # noqa: E402
 from oracle.hanabi_oracle import EffectOracle, pcg_hash  # noqa: E402
 from tests import static_emu  # noqa: E402
+from tests.effects import drifting_sparks, firework_trails, growing_dust, ribbon_asset  # noqa: E402
 from tests.helpers import Instance, RefWorld  # noqa: E402
-from tests.kernel_emu import EmuWorld  # noqa: E402
-from tests.test_gpu_effects import _firework_trails  # noqa: E402
-from tests.test_gpu_ribbons import _ribbon_asset  # noqa: E402
-from tests.test_gpu_scene import _drifting_sparks, _growing_dust  # noqa: E402
-from tests.test_kernel_emu_cpu import _assert_same  # noqa: E402
+from tests.kernel_emu import EmuWorld, assert_same  # noqa: E402
 
 
 def one(seed, orc, slib, sector_mix=False):
     rng = np.random.default_rng(seed)
     kind = int(rng.integers(0, 4))
-    asset = [_drifting_sparks, _firework_trails, _growing_dust, _ribbon_asset][kind](1)
+    asset = [drifting_sparks, firework_trails, growing_dust, ribbon_asset][kind](1)
     fields, size, _ = asset.particle_layout()
     n_inst = int(rng.integers(1, 10))
     caps = [int(rng.choice([1, 2, 31, 32, 33, 64, 127, 128, 129, 255, 256, 257, 511, 512, 513, 1023, 1024, 1025, 1500, 2049, 2600])) for _ in range(n_inst)]
@@ -55,7 +52,7 @@ def one(seed, orc, slib, sector_mix=False):
         ref.set_spawns(spawns, seeds)
         eo.frame(ref, orc)
         emu.frame_step(orc, ref.sim, spawns, seeds)
-        _assert_same(ref, emu.pull(), f"seed {seed} kind {kind} caps {caps} chunks {chunks} ctas {ctas} sector {sector} frame {f}")
+        assert_same(ref, emu.pull(), f"seed {seed} kind {kind} caps {caps} chunks {chunks} ctas {ctas} sector {sector} frame {f}")
     return kind
 
 

@@ -1,5 +1,5 @@
-"""Long-running fuzz of GPU spawn events under the CPU emulation: tests/test_kernel_emu_cpu.py::test_random_event_scenes over many
-seeds, default (atomic) and ordered append.   python tools/emu_fuzz_events.py [seconds] [first_seed]"""
+"""Long-running fuzz of GPU spawn events under the CPU emulation: tests/kernel_emu.py::random_event_scene (the scenes of
+tests/test_kernel_emu_cpu.py::test_random_event_scenes) over many seeds, default (atomic) and ordered append.   python tools/emu_fuzz_events.py [seconds] [first_seed]"""
 import sys
 import time
 from pathlib import Path
@@ -7,7 +7,7 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 from oracle import c_oracle  # noqa: E402
-from tests.test_kernel_emu_cpu import test_random_event_scenes  # noqa: E402
+from tests.kernel_emu import random_event_scene  # noqa: E402
 
 budget = float(sys.argv[1]) if len(sys.argv) > 1 else 120.0
 seed = int(sys.argv[2]) if len(sys.argv) > 2 else 3
@@ -15,7 +15,7 @@ orc = c_oracle.load()
 t0, n = time.time(), 0
 while time.time() - t0 < budget:
     for ordered in (False, True):
-        test_random_event_scenes(orc, ordered, seed)
+        random_event_scene(orc, ordered, seed)
         n += 1
     seed += 1
     if n % 10 == 0:

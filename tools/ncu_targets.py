@@ -85,25 +85,25 @@ def c5_init():
 
 
 def c3(mi):
-    from tests.test_gpu_effects import _force_field
+    from tests.effects import force_field
     P = mi << 20
-    asset = _force_field(P)
+    asset = force_field(P)
     burst(asset, P, P, props=asset.serialize_properties())
 
 
 def c2():
     """firework trails at its BASELINE capacity: 32768 slots, a burst of 30000, then plain frames."""
-    from tests.test_gpu_effects import _firework_trails
-    burst(_firework_trails(32768), 32768, 30000, update_frames=2)
+    from tests.effects import firework_trails
+    burst(firework_trails(32768), 32768, 30000, update_frames=2)
 
 
 def c4():
     """C4: 1024 instances x 65536 slots in one batch with the instancing.rs recipe: a frame that spawns one particle per
     instance into a nearly full slab (init with a depth-10 prefix search + bookkeeping of 1024 instances + update of 64 Mi)."""
-    from tests.test_gpu_config_sizes import _instancing
+    from tests.effects import instancing
     n_inst, cap = 1024, 65536
     ctx = hb.Context(0, stream.cuda_stream)
-    fx = _instancing(cap).generate()
+    fx = instancing(cap).generate()
     slab = ctx.slab_create(n_inst * cap, fx.particle_stride)
     effect = ctx.effect_compile(fx)
     for i in range(n_inst):
@@ -125,10 +125,10 @@ def c4():
 
 def churn(slot_order=False):
     """The steady-state churn world of perf_matrix.churn (16 Mi slots, ~13 Mi alive in recycled slots): one profiled frame."""
-    from tests.test_gpu_scene import _drifting_sparks
+    from tests.effects import drifting_sparks
     P = 16 << 20
     ctx = hb.Context(0, stream.cuda_stream)
-    fx = _drifting_sparks(P).generate(slot_order=slot_order)
+    fx = drifting_sparks(P).generate(slot_order=slot_order)
     slab = ctx.slab_create(P, fx.particle_stride)
     effect = ctx.effect_compile(fx)
     ctx.metadata_insert(0, R.initial_metadata(P, 0, fx.particle_stride // 4))

@@ -165,20 +165,20 @@ def c5_init_burst():
 
 
 def c2_trails():
-    from tests.test_gpu_effects import _firework_trails
-    _burst("C2 trails, 32Mi burst", _firework_trails(40 << 20), 40 << 20, 32 << 20)
+    from tests.effects import firework_trails
+    _burst("C2 trails, 32Mi burst", firework_trails(40 << 20), 40 << 20, 32 << 20)
 
 
 def c3_force_field():
-    from tests.test_gpu_effects import _force_field
+    from tests.effects import force_field
     for P in (1 << 20, 16 << 20):
-        asset = _force_field(P)
+        asset = force_field(P)
         _burst(f"C3 force field, {P >> 20}Mi burst", asset, P, P, props=asset.serialize_properties())
 
 
 def c3_fast_math():
-    from tests.test_gpu_effects import _force_field
-    asset = _force_field(16 << 20)
+    from tests.effects import force_field
+    asset = force_field(16 << 20)
     _burst("C3 force field FAST_MATH, 16Mi burst", asset, 16 << 20, 16 << 20, props=asset.serialize_properties(), fast_math=True)
 
 
@@ -210,10 +210,10 @@ def many_batches():
 
 def _churned(sector_planes: bool = False, slot_order: bool = False):
     """16 Mi slots of drifting sparks after 240 frames of constant spawning into recycled slots."""
-    from tests.test_gpu_scene import _drifting_sparks
+    from tests.effects import drifting_sparks
     P = 16 << 20
     ctx = hb.Context(0, stream.cuda_stream)
-    asset = _drifting_sparks(P)          # lifetimes U(0.2, 0.9) s
+    asset = drifting_sparks(P)          # lifetimes U(0.2, 0.9) s
     fx = asset.generate(sector_planes=sector_planes, slot_order=slot_order)
     stride = fx.particle_stride
     slab = ctx.slab_create(P, stride, sector_planes=sector_planes)
@@ -544,10 +544,10 @@ def interop():
 def c2_small():
     """BASELINE configs[1] at ITS size: firework trails, 32768 slots (48-byte records). The whole population is 1.5 MB: a
     frame is pure fixed cost (launch chain + dependent-load latency), reported in microseconds per frame."""
-    from tests.test_gpu_effects import _firework_trails
+    from tests.effects import firework_trails
     P = 32768
     ctx = hb.Context(0, stream.cuda_stream)
-    fx = _firework_trails(P).generate()
+    fx = firework_trails(P).generate()
     slab = ctx.slab_create(P, fx.particle_stride)
     effect = ctx.effect_compile(fx)
     ctx.metadata_insert(0, R.initial_metadata(P, 0, fx.particle_stride // 4))
@@ -578,10 +578,10 @@ def c4_recipe():
     """BASELINE configs[3] as stated (SURVEY 8d row C4): instancing.rs recipe, 1024 instances x 65536 slots in ONE batch, filled
     through the real init kernel; update-only frames, then frames that spawn one particle per instance (init with a
     depth-10 prefix search over 1024 instances + bookkeeping of 1024 instances + update)."""
-    from tests.test_gpu_config_sizes import _instancing
+    from tests.effects import instancing
     n_inst, cap = 1024, 65536
     ctx = hb.Context(0, stream.cuda_stream)
-    fx = _instancing(cap).generate()
+    fx = instancing(cap).generate()
     stride = fx.particle_stride
     slab = ctx.slab_create(n_inst * cap, stride)
     effect = ctx.effect_compile(fx)
@@ -617,10 +617,10 @@ def c4_recipe():
 
 def c3_chain():
     """C3 at its BASELINE size (1 Mi) as a frame chain (what a running effect costs per frame), strict and fast-math."""
-    from tests.test_gpu_effects import _force_field
+    from tests.effects import force_field
     P = 1 << 20
     for fast in (False, True):
-        asset = _force_field(P)
+        asset = force_field(P)
         ctx = hb.Context(0, stream.cuda_stream)
         fx = asset.generate(fast_math=fast)
         slab = ctx.slab_create(P, fx.particle_stride)

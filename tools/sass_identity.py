@@ -20,11 +20,10 @@ sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 
 def sources():
     from bevy_hanabi_b200 import recipes
-    from tests.test_gpu_events import _assets
-    from tests.test_gpu_effects import _force_field
-    p, c = _assets()
+    from tests.effects import event_assets, force_field
+    p, c = event_assets()
     return {"c5": recipes.c5_lowered().generate_source(), "parent": p.generate(num_event_bindings=1).generate_source(),
-            "child": c.generate(parent=p).generate_source(), "ff": _force_field(10).generate().generate_source()}
+            "child": c.generate(parent=p).generate_source(), "ff": force_field(10).generate().generate_source()}
 
 
 def sass(name, src, d: Path):

@@ -5,10 +5,10 @@ import numpy as np
 import torch
 import bevy_hanabi_b200 as hb
 from bevy_hanabi_b200 import _native as N, runtime as R
-from tests.test_gpu_ribbons import _ribbon_asset
+from tests.effects import ribbon_asset
 stream = torch.cuda.Stream(); torch.cuda.set_stream(stream)
 ctx = hb.Context(0, stream.cuda_stream)
-asset = _ribbon_asset(16); fx = asset.generate(); fields, size, _ = asset.particle_layout()
+asset = ribbon_asset(16); fx = asset.generate(); fields, size, _ = asset.particle_layout()
 off = {f.name: f.offset // 4 for f in fields}; words = size // 4
 effect = ctx.effect_compile(fx)
 for n in (512, 2048, 16384, 1 << 18, 1 << 20, 1 << 22):
