@@ -93,7 +93,7 @@ class SlabView(C.Structure):
 
 
 class AttrLayout(C.Structure):
-    _fields_ = [("name", C.c_char_p), ("value_type", u32), ("offset", u32)]
+    _fields_ = [("name", C.c_char_p), ("value_type", u32), ("offset", u32), ("flags", u32)]
 
 
 class EffectDesc(C.Structure):
@@ -134,6 +134,7 @@ EFFECT_ORDERED_EVENTS = 1 << 7
 EFFECT_SECTOR_PLANES = 1 << 8
 EFFECT_SLOT_ORDER = 1 << 9
 SLAB_SECTOR_PLANES = 1 << 0
+ATTR_UPDATE_READ_ONLY = 1 << 0
 
 
 def _load() -> C.CDLL:
@@ -193,6 +194,8 @@ SIGNATURES = {
     "hnb_compile_job_destroy": (None, [vp]),
     "hnb_effect_create_from_job": (i32, [vp, vp, P(u32)]),
     "hnb_effect_generate_source": (i32, [P(EffectDesc), C.c_char_p, C.c_size_t, P(C.c_size_t)]),
+    "hnb_effect_generate_source_for_plan": (i32, [P(EffectDesc), u32, P(u32), P(u32), C.c_char_p, C.c_size_t, P(C.c_size_t)]),
+    "hnb_effect_column_plan": (i32, [P(EffectDesc), P(u32), P(u32), P(u32)]),
     "hnb_nvrtc_check": (i32, [C.c_char_p, P(C.c_size_t)]),
     "hnb_set_sim_params": (i32, [vp, P(SimParams)]),
     "hnb_upload_spawners": (i32, [vp, P(Spawner), u32]),
@@ -222,6 +225,7 @@ SIGNATURES = {
     "hnb_ctx_set_count_mailbox": (i32, [vp, vp, u32, u32]),
     "hnb_ctx_last_epoch": (i32, [vp, P(u32)]),
     "hnb_ctx_tile_state_clears": (i32, [vp, P(C.c_uint64)]),
+    "hnb_ctx_plan_compiles": (i32, [vp, P(C.c_uint64)]),
     "hnb_host_alloc": (vp, [C.c_size_t]),
     "hnb_host_free": (None, [vp]),
     "hnb_ctx_read_debug": (i32, [vp, P(C.c_uint64), i32]),

@@ -83,6 +83,7 @@ void fill_layout(const ParticleLayout& pl, hnb_attr_layout* out, uint32_t cap, u
         out[i].name = static_name(pl.layout[i].name);
         out[i].value_type = pl.layout[i].type.code;
         out[i].offset = pl.layout[i].offset;
+        out[i].flags = 0;
     }
 }
 
@@ -258,6 +259,7 @@ int32_t hnb_asset_property_layout(const hnb_asset* a, hnb_attr_layout* out, uint
             out[i].name = nm;
             out[i].value_type = pl.layout[i].property.default_value.type.code;
             out[i].offset = pl.layout[i].offset;
+            out[i].flags = 0;
         }
     });
 }
@@ -289,12 +291,15 @@ int32_t hnb_asset_generate(const hnb_asset* a, const hnb_asset* parent, uint32_t
         auto g = std::make_unique<hnb_generated>();
         g->src = a->a.generate(parent ? &parent_layout : nullptr, num_event_bindings);
         g->name = a->a.name;
-        auto fill = [](const ParticleLayout& pl, std::vector<hnb_attr_layout>& v) {
-            for (const auto& l : pl.layout)
-                if (!l.is_pad) v.push_back({static_name(l.name), l.type.code, l.offset});
+        auto fill = [](const ParticleLayout& pl, std::vector<hnb_attr_layout>& v, const std::set<Attribute>* writes) {
+            for (const auto& l : pl.layout) {
+                if (l.is_pad) continue;
+                const bool read_only = writes && !writes->count(attribute_by_name(l.name));
+                v.push_back({static_name(l.name), l.type.code, l.offset, read_only ? uint32_t(HNB_ATTR_UPDATE_READ_ONLY) : 0u});
+            }
         };
-        fill(g->src.particle_layout, g->attrs);
-        if (g->src.parent_layout) fill(*g->src.parent_layout, g->parent_attrs);
+        fill(g->src.particle_layout, g->attrs, &g->src.update_writes);
+        if (g->src.parent_layout) fill(*g->src.parent_layout, g->parent_attrs, nullptr);
         *out = g.release();
     });
 }

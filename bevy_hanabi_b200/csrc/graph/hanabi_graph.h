@@ -252,6 +252,7 @@ struct Modifier {
     std::vector<uint32_t> params;   // kind-specific flags (attribute id, kill_inside, dimension, condition, child index)
     uint32_t allowed_contexts() const;          // bitmask of ModifierContext
     std::vector<Attribute> attributes() const;  // Modifier::attributes()
+    std::vector<Attribute> update_writes() const;  // attributes the code apply() emits in the update context assigns
     void apply(Module& module, ShaderWriter& ctx) const;  // Modifier::apply, emitting CUDA C
 };
 
@@ -267,6 +268,7 @@ struct EffectShaderSource {  // what generate() substitutes into the kernel temp
     std::string properties_struct;
     std::string init_code, init_extra, sim_space_code, age_code, reap_code, update_code, update_extra;
     uint32_t flags = 0;  // HNB_EFFECT_* layout flags
+    std::set<Attribute> update_writes;  // attributes the update body assigns; the others are HNB_ATTR_UPDATE_READ_ONLY
     std::optional<ParticleLayout> parent_layout;
     uint32_t num_event_bindings = 0;
 };

@@ -83,6 +83,20 @@ std::vector<Attribute> Modifier::attributes() const {
     return {};
 }
 
+std::vector<Attribute> Modifier::update_writes() const {
+    switch (kind) {
+        case ModifierKind::Accel: case ModifierKind::RadialAccel: case ModifierKind::TangentAccel: case ModifierKind::ConformToSphere:
+        case ModifierKind::LinearDrag: case ModifierKind::SetVelocityCircle: case ModifierKind::SetVelocitySphere:
+        case ModifierKind::SetVelocityTangent:
+            return {attr::VELOCITY};
+        case ModifierKind::SetPositionCircle: case ModifierKind::SetPositionSphere: case ModifierKind::SetPositionCone3d:
+            return {attr::POSITION};
+        case ModifierKind::SetAttribute: case ModifierKind::InheritAttribute: return {(Attribute)param(*this, 0)};
+        case ModifierKind::KillSphere: case ModifierKind::KillAabb: case ModifierKind::EmitSpawnEvent: return {};
+    }
+    return {};
+}
+
 void Modifier::apply(Module& module, ShaderWriter& context) const {
     const ModifierContext mc = context.modifier_context();
     if (!((uint32_t)mc & allowed_contexts())) throw ExprError(ExprError::InvalidModifierContext, "modifier used in an invalid context");
@@ -383,7 +397,10 @@ EffectShaderSource EffectAsset::generate(const ParticleLayout* parent_layout, ui
     bool emit = false;
     {
         ShaderWriter ctx(ModifierContext::Update, out.property_layout, out.particle_layout);
-        for (const auto& m : update_modifiers) m.apply(mod, ctx);
+        for (const auto& m : update_modifiers) {
+            m.apply(mod, ctx);
+            for (Attribute a : m.update_writes()) out.update_writes.insert(a);
+        }
         emit = ctx.emits_gpu_spawn_events().value_or(false);
         out.update_code = ctx.main_code;
         out.update_extra = ctx.extra_code;
@@ -398,6 +415,7 @@ EffectShaderSource EffectAsset::generate(const ParticleLayout* parent_layout, ui
         const std::string code = "\nparticle.position += particle.velocity * sim_params.delta_time;\n";
         if (motion_integration == MotionIntegration::PreUpdate) out.update_code.insert(0, code);
         else out.update_code += code;
+        out.update_writes.insert(attr::POSITION);
     }
 
     // aging / reaping (lib.rs:1223-1264)
@@ -406,6 +424,7 @@ EffectShaderSource EffectAsset::generate(const ParticleLayout* parent_layout, ui
         if (has_lifetime) out.age_code += "\n    const bool was_alive = particle.age < particle.lifetime; (void)was_alive;";
         else out.age_code += "\n    const bool was_alive = true; (void)was_alive;";  // the reference leaves it undeclared (latent bug)
         out.age_code += "\n    particle.age = particle.age + sim_params.delta_time;";
+        out.update_writes.insert(attr::AGE);
         if (has_lifetime) out.age_code += "\n    is_alive = particle.age < particle.lifetime;";
     } else {
         out.age_code = "\n    const bool was_alive = true; (void)was_alive;\n    is_alive = true;";

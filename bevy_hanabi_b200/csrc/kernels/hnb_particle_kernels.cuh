@@ -9,6 +9,7 @@
 //   HNB_RELAXED_ORDER, HNB_TILE_K
 //   struct Particle;  struct Properties;  struct RawParticle;  [struct ParentParticle]
 //   hnb_load_raw / hnb_store_raw / hnb_unpack / hnb_pack       (SoA planes <-> Particle)
+//   hnb_store_written                          the update's store: only the columns holding a word it may write
 //   hnb_init_body(Particle&, Ctx&)            = {{INIT_CODE}} + PREV/NEXT reset + {{SIM_SPACE}}
 //   hnb_update_body(Particle&, Ctx&) -> bool  = {{AGE_CODE}} {{REAP_CODE}} {{UPDATE_CODE}}, returns is_alive
 //
@@ -728,11 +729,13 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
                     }
 #endif
                     // hnb_pack<false> leaves the PREV/NEXT words of raw[k] as they were LOADED, and the store below writes whole
-                    // planes: the links are written back unchanged. That equals the reference's WRITEBACK_CODE (which never
-                    // stores them) only because no kernel of this path maintains links while an update is in flight; a
-                    // link-maintaining pass added later must not overlap hnb_update (or PREV/NEXT must get a plane of their own).
+                    // columns: a column that also holds a word the update writes gets its links written back unchanged.
+                    // That equals the reference's WRITEBACK_CODE (which never stores them) only because no kernel of this
+                    // path maintains links while an update is in flight; a link-maintaining pass added later must not
+                    // overlap hnb_update, or PREV/NEXT must be declared HNB_ATTR_UPDATE_READ_ONLY (the graph lowering does),
+                    // which gives them columns of their own that hnb_store_written never stores.
                     hnb_pack<false>(particle, raw[k]);
-                    hnb_store_raw(raw[k], P.slab, base_particle + pidx[k]);
+                    hnb_store_written(raw[k], P.slab, base_particle + pidx[k]);
                 }
                 const u32 ballot = __ballot_sync(0xffffffffu, alive);
                 if (lane == 0) survivors[j * HNB_TILE_K + k] = ballot;

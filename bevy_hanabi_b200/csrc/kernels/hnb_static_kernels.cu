@@ -408,7 +408,8 @@ __global__ void k_bits_from_list(u32* bits, const u32* list, u32 base, u32 alive
 //   s = pcg_hash(row ^ seed); six successive pcg_hash -> position, velocity in [-1,1); one more -> lifetime
 // `logical_first`: row of the LOGICAL instance stored at slab row `first` (a shard of an instance split by index range
 // over several devices holds the unsharded instance's values under shard-local indices).
-__global__ void k_fill_c5(float4* pos_age, float4* vel_life, u32* ping, u32* pong, u64* claim, u32 first, u32 count, u32 seed,
+// The eight record words go to whatever columns the slab's plan gives them.
+__global__ void k_fill_c5(PlaneSet planes, u32* ping, u32* pong, u64* claim, u32 first, u32 count, u32 seed,
                           f32 lifetime_lo, f32 lifetime_hi, u32 logical_first) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
@@ -420,9 +421,13 @@ __global__ void k_fill_c5(float4* pos_age, float4* vel_life, u32* ping, u32* pon
     u32 s = pcg_hash((logical_first + i) ^ seed);
     f32 v[7];
     for (int k = 0; k < 7; ++k) { s = pcg_hash(s); v[k] = to_float01(s); }
-    pos_age[row] = make_float4(v[0] * 2.0f - 1.0f, v[1] * 2.0f - 1.0f, v[2] * 2.0f - 1.0f, 0.0f);
-    vel_life[row] = make_float4(v[3] * 2.0f - 1.0f, v[4] * 2.0f - 1.0f, v[5] * 2.0f - 1.0f,
-                                lifetime_lo + v[6] * (lifetime_hi - lifetime_lo));
+    const f32 rec[8] = {v[0] * 2.0f - 1.0f, v[1] * 2.0f - 1.0f, v[2] * 2.0f - 1.0f, 0.0f,
+                        v[3] * 2.0f - 1.0f, v[4] * 2.0f - 1.0f, v[5] * 2.0f - 1.0f, lifetime_lo + v[6] * (lifetime_hi - lifetime_lo)};
+#pragma unroll
+    for (u32 w = 0; w < 8; ++w) {
+        const u32 p = planes.word_to_plane[w];
+        ((f32*)planes.ptr[p])[u64(row) * planes.words[p] + (w - planes.word_off[p])] = rec[w];
+    }
     ping[row] = i;  // instance-local identity alive list in both columns
     pong[row] = i;
 }
@@ -863,9 +868,9 @@ cudaError_t launch_bits_from_list(u32* bits, const u32* list, u32 base, u32 aliv
     k_bits_from_list<<<blocks_for(alive_count, 256), 256, 0, st>>>(bits, list, base, alive_count);
     return cudaGetLastError();
 }
-cudaError_t launch_fill_c5(void* pos_age, void* vel_life, u32* ping, u32* pong, u64* claim, u32 first, u32 count, u32 seed, f32 lo, f32 hi, u32 logical_first, cudaStream_t st) {
+cudaError_t launch_fill_c5(const PlaneSet& planes, u32* ping, u32* pong, u64* claim, u32 first, u32 count, u32 seed, f32 lo, f32 hi, u32 logical_first, cudaStream_t st) {
     if (count == 0) return cudaSuccess;
-    k_fill_c5<<<blocks_for(count, 256), 256, 0, st>>>((float4*)pos_age, (float4*)vel_life, ping, pong, claim, first, count, seed, lo, hi, logical_first);
+    k_fill_c5<<<blocks_for(count, 256), 256, 0, st>>>(planes, ping, pong, claim, first, count, seed, lo, hi, logical_first);
     return cudaGetLastError();
 }
 cudaError_t launch_repack_gather(const RepackArgs& a, const void* col, void* scratch, u32 width, cudaStream_t st) {

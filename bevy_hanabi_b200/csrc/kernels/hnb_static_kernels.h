@@ -128,7 +128,7 @@ cudaError_t launch_planes_to_aos(u32* aos, const PlaneSet& planes, u32 first, u3
 cudaError_t launch_indirect_interleave(u32* rows3, const u32* ping, const u32* pong, const u32* dead, u32 first, u32 count, cudaStream_t st);
 cudaError_t launch_indirect_deinterleave(const u32* rows3, u32* ping, u32* pong, u32* dead, u32 first, u32 count, cudaStream_t st);
 // also sets the identity claims `claim[2]` of both columns to {first, count}
-cudaError_t launch_fill_c5(void* pos_age, void* vel_life, u32* ping, u32* pong, u64* claim, u32 first, u32 count, u32 seed, f32 lo, f32 hi, u32 logical_first, cudaStream_t st);
+cudaError_t launch_fill_c5(const PlaneSet& planes, u32* ping, u32* pong, u64* claim, u32 first, u32 count, u32 seed, f32 lo, f32 hi, u32 logical_first, cudaStream_t st);
 cudaError_t launch_measure_sm_clock(u64* out2, u64 window_ns, cudaStream_t st);
 cudaError_t launch_checksum(const PlaneSet& planes, u32 first, u32 count, u32 stride_words, u64 index_base, u64* out, cudaStream_t st);
 

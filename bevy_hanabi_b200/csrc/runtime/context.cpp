@@ -86,8 +86,13 @@ struct Slab {
     bool live = false;
     uint32_t capacity = 0, stride = 0;
     bool sector_planes = false;  // HNB_SLAB_SECTOR_PLANES
-    std::vector<Plane> planes;   // physical columns
-    DeviceArray<char> d_planes[HNB_RT_MAX_PLANES];
+    // Physical columns, carved from one zero-filled block of capacity x stride bytes: column p starts at capacity x
+    // planes[p].offset. The first effect bound to the slab fixes the plan (fix_plan); before that, calls that write
+    // records write the default cut (`written`).
+    std::vector<Plane> planes;
+    bool plan_fixed = false, written = false;
+    DeviceArray<char> d_block;
+    char* column(size_t p) const { return d_block.get() + size_t(capacity) * planes[p].offset; }
     DeviceArray<uint32_t> ping, pong, dead;
     DeviceArray<uint32_t> alive_bits;  // one bit per row (HNB_EFFECT_SLOT_ORDER effects keep it current)
     DeviceArray<unsigned long long> ident_claim;  // [2]: identity claims of ping / pong (hnb_claim_pack)
@@ -103,12 +108,48 @@ struct KernelModule {
     std::string log;
 };
 
+// A deep copy of an effect descriptor: what a context needs to compile the effect again for another column plan.
+struct OwnedDesc {
+    hnb_effect_desc d{};
+    std::vector<std::string> names, parent_names;
+    std::vector<hnb_attr_layout> attrs, parent_attrs;
+    std::string name, properties_struct, init_code, init_extra, sim_space_code, age_code, reap_code, update_code, update_extra;
+    explicit OwnedDesc(const hnb_effect_desc& src) {
+        auto s = [](const char* p) { return std::string(p ? p : ""); };
+        name = s(src.name); properties_struct = s(src.properties_struct); init_code = s(src.init_code);
+        init_extra = s(src.init_extra); sim_space_code = s(src.sim_space_code); age_code = s(src.age_code);
+        reap_code = s(src.reap_code); update_code = s(src.update_code); update_extra = s(src.update_extra);
+        auto copy = [&](const hnb_attr_layout* a, uint32_t n, std::vector<std::string>& ns, std::vector<hnb_attr_layout>& out) {
+            for (uint32_t i = 0; a && i < n; ++i) ns.push_back(s(a[i].name));
+            for (uint32_t i = 0; a && i < n; ++i) out.push_back({ns[i].c_str(), a[i].value_type, a[i].offset, a[i].flags});
+        };
+        copy(src.attrs, src.n_attrs, names, attrs);
+        copy(src.parent_attrs, src.n_parent_attrs, parent_names, parent_attrs);
+        d = src;
+        d.name = name.c_str(); d.properties_struct = src.properties_struct ? properties_struct.c_str() : nullptr;
+        d.init_code = init_code.c_str(); d.init_extra = init_extra.c_str(); d.sim_space_code = sim_space_code.c_str();
+        d.age_code = age_code.c_str(); d.reap_code = reap_code.c_str(); d.update_code = update_code.c_str();
+        d.update_extra = update_extra.c_str();
+        d.attrs = attrs.empty() ? nullptr : attrs.data();
+        d.parent_attrs = parent_attrs.empty() ? nullptr : parent_attrs.data();
+    }
+    OwnedDesc(const OwnedDesc&) = delete;
+    OwnedDesc& operator=(const OwnedDesc&) = delete;
+};
+
 struct Effect {
     bool live = false;
     uint64_t hash = 0;
-    KernelModule* km = nullptr;
+    KernelModule* km = nullptr;        // the module of the effect's own column plan
+    std::vector<Plane> plan;           // column_plan of the descriptor
+    std::shared_ptr<const OwnedDesc> desc;
+    struct PlanModule {
+        std::vector<Plane> plan, parent_plan;  // parent_plan empty: a parent slab in the default cut
+        KernelModule* km;
+    };
+    std::vector<PlanModule> plan_modules;  // modules for slabs (or parent slabs) of other plans
+    bool fast_math = false;
     uint32_t tile_k = 4, flags = 0, particle_stride = 0, parent_stride = 0, rows_per_lane = 16, update_smem = 0;
-    int update_blocks_per_sm = 1;
     uint32_t props_size = 0, props_stride = 0;
     DeviceArray<char> d_props;  // rows of props_stride bytes
     std::string name;
@@ -188,6 +229,7 @@ struct hnb_ctx {
     std::vector<DeviceArray<unsigned long long>> d_tile_state;  // per batch
     std::vector<hnb_rt::TileStateSlot> tile_state_slot;  // when the batch's states were last zeroed (tile_state_rule.h)
     uint64_t tile_state_clears = 0;  // zeroings tile_state_needs_clear asked for (hnb_ctx_tile_state_clears)
+    uint64_t plan_compiles = 0;      // (effect, other column plan) modules made by module_for_plan (hnb_ctx_plan_compiles)
     uint64_t md_generation = 1;            // bumped by hnb_metadata_insert
 
     std::vector<Slab> slabs;
@@ -333,20 +375,55 @@ Effect& get_effect(hnb_ctx* c, hnb_effect e) {
     return c->effects[e];
 }
 
-hnb::PlaneSet plane_set(const Slab& s) {
+hnb::PlaneSet plane_set(const std::vector<Plane>& planes, char* block, uint32_t capacity) {
     hnb::PlaneSet ps{};
-    for (size_t p = 0; p < s.planes.size(); ++p) {
-        ps.ptr[p] = s.d_planes[p].get();
-        ps.words[p] = s.planes[p].width / 4;
-        ps.word_off[p] = s.planes[p].offset / 4;
-        for (uint32_t w = 0; w < s.planes[p].width / 4; ++w) ps.word_to_plane[s.planes[p].offset / 4 + w] = (unsigned char)p;
+    for (size_t p = 0; p < planes.size(); ++p) {
+        ps.ptr[p] = block + size_t(capacity) * planes[p].offset;
+        ps.words[p] = planes[p].width / 4;
+        ps.word_off[p] = planes[p].offset / 4;
+        for (uint32_t w = 0; w < planes[p].width / 4; ++w) ps.word_to_plane[planes[p].offset / 4 + w] = (unsigned char)p;
     }
     return ps;
 }
+hnb::PlaneSet plane_set(const Slab& s) { return plane_set(s.planes, s.d_block.get(), s.capacity); }
+
+// AoS records <-> columns go through a device staging buffer in chunks of this size.
+constexpr size_t kChunkBytes = size_t(64) << 20;
+
+// The first effect bound to a slab (a launch, hnb_slab_repack, hnb_instance_restore) gives it that effect's column plan;
+// later binds keep it, and so does a slab whose columns were handed out (hnb_slab_device_view pins the plan it shows).
+// Records written before (in the default cut) move to the new columns once, through a second block of capacity x stride
+// bytes and one synchronisation; when that block cannot be allocated the slab keeps its default cut (the effect then runs
+// a module generated for it). Callers validate everything else first: a failure here leaves the slab as it was.
+void fix_plan(hnb_ctx* c, Slab& s, const std::vector<Plane>& plan) {
+    if (s.plan_fixed) return;
+    if (plan != s.planes && s.written) {
+        DeviceArray<char> next, staging;
+        const uint32_t rows_per_chunk = (uint32_t)std::min<size_t>(s.capacity, std::max<size_t>(1, kChunkBytes / s.stride));
+        if (next.alloc(size_t(s.capacity) * s.stride) != cudaSuccess || staging.alloc(size_t(rows_per_chunk) * s.stride) != cudaSuccess) {
+            (void)cudaGetLastError();
+            s.plan_fixed = true;
+            return;
+        }
+        const hnb::PlaneSet from = plane_set(s), to = plane_set(plan, next.get(), s.capacity);
+        uint32_t* stage = reinterpret_cast<uint32_t*>(staging.get());
+        for (uint32_t done = 0; done < s.capacity; done += rows_per_chunk) {
+            const uint32_t n = std::min(rows_per_chunk, s.capacity - done);
+            CUDA_CHECK(hnb::launch_planes_to_aos(stage, from, done, n, s.stride / 4, c->stream));
+            CUDA_CHECK(hnb::launch_aos_to_planes(stage, to, done, n, s.stride / 4, c->stream));
+            c->launches += 2;
+        }
+        CUDA_CHECK(cudaStreamSynchronize(c->stream));  // the old block and the staging buffer are released below
+        s.d_block.swap(next);
+    }
+    s.planes = plan;
+    s.plan_fixed = true;
+}
+void fix_default_plan(hnb_ctx* c, Slab& s) { fix_plan(c, s, physical_planes(s.stride, s.sector_planes)); }
 
 hnb::SlabView slab_view(const Slab& s) {
     hnb::SlabView v{};
-    for (size_t p = 0; p < s.planes.size(); ++p) v.planes[p] = s.d_planes[p].get();
+    for (size_t p = 0; p < s.planes.size(); ++p) v.planes[p] = s.column(p);
     v.particle_index[0] = s.ping.get();
     v.particle_index[1] = s.pong.get();
     v.dead_index = s.dead.get();
@@ -372,8 +449,6 @@ void check_rows(const Slab& s, uint32_t first, uint32_t count) {
     if (uint64_t(first) + count > s.capacity) fail(HNB_ERR_OUT_OF_RANGE, "row range exceeds slab capacity");
 }
 
-// Staging through a device buffer in chunks (AoS <-> planes transposes run on the device).
-constexpr size_t kChunkBytes = size_t(64) << 20;
 
 // `precompiled`: a cubin already built for exactly this source (hnb_compile_job), or NULL to compile here.
 KernelModule* get_module(hnb_ctx* c, const std::string& source, const std::string& name, uint64_t hash, bool fast_math,
@@ -391,15 +466,44 @@ KernelModule* get_module(hnb_ctx* c, const std::string& source, const std::strin
     if (r != CUDA_SUCCESS) fail(HNB_ERR_CUDA, "cuModuleGetFunction(hnb_init): " + cu_error_string(c->drv, r));
     r = c->drv.ModuleGetFunction(&km->update, km->mod, "hnb_update");
     if (r != CUDA_SUCCESS) fail(HNB_ERR_CUDA, "cuModuleGetFunction(hnb_update): " + cu_error_string(c->drv, r));
-    km->update_blocks_per_sm = 1;  // per effect: depends on its dynamic shared memory (see hnb_effect_compile)
+    km->update_blocks_per_sm = 1;  // depends on the effect's dynamic shared memory (set_update_smem)
     KernelModule* out = km.get();
     c->modules.emplace(hash, std::move(km));
     return out;
 }
 
+// Lets hnb_update of `km` take `smem` bytes of dynamic shared memory and records how many of its CTAs fit on an SM.
+void set_update_smem(hnb_ctx* c, KernelModule* km, uint32_t smem) {
+    CUresult r = c->drv.FuncSetAttribute(km->update, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem);
+    if (r != CUDA_SUCCESS) fail(HNB_ERR_CUDA, "cuFuncSetAttribute(max dynamic smem " + std::to_string(smem) + "): " + cu_error_string(c->drv, r));
+    int bps = 0;
+    r = c->drv.OccupancyMaxActiveBlocksPerMultiprocessor(&bps, km->update, 256, smem);
+    km->update_blocks_per_sm = (r != CUDA_SUCCESS || bps < 1) ? 1 : bps;
+}
+
+// The module that runs `fx` on a slab of column plan `plan`, reading a parent slab of plan `parent` (NULL: none, or the
+// default cut): the effect's own, or one compiled for these plans on first use.
+KernelModule* module_for_plan(hnb_ctx* c, Effect& fx, const std::vector<Plane>& plan, const std::vector<Plane>* parent) {
+    static const std::vector<Plane> kDefault;
+    const std::vector<Plane>& pp = parent ? *parent : kDefault;
+    if (plan == fx.plan && pp.empty()) return fx.km;
+    for (const auto& pm : fx.plan_modules)
+        if (pm.plan == plan && pm.parent_plan == pp) return pm.km;
+    const std::string source = generate_effect_source(fx.desc->d, &plan, parent);
+    KernelModule* km = get_module(c, source, fx.name, fnv1a64(source), fx.fast_math);
+    set_update_smem(c, km, fx.update_smem);
+    fx.plan_modules.push_back({plan, pp, km});
+    c->plan_compiles++;
+    return km;
+}
+
 struct LaunchPlan {
     Effect* fx;
     Slab* slab;
+    KernelModule* km;  // fx compiled for `target` (and the parent slab's plan)
+    // The plan the slab has, or will have once adopt_plans fixes it (the effect's own); then the parent slab, if any.
+    const std::vector<Plane>* target;
+    Slab* parent;
     uint32_t batch;
     uint32_t total_spawn;
     hnb::BatchParams params;
@@ -422,6 +526,16 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
     if (lp.fx->particle_stride != lp.slab->stride) fail(HNB_ERR_LAYOUT, "effect particle stride does not match the slab");
     if (((lp.fx->flags & HNB_EFFECT_SECTOR_PLANES) != 0) != lp.slab->sector_planes)
         fail(HNB_ERR_LAYOUT, "effect and slab disagree on HNB_EFFECT_SECTOR_PLANES / HNB_SLAB_SECTOR_PLANES");
+    lp.target = lp.slab->plan_fixed ? &lp.slab->planes : &lp.fx->plan;  // nothing changes before the frame is validated
+    lp.parent = nullptr;
+    const std::vector<Plane>* parent_plan = nullptr;
+    if (bl.parent_slab != 0xFFFFFFFFu) {
+        lp.parent = &get_slab(c, bl.parent_slab);
+        if (lp.parent->sector_planes) fail(HNB_ERR_LAYOUT, "a parent slab read by a child effect must not use sector planes");
+        // an unbound parent slab is in the default cut, and adopt_plans keeps it there
+        if (!is_default_cut(lp.parent->planes, lp.parent->stride)) parent_plan = &lp.parent->planes;
+    }
+    lp.km = module_for_plan(c, *lp.fx, *lp.target, parent_plan);
     if (bl.batch_info_index >= c->B) fail(HNB_ERR_OUT_OF_RANGE, "batch_info_index out of range");
     lp.batch = bl.batch_info_index;
     lp.total_spawn = bl.total_spawn_count;
@@ -438,7 +552,7 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
     //    an earlier GPU. On an H100 (tools/sweep_small.py, C5) the rule is within 3 % of the best forced chunk count from
     //    1 Mi rows up; at 256-512 Ki rows forcing 3-4 chunks shortens the frame by 15-20 % (not retuned).
     const uint32_t sub_tile = 32u * lp.fx->tile_k;
-    const uint32_t total_warps = uint32_t(lp.fx->update_blocks_per_sm) * uint32_t(c->sm_count) * 8u;
+    const uint32_t total_warps = uint32_t(lp.km->update_blocks_per_sm) * uint32_t(c->sm_count) * 8u;
     const uint32_t max_chunks = std::max(1u, lp.fx->rows_per_lane / lp.fx->tile_k);
     uint32_t chunks = c->tile_chunks_override;
     if (chunks == 0) {
@@ -540,11 +654,7 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
     P.properties = lp.fx->d_props.get();
     P.properties_stride = lp.fx->props_stride;
     P.slab = slab_view(*lp.slab);
-    if (bl.parent_slab != 0xFFFFFFFFu) {
-        const Slab& parent = get_slab(c, bl.parent_slab);
-        if (parent.sector_planes) fail(HNB_ERR_LAYOUT, "a parent slab read by a child effect must use the default plane layout");
-        P.parent_slab = slab_view(parent);
-    }
+    if (lp.parent) P.parent_slab = slab_view(*lp.parent);
     if (consume) P.consume_events = c->event_buffers[bl.consume_events].get();
     for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
         if (bl.emit_events[i] != 0xFFFFFFFFu) {
@@ -575,10 +685,27 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
     P.tile_rows = tile_word;
     lp.init_blocks = ceil_div(init_threads, 256 * hnb_rt::kInitItems);  // HNB_INIT_ITEMS logical init threads per CUDA thread
     uint32_t max_tiles = lp.slab->capacity / small_tile + bi.prefix_sum_count + 1;
-    lp.update_blocks = std::min<uint32_t>(ceil_div(max_tiles, 8), uint32_t(lp.fx->update_blocks_per_sm) * uint32_t(c->sm_count));
+    lp.update_blocks = std::min<uint32_t>(ceil_div(max_tiles, 8), uint32_t(lp.km->update_blocks_per_sm) * uint32_t(c->sm_count));
     if (lp.update_blocks == 0) lp.update_blocks = 1;
     if (lp.fx->props_size && !lp.fx->d_props) fail(HNB_ERR_NOT_READY, "effect uses properties but none were uploaded");
     return lp;
+}
+
+// After every launch of a call has been planned and validated: the first bind of a slab fixes its plan (fix_plan; an
+// unbound parent slab keeps the default cut), which may move its records, so the launch parameters take the columns
+// again. A launch whose slab ended in another plan than it was planned for (two effects of different plans binding one
+// fresh slab in one frame, or no memory for the move) is planned again.
+void adopt_plans(hnb_ctx* c, LaunchPlan* plans, const hnb_batch_launch* batches, uint32_t n, bool set_ranges) {
+    for (uint32_t i = 0; i < n; ++i) {
+        fix_plan(c, *plans[i].slab, *plans[i].target);
+        if (plans[i].parent) fix_default_plan(c, *plans[i].parent);
+    }
+    for (uint32_t i = 0; i < n; ++i) {
+        LaunchPlan& lp = plans[i];
+        if (lp.slab->planes != *lp.target) lp = plan_batch(c, batches[i], set_ranges);
+        lp.params.slab = slab_view(*lp.slab);
+        if (lp.parent) lp.params.parent_slab = slab_view(*lp.parent);
+    }
 }
 
 // hnb_init / hnb_update start with griddepcontrol.wait, so they may always be launched with programmatic stream
@@ -609,7 +736,7 @@ void launch_update(hnb_ctx* c, LaunchPlan& lp, cudaStream_t st = nullptr) {
         else { CUDA_CHECK(ev.first.create(cudaEventDefault)); CUDA_CHECK(ev.second.create(cudaEventDefault)); }
         CUDA_CHECK(cudaEventRecord(ev.first, st));
     }
-    launch_kernel(c, lp.fx->km->update, lp.update_blocks, lp.params, lp.fx->update_smem, st);
+    launch_kernel(c, lp.km->update, lp.update_blocks, lp.params, lp.fx->update_smem, st);
     if (c->timing) {
         CUDA_CHECK(cudaEventRecord(ev.second, st));
         c->ev_pending.push_back(std::move(ev));
@@ -799,8 +926,9 @@ int32_t hnb_slab_create_ex(hnb_ctx* c, uint32_t capacity_rows, uint32_t stride, 
         s.stride = stride;
         s.sector_planes = (flags & HNB_SLAB_SECTOR_PLANES) != 0;
         s.planes = physical_planes(stride, s.sector_planes);
-        // planes zero-filled (debug builds of the reference poison the particle buffer instead, effect_cache.rs:284-296)
-        for (size_t p = 0; p < s.planes.size(); ++p) CUDA_CHECK(grow(s.d_planes[p], size_t(capacity_rows) * s.planes[p].width, 0, c->stream));
+        s.plan_fixed = s.sector_planes;  // sector-plane effects address the sector cut only
+        // zero-filled (debug builds of the reference poison the particle buffer instead, effect_cache.rs:284-296)
+        CUDA_CHECK(grow(s.d_block, size_t(capacity_rows) * stride, 0, c->stream));
         CUDA_CHECK(s.ping.alloc(capacity_rows));
         CUDA_CHECK(s.pong.alloc(capacity_rows));
         CUDA_CHECK(s.dead.alloc(capacity_rows));
@@ -852,6 +980,7 @@ void transfer_aos(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, void* 
     Slab& s = get_slab(c, h);
     check_rows(s, first, count);
     if (count == 0) return;
+    s.written |= upload;
     const uint32_t rows_per_chunk = (uint32_t)std::max<size_t>(1, kChunkBytes / s.stride);
     DeviceArray<char> staging;
     CUDA_CHECK(staging.alloc(size_t(std::min(rows_per_chunk, count)) * s.stride));
@@ -930,6 +1059,7 @@ int32_t hnb_slab_import_aos_device(hnb_ctx* c, hnb_slab h, uint32_t first, uint3
         check_rows(s, first, count);
         if (count && !d_src) fail(HNB_ERR_INVALID_ARG, "d_src is NULL");
         if ((uintptr_t)d_src & 3u) fail(HNB_ERR_INVALID_ARG, "d_src must be 4-byte aligned (16-byte aligned for full speed)");
+        s.written = true;
         CUDA_CHECK(hnb::launch_aos_to_planes((const uint32_t*)d_src, plane_set(s), first, count, s.stride / 4, c->stream));
         c->launches += count ? 1 : 0;
     });
@@ -957,12 +1087,13 @@ int32_t hnb_slab_device_view(hnb_ctx* c, hnb_slab h, hnb_slab_view* out) {
     return guarded([&] {
         Slab& s = get_slab(c, h);
         if (!out) fail(HNB_ERR_INVALID_ARG, "out is NULL");
+        fix_default_plan(c, s);  // handed-out columns never move: an unbound slab keeps the default cut from now on
         memset(out, 0, sizeof(*out));
         out->capacity_rows = s.capacity;
         out->particle_stride = s.stride;
         out->num_planes = (uint32_t)s.planes.size();
         for (size_t p = 0; p < s.planes.size(); ++p) {
-            out->planes[p] = s.d_planes[p].get();
+            out->planes[p] = s.column(p);
             out->plane_offset[p] = s.planes[p].offset;
             out->plane_width[p] = s.planes[p].width;
         }
@@ -1007,8 +1138,9 @@ int32_t hnb_slab_fill_c5_ex(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t cou
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
         if (s.stride != 32) fail(HNB_ERR_LAYOUT, "hnb_slab_fill_c5 needs the 32-byte {position,age,velocity,lifetime} layout");
-        if (s.sector_planes) fail(HNB_ERR_LAYOUT, "hnb_slab_fill_c5 writes the default plane layout; spawn through the init pass or use hnb_slab_upload_aos");
-        CUDA_CHECK(hnb::launch_fill_c5(s.d_planes[0].get(), s.d_planes[1].get(), s.ping.get(), s.pong.get(), s.ident_claim.get(), first, count, seed, lo, hi,
+        if (s.sector_planes) fail(HNB_ERR_LAYOUT, "hnb_slab_fill_c5 writes the default or a column plan; spawn through the init pass or use hnb_slab_upload_aos");
+        s.written = true;
+        CUDA_CHECK(hnb::launch_fill_c5(plane_set(s), s.ping.get(), s.pong.get(), s.ident_claim.get(), first, count, seed, lo, hi,
                                        logical_first, c->stream));
         CUDA_CHECK(hnb::launch_bits_range(s.alive_bits.get(), first, count, true, c->stream));
         c->launches += 2;
@@ -1066,6 +1198,7 @@ int32_t hnb_slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_
         const Effect& fx = get_effect(c, e);
         check_instance_slice(c, s, fx, metadata_row, first, rows, "hnb_slab_repack");
         if (rows == 0) return;
+        fix_plan(c, s, fx.plan);
         CUDA_CHECK(cudaSetDevice(c->device));
         const hnb::RepackArgs a = repack_args(c, s, metadata_row, first, rows);
         uint32_t widest = 0;
@@ -1075,9 +1208,9 @@ int32_t hnb_slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_
         cudaError_t err = cudaSuccess;
         for (size_t p = 0; p < s.planes.size() && err == cudaSuccess; ++p) {
             const uint32_t width = s.planes[p].width;
-            err = hnb::launch_repack_gather(a, s.d_planes[p].get(), scratch, width, c->stream);
+            err = hnb::launch_repack_gather(a, s.column(p), scratch, width, c->stream);
             if (err == cudaSuccess)
-                err = cudaMemcpyAsync(s.d_planes[p].get() + size_t(first) * width, scratch, size_t(rows) * width, cudaMemcpyDeviceToDevice, c->stream);
+                err = cudaMemcpyAsync(s.column(p) + size_t(first) * width, scratch, size_t(rows) * width, cudaMemcpyDeviceToDevice, c->stream);
             c->launches++;
         }
         // the lists last: every gather reads them
@@ -1126,6 +1259,8 @@ int32_t hnb_instance_restore(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t meta
         if (src_bytes < sizeof(hnb_instance_snapshot_header)) fail(HNB_ERR_INVALID_ARG, "hnb_instance_restore: src_bytes is below the 64-byte header");
         if (rows == 0) return;
         CUDA_CHECK(cudaSetDevice(c->device));
+        fix_plan(c, s, fx.plan);
+        s.written = true;
         hnb::SnapshotArgs a = snapshot_args(c, s, metadata_row, first, rows);
         a.src_bytes = src_bytes;
         CUDA_CHECK(hnb::launch_restore_scatter(a, (const uint32_t*)d_src, c->stream));
@@ -1177,15 +1312,43 @@ int32_t hnb_slab_checksum_indirect(hnb_ctx* c, hnb_slab h, uint32_t first, uint3
 }
 
 // ---- effects --------------------------------------------------------------------------------
+namespace {
+void copy_source(const std::string& src, char* out, size_t cap, size_t* len) {
+    if (len) *len = src.size();
+    if (out && cap) {
+        size_t n = std::min(cap - 1, src.size());
+        memcpy(out, src.data(), n);
+        out[n] = 0;
+    }
+}
+}  // namespace
+
 int32_t hnb_effect_generate_source(const hnb_effect_desc* desc, char* out, size_t cap, size_t* len) {
     return guarded([&] {
         if (!desc) fail(HNB_ERR_INVALID_ARG, "desc is NULL");
-        std::string src = generate_effect_source(*desc);
-        if (len) *len = src.size();
-        if (out && cap) {
-            size_t n = std::min(cap - 1, src.size());
-            memcpy(out, src.data(), n);
-            out[n] = 0;
+        copy_source(generate_effect_source(*desc), out, cap, len);
+    });
+}
+
+int32_t hnb_effect_generate_source_for_plan(const hnb_effect_desc* desc, uint32_t n_planes, const uint32_t* offsets, const uint32_t* widths,
+                                            char* out, size_t cap, size_t* len) {
+    return guarded([&] {
+        if (!desc || !offsets || !widths) fail(HNB_ERR_INVALID_ARG, "NULL argument");
+        if (n_planes > HNB_RT_MAX_PLANES) fail(HNB_ERR_INVALID_ARG, "more than 16 columns");
+        std::vector<Plane> plan;
+        for (uint32_t p = 0; p < n_planes; ++p) plan.push_back({offsets[p], widths[p]});
+        copy_source(generate_effect_source(*desc, &plan), out, cap, len);
+    });
+}
+
+int32_t hnb_effect_column_plan(const hnb_effect_desc* desc, uint32_t* offsets, uint32_t* widths, uint32_t* n) {
+    return guarded([&] {
+        if (!desc || !n) fail(HNB_ERR_INVALID_ARG, "NULL argument");
+        const std::vector<Plane> plan = column_plan(desc->particle_stride, desc->attrs, desc->attrs ? desc->n_attrs : 0, desc->flags);
+        *n = (uint32_t)plan.size();
+        for (size_t p = 0; p < plan.size(); ++p) {
+            if (offsets) offsets[p] = plan[p].offset;
+            if (widths) widths[p] = plan[p].width;
         }
     });
 }
@@ -1208,10 +1371,14 @@ struct EffectBlueprint {
     uint64_t hash = 0;
     bool fast_math = false;
     uint32_t tile_k = 4, rows_per_lane = 16, update_smem = 0, flags = 0, particle_stride = 0, parent_stride = 0, props_size = 0;
+    std::vector<Plane> plan;
+    std::shared_ptr<const OwnedDesc> desc;
 };
 static EffectBlueprint make_blueprint(const hnb_effect_desc& desc) {
     EffectBlueprint bp;
     bp.source = generate_effect_source(desc);
+    bp.plan = column_plan(desc.particle_stride, desc.attrs, desc.n_attrs, desc.flags);
+    bp.desc = std::make_shared<const OwnedDesc>(desc);
     bp.hash = fnv1a64(bp.source);
     bp.name = desc.name ? desc.name : "effect";
     bp.fast_math = (desc.flags & HNB_EFFECT_FAST_MATH) != 0;  // the flag is part of the source (hash)
@@ -1234,14 +1401,10 @@ static hnb_effect install_effect(hnb_ctx* c, const EffectBlueprint& bp, const st
     fx.tile_k = bp.tile_k;
     fx.rows_per_lane = bp.rows_per_lane;
     fx.update_smem = bp.update_smem;
-    {
-        CUresult r = c->drv.FuncSetAttribute(fx.km->update, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)fx.update_smem);
-        if (r != CUDA_SUCCESS) fail(HNB_ERR_CUDA, "cuFuncSetAttribute(max dynamic smem " + std::to_string(fx.update_smem) + "): " + cu_error_string(c->drv, r));
-        int bps = 0;
-        r = c->drv.OccupancyMaxActiveBlocksPerMultiprocessor(&bps, fx.km->update, 256, fx.update_smem);
-        if (r != CUDA_SUCCESS || bps < 1) bps = 1;
-        fx.update_blocks_per_sm = bps;
-    }
+    set_update_smem(c, fx.km, fx.update_smem);
+    fx.plan = bp.plan;
+    fx.desc = bp.desc;
+    fx.fast_math = bp.fast_math;
     fx.flags = bp.flags;
     fx.particle_stride = bp.particle_stride;
     fx.parent_stride = bp.parent_stride;
@@ -1454,6 +1617,7 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
         plans.reserve(n);
         for (uint32_t i = 0; i < n; ++i) plans.push_back(plan_batch(c, batches[i], true));
         check_coverage(c, plans);  // nothing has been enqueued yet: a bad frame is skipped as a whole
+        adopt_plans(c, plans.data(), batches, n, true);
         next_epoch(c);
         // The frame block reaches the device with ONE copy — or with none: when no table row, tile size or init range
         // changed since the last upload (a steady-state frame without spawns), the only new bytes are the 64-byte
@@ -1492,7 +1656,7 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
             Fork fork(c, reads_parent ? 1 : inits);
             uint32_t k = 0;
             for (auto& lp : plans)
-                if (lp.init_blocks) launch_kernel(c, lp.fx->km->init, lp.init_blocks, lp.params, hnb_rt::kInitSmemBytes, fork.lane(k++));
+                if (lp.init_blocks) launch_kernel(c, lp.km->init, lp.init_blocks, lp.params, hnb_rt::kInitSmemBytes, fork.lane(k++));
             fork.join();
         }
         // passes "hanabi:indirect_dispatch" + "hanabi:update_prefix_sum" (mod.rs:7182-7275), fused
@@ -1559,6 +1723,7 @@ int32_t hnb_pass_sort(hnb_ctx* c, const hnb_batch_launch* b) {
         if (!b) fail(HNB_ERR_INVALID_ARG, "batch is NULL");
         ensure_scratch(c);
         LaunchPlan lp = plan_batch(c, *b, false);
+        adopt_plans(c, &lp, b, 1, false);
         flush_arena(c, false);
         launch_ribbon_sort(c, lp);
     });
@@ -1575,11 +1740,12 @@ int32_t hnb_pass_init(hnb_ctx* c, const hnb_batch_launch* b) {
         if (b->batch_info_index < c->init_pending.size() && c->init_pending[b->batch_info_index])
             fail(HNB_ERR_INVALID_ARG, "hnb_pass_init: this batch already has an init pass pending; run hnb_pass_indirect first");
         LaunchPlan lp = plan_batch(c, *b, true);
+        adopt_plans(c, &lp, b, 1, true);
         c->header()->num_batches = c->B;
         if (c->header()->epoch == 0) next_epoch(c);
         flush_arena(c, true);
         if (lp.init_blocks) {
-            launch_kernel(c, lp.fx->km->init, lp.init_blocks, lp.params, hnb_rt::kInitSmemBytes);
+            launch_kernel(c, lp.km->init, lp.init_blocks, lp.params, hnb_rt::kInitSmemBytes);
             if (c->init_pending.size() <= b->batch_info_index) c->init_pending.resize(size_t(b->batch_info_index) + 1, 0);
             c->init_pending[b->batch_info_index] = 1;
         }
@@ -1619,6 +1785,7 @@ int32_t hnb_pass_update(hnb_ctx* c, const hnb_batch_launch* b) {
         if (!b) fail(HNB_ERR_INVALID_ARG, "batch is NULL");
         ensure_scratch(c);
         LaunchPlan lp = plan_batch(c, *b, false);
+        adopt_plans(c, &lp, b, 1, false);
         next_epoch(c);
         flush_arena(c, false);
         CUDA_CHECK(hnb::launch_tile_prefix(static_tables(c), lp.batch, lp.params.tile_rows, c->stream));
@@ -1723,6 +1890,12 @@ int32_t hnb_ctx_tile_state_clears(hnb_ctx* c, uint64_t* clears) {
     return guarded([&] {
         if (!c || !clears) fail(HNB_ERR_INVALID_ARG, "NULL argument");
         *clears = c->tile_state_clears;
+    });
+}
+int32_t hnb_ctx_plan_compiles(hnb_ctx* c, uint64_t* compiles) {
+    return guarded([&] {
+        if (!c || !compiles) fail(HNB_ERR_INVALID_ARG, "NULL argument");
+        *compiles = c->plan_compiles;
     });
 }
 

@@ -75,6 +75,52 @@ std::vector<Plane> physical_planes(uint32_t stride_bytes, bool sector_planes) {
 
 namespace {
 
+// Per AoS word: does some attribute the update may write cover it (attributes without HNB_ATTR_UPDATE_READ_ONLY)?
+std::vector<bool> written_words(uint32_t stride, const hnb_attr_layout* attrs, uint32_t n_attrs) {
+    std::vector<bool> written(stride / 4, false);
+    for (uint32_t i = 0; i < n_attrs; ++i) {
+        const auto ti = value_type_info(attrs[i].value_type);
+        if (attrs[i].offset & 3u || attrs[i].offset + 4u * ti.count > stride) throw std::invalid_argument("attribute offset out of the particle record");
+        if (attrs[i].flags & HNB_ATTR_UPDATE_READ_ONLY) continue;
+        for (int c = 0; c < ti.count; ++c) written[attrs[i].offset / 4 + c] = true;
+    }
+    return written;
+}
+
+bool any_read_only(const hnb_attr_layout* attrs, uint32_t n_attrs) {
+    for (uint32_t i = 0; i < n_attrs; ++i)
+        if (attrs[i].flags & HNB_ATTR_UPDATE_READ_ONLY) return true;
+    return false;
+}
+
+}  // namespace
+
+std::vector<Plane> column_plan(uint32_t stride, const hnb_attr_layout* attrs, uint32_t n_attrs, uint32_t effect_flags) {
+    if (effect_flags & HNB_EFFECT_SECTOR_PLANES) return physical_planes(stride, true);
+    std::vector<Plane> cut = cut_planes(stride);
+    if ((effect_flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS) || !any_read_only(attrs, n_attrs)) return cut;
+    const std::vector<bool> written = written_words(stride, attrs, n_attrs);
+    std::vector<Plane> out;
+    for (uint32_t w = 0; w < written.size();) {
+        uint32_t end = w;
+        while (end < written.size() && written[end] == written[w]) ++end;
+        // a column of width W starts at a multiple of W: a slab block carves it at capacity * offset bytes, aligned for
+        // W-byte loads whatever the capacity
+        for (uint32_t off = 4 * w; off < 4 * end;) {
+            uint32_t width = 16;
+            while (width > 4 && (off % width || off + width > 4 * end)) width /= 2;
+            out.push_back({off, width});
+            off += width;
+        }
+        w = end;
+    }
+    return out.size() > HNB_RT_MAX_PLANES ? cut : out;
+}
+
+bool is_default_cut(const std::vector<Plane>& plan, uint32_t stride) { return plan == cut_planes(stride); }
+
+namespace {
+
 const char* comp_name(int c) {
     static const char* n[] = {"x", "y", "z", "w"};
     return n[c];
@@ -107,9 +153,10 @@ static std::string piece_address(const std::vector<Plane>& pieces, size_t p, boo
     throw std::logic_error("piece_address");
 }
 
+// `planes`: the record pieces the generated code addresses (the column plan; with sector planes the default cut, whose
+// 16-byte pieces pair up into 32-byte columns).
 void gen_layout_code(std::ostringstream& o, const char* prefix, const char* struct_name, const hnb_attr_layout* attrs,
-                     uint32_t n_attrs, uint32_t stride, bool with_store, bool sector = false) {
-    auto planes = cut_planes(stride);
+                     uint32_t n_attrs, uint32_t stride, const std::vector<Plane>& planes, bool with_store, bool sector = false) {
     // map AoS word -> field component
     std::vector<FieldRef> words(stride / 4);
     std::vector<bool> skip_pack(stride / 4, false);
@@ -155,6 +202,19 @@ void gen_layout_code(std::ostringstream& o, const char* prefix, const char* stru
     if (with_store) {
         o << "HNB_DI void " << fn_prefix << "store_raw(const " << raw_t << "& r, const SlabView& s, u32 row) {\n";
         for (size_t p = 0; p < planes.size(); ++p) {
+            const char* t = planes[p].width == 16 ? "float4" : planes[p].width == 8 ? "float2" : "f32";
+            o << "    HNB_STORE_PLANE(" << t << ", " << piece_address(planes, p, sector) << ", r.q" << p << ");\n";
+        }
+        o << "}\n";
+        // The update's store: the pieces holding a word the update may write. With no read-only attribute, every piece
+        // (the same stores as store_raw).
+        const bool all = !any_read_only(attrs, n_attrs);
+        const std::vector<bool> written = written_words(stride, attrs, n_attrs);
+        o << "HNB_DI void " << fn_prefix << "store_written(const " << raw_t << "& r, const SlabView& s, u32 row) {\n";
+        for (size_t p = 0; p < planes.size(); ++p) {
+            bool store = all;
+            for (uint32_t w = 0; w < planes[p].width / 4; ++w) store = store || written[planes[p].offset / 4 + w];
+            if (!store) continue;
             const char* t = planes[p].width == 16 ? "float4" : planes[p].width == 8 ? "float2" : "f32";
             o << "    HNB_STORE_PLANE(" << t << ", " << piece_address(planes, p, sector) << ", r.q" << p << ");\n";
         }
@@ -240,9 +300,23 @@ uint32_t choose_tile_k(const hnb_effect_desc& d) {
     return 1;
 }
 
-std::string generate_effect_source(const hnb_effect_desc& d) {
+void check_plan(const std::vector<Plane>& plan, uint32_t stride) {
+    uint32_t off = 0;
+    for (const Plane& p : plan) {
+        if (p.offset != off || (p.width != 4 && p.width != 8 && p.width != 16) || p.offset % p.width)
+            throw std::invalid_argument("column plan: columns must be contiguous, 4, 8 or 16 bytes wide and aligned to their width");
+        off += p.width;
+    }
+    if (off != stride || plan.empty() || plan.size() > HNB_RT_MAX_PLANES) throw std::invalid_argument("column plan does not cover the particle record");
+}
+
+std::string generate_effect_source(const hnb_effect_desc& d, const std::vector<Plane>* plan, const std::vector<Plane>* parent_plan) {
     if (!d.attrs || d.n_attrs == 0) throw std::invalid_argument("effect has an empty particle layout");
-    const auto planes = cut_planes(d.particle_stride);
+    const bool sector = (d.flags & HNB_EFFECT_SECTOR_PLANES) != 0;
+    if (plan && sector) throw std::invalid_argument("a sector-plane effect has no other column plan");
+    if (plan) check_plan(*plan, d.particle_stride);
+    if (parent_plan) check_plan(*parent_plan, d.parent_particle_stride);
+    const auto planes = sector ? cut_planes(d.particle_stride) : plan ? *plan : column_plan(d.particle_stride, d.attrs, d.n_attrs, d.flags);
     const bool read_parent = (d.flags & HNB_EFFECT_READ_PARENT_PARTICLE) != 0;
     const bool consume = (d.flags & HNB_EFFECT_CONSUME_GPU_SPAWN_EVENTS) != 0;
     const bool emit = (d.flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS) != 0;
@@ -296,8 +370,12 @@ std::string generate_effect_source(const hnb_effect_desc& d) {
          "#define HNB_STORE_PLANE(T, base, row, v) (((T*)(base))[row] = (v))\n"
          "#endif\n";
     // {{ATTRIBUTES}} / {{PROPERTIES}} / {{PARENT_ATTRIBUTES}}
-    gen_layout_code(o, "", "Particle", d.attrs, d.n_attrs, d.particle_stride, true, (d.flags & HNB_EFFECT_SECTOR_PLANES) != 0);
-    if (read_parent) gen_layout_code(o, "Parent", "ParentParticle", d.parent_attrs, d.n_parent_attrs, d.parent_particle_stride, false);
+    gen_layout_code(o, "", "Particle", d.attrs, d.n_attrs, d.particle_stride, planes, true, sector);
+    // a parent slab is read in the default cut (emitting effects keep it: column_plan), or in the plan its first bound
+    // effect gave it
+    if (read_parent)
+        gen_layout_code(o, "Parent", "ParentParticle", d.parent_attrs, d.n_parent_attrs, d.parent_particle_stride,
+                        parent_plan ? *parent_plan : cut_planes(d.parent_particle_stride), false);
     if (d.properties_size) {
         o << "struct Properties {\n" << nz(d.properties_struct) << "\n};\n";
         o << "static_assert(sizeof(Properties) == " << d.properties_size << ", \"Properties layout mismatch\");\n";

@@ -22,6 +22,7 @@ ValueTypeInfo value_type_info(uint32_t value_type);
 struct Plane {
     uint32_t offset;
     uint32_t width;
+    bool operator==(const Plane& o) const { return offset == o.offset && width == o.width; }
 };
 // Cut an AoS record of `stride_bytes` into planes: as many 16-byte planes as fit, then an 8- and/or
 // 4-byte tail. Because the reference layout keeps vec3/vec4 16-byte aligned and vec2 8-byte aligned
@@ -29,6 +30,12 @@ struct Plane {
 std::vector<Plane> cut_planes(uint32_t stride_bytes);
 // Physical columns of a slab: the pieces themselves, or (sector planes) pairs of 16-byte pieces in 32-byte-wide columns.
 std::vector<Plane> physical_planes(uint32_t stride_bytes, bool sector_planes);
+// The effect's column plan (hnb_effect_column_plan): the default cut unless some attribute is HNB_ATTR_UPDATE_READ_ONLY;
+// then runs of written / unwritten words get columns of their own, so the update stores only columns it writes.
+std::vector<Plane> column_plan(uint32_t stride_bytes, const hnb_attr_layout* attrs, uint32_t n_attrs, uint32_t effect_flags);
+bool is_default_cut(const std::vector<Plane>& plan, uint32_t stride_bytes);
+// Throws std::invalid_argument unless `plan` is contiguous 4/8/16-byte columns, each aligned to its width, covering the record.
+void check_plan(const std::vector<Plane>& plan, uint32_t stride_bytes);
 
 // Update tiles are walked by one warp each: tile_rows = 32 lanes * k rows per lane * chunks. k is
 // chosen from the record size (register footprint) at compile time, the chunk count per launch.
@@ -41,7 +48,9 @@ uint32_t choose_tile_k(const hnb_effect_desc& d);
 // parked-tile record + Properties staging).
 uint32_t update_smem_bytes(const hnb_effect_desc& d);
 
-// The complete translation unit (throws std::invalid_argument on a bad description).
-std::string generate_effect_source(const hnb_effect_desc& d);
+// The complete translation unit (throws std::invalid_argument on a bad description), for the effect's own column plan or
+// for `plan` (a slab's plan other than the effect's), reading a parent slab in the default cut or in `parent_plan`.
+std::string generate_effect_source(const hnb_effect_desc& d, const std::vector<Plane>* plan = nullptr,
+                                   const std::vector<Plane>* parent_plan = nullptr);
 
 }  // namespace hnb_rt

@@ -800,7 +800,8 @@ class EffectAsset:
                 return x.decode() if x else ""
 
             fx = LoweredEffect(
-                name=s(d.name), attrs=[AttrField(s(d.attrs[i].name), d.attrs[i].value_type, d.attrs[i].offset) for i in range(d.n_attrs)],
+                name=s(d.name), attrs=[AttrField(s(d.attrs[i].name), d.attrs[i].value_type, d.attrs[i].offset, d.attrs[i].flags)
+                                            for i in range(d.n_attrs)],
                 particle_stride=d.particle_stride, init_code=s(d.init_code), init_extra=s(d.init_extra), sim_space_code=s(d.sim_space_code),
                 age_code=s(d.age_code), reap_code=s(d.reap_code), update_code=s(d.update_code), update_extra=s(d.update_extra),
                 properties_struct=s(d.properties_struct), properties_size=d.properties_size,

@@ -48,8 +48,10 @@ def c5_generated_source() -> str:
 
 
 def c5_asset(capacity: int):
-    """Config C5 authored through the public API (the path a Hanabi user takes): the generated code is
-    identical to `c5_lowered()` (tests/test_authoring_cpu.py)."""
+    """Config C5 authored through the public API (the path a Hanabi user takes): the same update and init code as
+    `c5_lowered()` (tests/test_authoring_cpu.py), plus the lowering's write set: LIFETIME is declared
+    HNB_ATTR_UPDATE_READ_ONLY, so its column plan is [0,16) [16,24) [24,28) [28,32) where `c5_lowered()`, which declares
+    no write set, keeps the default cut."""
     from . import graph as G
     w = G.ExprWriter()
     A = G.Attribute

@@ -20,6 +20,7 @@ class AttrField:
     name: str
     value_type: int
     offset: int
+    flags: int = 0  # ATTR_UPDATE_READ_ONLY: the update body never assigns it
 
 
 @dataclass
@@ -53,7 +54,7 @@ class LoweredEffect:
         def arr(fields):
             a = (N.AttrLayout * max(1, len(fields)))()
             for i, f in enumerate(fields):
-                a[i] = N.AttrLayout(b(f.name), f.value_type, f.offset)
+                a[i] = N.AttrLayout(b(f.name), f.value_type, f.offset, f.flags)
             keep.append(a)
             return a
 
@@ -85,6 +86,24 @@ class LoweredEffect:
         check(lib.hnb_effect_generate_source(C.byref(d), None, 0, C.byref(n)))
         buf = C.create_string_buffer(n.value + 1)
         check(lib.hnb_effect_generate_source(C.byref(d), buf, n.value + 1, C.byref(n)))
+        return buf.value.decode()
+
+    def column_plan(self) -> list[tuple[int, int]]:
+        """The effect's column plan as (offset, width) pairs (hnb_effect_column_plan)."""
+        d, _keep = self.to_c()
+        off, wid, n = (C.c_uint32 * 16)(), (C.c_uint32 * 16)(), C.c_uint32()
+        check(lib.hnb_effect_column_plan(C.byref(d), off, wid, C.byref(n)))
+        return [(off[i], wid[i]) for i in range(n.value)]
+
+    def generate_source_for_plan(self, plan: Sequence[tuple[int, int]]) -> str:
+        """The translation unit a context compiles for this effect on a slab of column plan `plan`."""
+        d, _keep = self.to_c()
+        off = (C.c_uint32 * 16)(*[o for o, _ in plan])
+        wid = (C.c_uint32 * 16)(*[w for _, w in plan])
+        n = C.c_size_t(0)
+        check(lib.hnb_effect_generate_source_for_plan(C.byref(d), len(plan), off, wid, None, 0, C.byref(n)))
+        buf = C.create_string_buffer(n.value + 1)
+        check(lib.hnb_effect_generate_source_for_plan(C.byref(d), len(plan), off, wid, buf, n.value + 1, C.byref(n)))
         return buf.value.decode()
 
 
@@ -446,6 +465,12 @@ class Context:
         """How often a batch's look-back tile states were zeroed before an update launch (hnb_ctx_tile_state_clears)."""
         n = C.c_uint64(0)
         check(lib.hnb_ctx_tile_state_clears(self._h, C.byref(n)))
+        return n.value
+
+    def plan_compiles(self) -> int:
+        """Modules compiled for effects bound to slabs of another column plan (hnb_ctx_plan_compiles)."""
+        n = C.c_uint64(0)
+        check(lib.hnb_ctx_plan_compiles(self._h, C.byref(n)))
         return n.value
 
     def mailbox_count(self, epoch: int, row: int = 0, spin: bool = True):

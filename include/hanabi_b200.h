@@ -171,9 +171,19 @@ typedef uint32_t hnb_effect;  /* a compiled effect registered with a context (se
 /**
  * Allocate a slab of `capacity_rows` particles whose reference AoS record is
  * `particle_stride_bytes` (ParticleLayout::min_binding_size, attributes.rs:1837).
- * Storage is SoA: the AoS record is cut into 16-byte planes (float4 columns; an 8- or 4-byte
- * tail gets a float2/u32 column), plus three u32 columns ping/pong/dead. dead[i] = i
- * (effect_cache.rs:309-322); ping/pong = 0.
+ * Storage is SoA: one zero-filled block of capacity_rows x stride bytes, carved into columns (float4, float2 or u32
+ * elements) by a column plan (hnb_effect_column_plan), plus three u32 columns ping/pong/dead. dead[i] = i
+ * (effect_cache.rs:309-322); ping/pong = 0. Every plan fits the same block, so the plan is chosen late: the first effect
+ * bound to the slab (its first init/update launch, hnb_slab_repack or hnb_instance_restore) fixes that effect's plan.
+ * Before that the slab is in the default cut (what hnb_slab_device_view shows, and where hnb_slab_fill_c5 and the AoS
+ * uploads write); records written before the first bind move to the effect's columns then, once, after the launches of
+ * that call were validated (a device copy through a second block of capacity x stride bytes, and one synchronisation; if
+ * the block cannot be allocated the slab keeps the default cut). hnb_slab_device_view pins the plan it shows. A child
+ * reads its parent slab in whatever plan the slab has. An effect bound later to a slab of another plan runs a
+ * module compiled for the slab's plan (hnb_ctx_plan_compiles). Slabs of HNB_SLAB_SECTOR_PLANES keep the sector cut.
+ * A plan with columns narrower than 16 bytes costs more DRAM sectors per gathered record once an effect's alive list has
+ * become a permutation of its slice (C5: 4 sectors read and 3 written instead of 2 and 2); hnb_slab_repack or
+ * HNB_EFFECT_SLOT_ORDER restore coalesced access, sector planes halve the sectors of 16-byte pieces.
  */
 HNB_API int32_t hnb_slab_create(hnb_ctx* ctx, uint32_t capacity_rows, uint32_t particle_stride_bytes,
                                 hnb_slab* out);
@@ -328,7 +338,10 @@ typedef struct hnb_slab_view {
     uint32_t plane_width[16];  /* 16, 8 or 4 bytes (32 with HNB_SLAB_SECTOR_PLANES: two 16-byte pieces per element) */
     uint32_t *ping, *pong, *dead; /* the three u32 columns of IndirectEntry */
 } hnb_slab_view;
-/** A read path for renderers. Writing the index columns (ping / pong) through it is not supported: the update pass may
+/** A read path for renderers. The pointers, offsets and widths stay valid for the slab's lifetime: a slab whose plan no
+ * effect has fixed yet (section 3) is pinned to the default cut by this call, and effects bound to it later run modules
+ * generated for that cut. Take the view after the first hnb_simulate that binds the slab to see the effect's own plan.
+ * Writing the index columns (ping / pong) through it is not supported: the update pass may
  * skip alive-list loads and stores where it knows a column to be the identity, and a write through the view does not
  * drop that knowledge. Use hnb_slab_import_indirect_device or hnb_slab_upload_indirect to change the lists. */
 HNB_API int32_t hnb_slab_device_view(hnb_ctx* ctx, hnb_slab slab, hnb_slab_view* out);
@@ -367,7 +380,18 @@ typedef struct hnb_attr_layout {
     const char* name;    /* field name, e.g. "position" */
     uint32_t value_type; /* hnb_value_type */
     uint32_t offset;     /* byte offset in the AoS record */
+    uint32_t flags;      /* HNB_ATTR_* (0 = the update may write the attribute) */
 } hnb_attr_layout;
+
+/**
+ * HNB_ATTR_UPDATE_READ_ONLY: no code of the update body (age, reap, update code and UPDATE_EXTRA) assigns this attribute.
+ * The effect's column plan then gives the read-only words columns of their own, and the update pass stores only the
+ * columns that hold a word it writes: C5 ({position, age, velocity, lifetime}, lifetime read-only) moves 32 B read + 28 B
+ * written per particle-step instead of 32 + 32. The runtime trusts the declaration: an update that assigns a read-only
+ * attribute has the assignment dropped wherever the attribute sits in an unstored column. The graph lowering
+ * (hnb_asset_generate) sets the flag from the code it emits. Ignored for parent layouts.
+ */
+enum { HNB_ATTR_UPDATE_READ_ONLY = 1u << 0 };
 
 enum {
     HNB_EFFECT_LOCAL_SPACE = 1u << 0,          /* LayoutFlags::LOCAL_SPACE_SIMULATION */
@@ -450,6 +474,22 @@ HNB_API int32_t hnb_effect_create_from_job(hnb_ctx* ctx, hnb_compile_job* job, h
  * in *len. Used by the CPU test-suite (≙ the reference's naga validation tests).
  */
 HNB_API int32_t hnb_effect_generate_source(const hnb_effect_desc* desc, char* out, size_t cap, size_t* len);
+/** The effect's column plan (no GPU needed): *n columns, column p holding bytes [offsets[p], offsets[p] + widths[p]) of
+ *  every record (at most 16; `offsets` / `widths` may be NULL to ask for *n only). A pure function of the stride, the
+ *  attributes' offsets and HNB_ATTR_UPDATE_READ_ONLY flags, and the effect flags:
+ *   - no read-only attribute, HNB_EFFECT_SECTOR_PLANES or HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS: the default cut (as many
+ *     16-byte columns as fit, then an 8- and/or 4-byte tail; 32-byte-wide pairs with sector planes). Children read a
+ *     parent slab in the default cut;
+ *   - otherwise every maximal run of words of one class (written by the update, or not: read-only attributes and
+ *     padding) is cut into 16-, 8- and 4-byte columns, each at an offset that is a multiple of its width.
+ *     C5 with a read-only lifetime: [0,16) [16,24) [24,28) [28,32). A plan of more than 16 columns falls back to the
+ *     default cut. */
+HNB_API int32_t hnb_effect_column_plan(const hnb_effect_desc* desc, uint32_t* offsets, uint32_t* widths, uint32_t* n);
+/** hnb_effect_generate_source for the module a context compiles when the effect is bound to a slab whose plan is
+ *  `n_planes` columns (`offsets`, `widths`) other than its own: the update stores every column holding a word it may
+ *  write. */
+HNB_API int32_t hnb_effect_generate_source_for_plan(const hnb_effect_desc* desc, uint32_t n_planes, const uint32_t* offsets,
+                                                    const uint32_t* widths, char* out, size_t cap, size_t* len);
 /** NVRTC-compile a translation unit for sm_90a without loading it (no GPU needed). On failure
  *  the compiler log is available from hnb_last_error(). `cubin_size` may be NULL. */
 HNB_API int32_t hnb_nvrtc_check(const char* source, size_t* cubin_size);
@@ -547,6 +587,10 @@ HNB_API int32_t hnb_ctx_last_epoch(hnb_ctx* ctx, uint32_t* epoch);
  *  changed (effect, slab, tile size or instance set of an HNB_EFFECT_SLOT_ORDER batch) or because an HNB_EFFECT_SLOT_ORDER
  *  batch's states were 64 or more frames old (their words keep 6 bits of epoch). Batches of the other orders never add to it. */
 HNB_API int32_t hnb_ctx_tile_state_clears(hnb_ctx* ctx, uint64_t* clears);
+/** Number of modules the context compiled (or took from its module cache) for an effect bound to a slab whose column plan
+ *  is not the effect's own (section 3: a slab keeps the plan of the first effect bound to it). Each (effect, plan) pair counts
+ *  once. */
+HNB_API int32_t hnb_ctx_plan_compiles(hnb_ctx* ctx, uint64_t* compiles);
 /** Pinned host memory helpers for the async paths. */
 HNB_API void* hnb_host_alloc(size_t bytes);
 HNB_API void hnb_host_free(void* p);
