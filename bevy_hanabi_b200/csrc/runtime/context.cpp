@@ -18,6 +18,7 @@
 #include <string>
 #include <thread>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "../kernels/hnb_static_kernels.h"
@@ -250,7 +251,7 @@ struct hnb_ctx {
     bool param_upload = true; // HNB_PARAM_UPLOAD=0: always copy the frame block with the copy engine (never as a kernel parameter)
     unsigned long long* mailbox = nullptr;  // device alias of the caller's pinned count mailbox (hnb_ctx_set_count_mailbox)
     uint32_t mailbox_rows = 0, mailbox_ring = 0;
-    bool plan_dirty = false;  // plan_batch changed a tile-size or range word of the host frame block since the last upload
+    bool plan_dirty = false;  // bind_launch changed a tile-size or range word of the host frame block since the last upload
     uint64_t frame_copies = 0, frames = 0;  // hnb_simulate calls that needed the host->device copy of the frame block / all calls
     DeviceArray<unsigned long long> d_debug;  // 16 diagnostic counters + a 64-frame timeline ring of 4 words (HNB_PROFILE kernels)
 
@@ -500,82 +501,35 @@ KernelModule* module_for_plan(hnb_ctx* c, Effect& fx, const std::vector<Plane>& 
 struct LaunchPlan {
     Effect* fx;
     Slab* slab;
-    KernelModule* km;  // fx compiled for `target` (and the parent slab's plan)
-    // The plan the slab has, or will have once adopt_plans fixes it (the effect's own); then the parent slab, if any.
-    const std::vector<Plane>* target;
-    Slab* parent;
+    Slab* parent;      // the parent slab a child reads, or NULL
+    KernelModule* km;  // fx compiled for the slab's plan and the parent slab's (bind_launch)
     uint32_t batch;
-    uint32_t total_spawn;
+    uint32_t init_threads;
     hnb::BatchParams params;
     uint32_t init_blocks;
     uint32_t update_blocks;
 };
 
-void ensure_tile_state(hnb_ctx* c, uint32_t batch, uint32_t tiles) {
-    if (c->d_tile_state[batch].size() >= tiles) return;
-    CUDA_CHECK(grow(c->d_tile_state[batch], tiles + tiles / 2 + 64, 0, c->stream));
-    c->tile_state_slot[batch] = hnb_rt::TileStateSlot{};
-}
-
-// Build the kernel parameters of one batch and write its per-instance init thread ranges and tile
-// size into the host arena.
-LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
+// Every check of one launch; writes nothing, so a call can refuse a bad launch without side effects. Fills in what needs
+// no module: the effect, the slabs, the batch and the init threads.
+LaunchPlan check_launch(hnb_ctx* c, const hnb_batch_launch& bl) {
     LaunchPlan lp{};
     lp.fx = &get_effect(c, bl.effect);
     lp.slab = &get_slab(c, bl.slab);
-    if (lp.fx->particle_stride != lp.slab->stride) fail(HNB_ERR_LAYOUT, "effect particle stride does not match the slab");
-    if (((lp.fx->flags & HNB_EFFECT_SECTOR_PLANES) != 0) != lp.slab->sector_planes)
+    const Effect& fx = *lp.fx;
+    if (fx.particle_stride != lp.slab->stride) fail(HNB_ERR_LAYOUT, "effect particle stride does not match the slab");
+    if (((fx.flags & HNB_EFFECT_SECTOR_PLANES) != 0) != lp.slab->sector_planes)
         fail(HNB_ERR_LAYOUT, "effect and slab disagree on HNB_EFFECT_SECTOR_PLANES / HNB_SLAB_SECTOR_PLANES");
-    lp.target = lp.slab->plan_fixed ? &lp.slab->planes : &lp.fx->plan;  // nothing changes before the frame is validated
-    lp.parent = nullptr;
-    const std::vector<Plane>* parent_plan = nullptr;
     if (bl.parent_slab != 0xFFFFFFFFu) {
         lp.parent = &get_slab(c, bl.parent_slab);
         if (lp.parent->sector_planes) fail(HNB_ERR_LAYOUT, "a parent slab read by a child effect must not use sector planes");
-        // an unbound parent slab is in the default cut, and adopt_plans keeps it there
-        if (!is_default_cut(lp.parent->planes, lp.parent->stride)) parent_plan = &lp.parent->planes;
     }
-    lp.km = module_for_plan(c, *lp.fx, *lp.target, parent_plan);
     if (bl.batch_info_index >= c->B) fail(HNB_ERR_OUT_OF_RANGE, "batch_info_index out of range");
     lp.batch = bl.batch_info_index;
-    lp.total_spawn = bl.total_spawn_count;
     const hnb_batch_info& bi = c->h_at<hnb_batch_info>(c->lay.off_batch_infos)[lp.batch];
     if (uint64_t(bi.prefix_sum_offset) + bi.prefix_sum_count > c->E || uint64_t(bi.spawner_base) + bi.prefix_sum_count > c->E)
         fail(HNB_ERR_OUT_OF_RANGE, "batch references instances outside the uploaded spawner table");
-    // Rows per warp tile: 32 lanes x K rows per lane x chunks. Larger tiles shorten the look-back chain and
-    // amortise the per-tile work (ticket, state word, instance lookup); smaller tiles spread a small slab over more
-    // warps. With W = one sub-tile per resident warp (C5 on an H100: 3168 warps x 128 rows = 396 Ki rows):
-    //  * from 8 W up the launch streams at the HBM rate and the largest tile wins at every size;
-    //  * below, the launch is latency-bound and runs in ROUNDS: every resident warp takes one tile per round, and a tile
-    //    costs a fixed part (ticket, first alive-list entries, look-back, compaction) plus a part per sub-tile: pick the
-    //    chunk count that minimises rounds x (3.6 + chunks), preferring larger tiles on a tie. The constant was fitted on
-    //    an earlier GPU. On an H100 (tools/sweep_small.py, C5) the rule is within 3 % of the best forced chunk count from
-    //    1 Mi rows up; at 256-512 Ki rows forcing 3-4 chunks shortens the frame by 15-20 % (not retuned).
-    const uint32_t sub_tile = 32u * lp.fx->tile_k;
-    const uint32_t total_warps = uint32_t(lp.km->update_blocks_per_sm) * uint32_t(c->sm_count) * 8u;
-    const uint32_t max_chunks = std::max(1u, lp.fx->rows_per_lane / lp.fx->tile_k);
-    uint32_t chunks = c->tile_chunks_override;
-    if (chunks == 0) {
-        const uint64_t wave = uint64_t(total_warps) * sub_tile;
-        const uint64_t rows = lp.slab->capacity;
-        if (rows >= 8 * wave) {
-            chunks = max_chunks;
-        } else {
-            double best = 0.0;
-            for (uint32_t ch = 1; ch <= max_chunks; ++ch) {
-                const uint64_t tiles = (rows + uint64_t(sub_tile) * ch - 1) / (uint64_t(sub_tile) * ch) + bi.prefix_sum_count - 1;
-                const uint64_t rounds = std::max<uint64_t>(1, (tiles + total_warps - 1) / total_warps);
-                const double cost = double(rounds) * (3.6 + double(ch));
-                if (chunks == 0 || cost <= best) { best = cost; chunks = ch; }
-            }
-        }
-    }
-    chunks = std::max(1u, std::min(chunks, max_chunks));
-    const uint32_t tile = sub_tile * chunks;
-    // Tile size word shared with the bookkeeping kernels (hnb_tile_rows + flags)
-    const bool slot_order = (lp.fx->flags & HNB_EFFECT_SLOT_ORDER) != 0;
-    const uint32_t tile_word = tile | (slot_order ? HNB_TILE_SLOT_ORDER : 0u), small_tile = tile;
-    if (slot_order) {
+    if (fx.flags & HNB_EFFECT_SLOT_ORDER) {
         // bitmap words must belong to one instance (and one warp) each
         const hnb_spawner* sp = c->h_at<hnb_spawner>(c->lay.off_spawners);
         for (uint32_t i = 0; i < bi.prefix_sum_count; ++i)
@@ -583,31 +537,98 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
         // a slot-order state word packs each running count into 28 bits
         if (lp.slab->capacity >= (1u << 28)) fail(HNB_ERR_LAYOUT, "HNB_EFFECT_SLOT_ORDER needs a slab of fewer than 2^28 rows");
     }
-    if (c->h_at<uint32_t>(c->lay.off_tile_size)[lp.batch] != tile_word) {
-        c->h_at<uint32_t>(c->lay.off_tile_size)[lp.batch] = tile_word;
-        c->plan_dirty = true;
-    }
-
-    const bool consume = (lp.fx->flags & HNB_EFFECT_CONSUME_GPU_SPAWN_EVENTS) != 0;
-    uint32_t init_threads = 0;
-    if (consume) {
+    if (fx.flags & HNB_EFFECT_CONSUME_GPU_SPAWN_EVENTS) {
         if (bl.consume_events >= c->event_buffers.size()) fail(HNB_ERR_INVALID_ARG, "event-driven effect needs a consume_events buffer");
         // One logical init thread per event-buffer ENTRY, not per 64-thread workgroup of the reference's dispatch: the
         // threads of the last partial workgroup would read past the buffer when a parent over-emits (event_count is
         // unclamped, lib.rs:976-993), which WGSL's robust buffer access forgives and raw CUDA does not. The init
         // accounting in the bookkeeping kernel uses the same bound (range = capacity).
-        init_threads = uint32_t(c->event_buffers[bl.consume_events].size());
+        lp.init_threads = uint32_t(c->event_buffers[bl.consume_events].size());
     } else {
-        init_threads = ceil_div(lp.total_spawn, 64) * 64;  // dispatch_workgroups(ceil(n/64)), mod.rs:7157-7173
+        lp.init_threads = ceil_div(bl.total_spawn_count, 64) * 64;  // dispatch_workgroups(ceil(n/64)), mod.rs:7157-7173
     }
+    for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i)
+        if (bl.emit_events[i] != 0xFFFFFFFFu && bl.emit_events[i] >= c->event_buffers.size()) fail(HNB_ERR_INVALID_ARG, "invalid emit event buffer");
+    if ((fx.flags & HNB_EFFECT_ORDERED_EVENTS) && (fx.flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS) && bi.prefix_sum_count != 1)
+        fail(HNB_ERR_INVALID_ARG, "HNB_EFFECT_ORDERED_EVENTS needs a batch of exactly one instance");
+    if (fx.props_size && !fx.d_props) fail(HNB_ERR_NOT_READY, "effect uses properties but none were uploaded");
+    lp.init_blocks = ceil_div(lp.init_threads, 256 * hnb_rt::kInitItems);  // HNB_INIT_ITEMS logical init threads per CUDA thread
+    return lp;
+}
+
+// The first bind of a slab fixes its plan (fix_plan) to the launch's effect's own; an unbound parent slab read by a child
+// keeps the default cut. Launch order decides when two effects of different plans bind one fresh slab in one call.
+void fix_launch_plans(hnb_ctx* c, const LaunchPlan& lp) {
+    fix_plan(c, *lp.slab, lp.fx->plan);
+    if (lp.parent) fix_default_plan(c, *lp.parent);
+}
+
+// Sub-tiles per update tile (`forced`: HNB_TILE_CHUNKS, 0 = by slab size) for `rows` slab rows in `instances` instances.
+// Rows per warp tile: 32 lanes x K rows per lane x chunks. Larger tiles shorten the look-back chain and amortise the
+// per-tile work (ticket, state word, instance lookup); smaller tiles spread a small slab over more warps. With W = one
+// sub-tile per resident warp (C5 on an H100: 3168 warps x 128 rows = 396 Ki rows):
+//  * from 8 W up the launch streams at the HBM rate and the largest tile wins at every size;
+//  * below, the launch is latency-bound and runs in ROUNDS: every resident warp takes one tile per round, and a tile
+//    costs a fixed part (ticket, first alive-list entries, look-back, compaction) plus a part per sub-tile: pick the
+//    chunk count that minimises rounds x (3.6 + chunks), preferring larger tiles on a tie. The constant was fitted on
+//    an earlier GPU. On an H100 (tools/sweep_small.py, C5) the rule is within 3 % of the best forced chunk count from
+//    1 Mi rows up; at 256-512 Ki rows forcing 3-4 chunks shortens the frame by 15-20 % (not retuned).
+uint32_t tile_chunks(uint32_t forced, uint64_t rows, uint32_t instances, uint32_t sub_tile, uint32_t total_warps, uint32_t max_chunks) {
+    uint32_t chunks = forced;
+    if (chunks == 0) {
+        const uint64_t wave = uint64_t(total_warps) * sub_tile;
+        if (rows >= 8 * wave) {
+            chunks = max_chunks;
+        } else {
+            double best = 0.0;
+            for (uint32_t ch = 1; ch <= max_chunks; ++ch) {
+                const uint64_t tiles = (rows + uint64_t(sub_tile) * ch - 1) / (uint64_t(sub_tile) * ch) + instances - 1;
+                const uint64_t rounds = std::max<uint64_t>(1, (tiles + total_warps - 1) / total_warps);
+                const double cost = double(rounds) * (3.6 + double(ch));
+                if (chunks == 0 || cost <= best) { best = cost; chunks = ch; }
+            }
+        }
+    }
+    return std::max(1u, std::min(chunks, max_chunks));
+}
+
+void ensure_tile_state(hnb_ctx* c, uint32_t batch, uint32_t tiles) {
+    if (c->d_tile_state[batch].size() >= tiles) return;
+    CUDA_CHECK(grow(c->d_tile_state[batch], tiles + tiles / 2 + 64, 0, c->stream));
+    c->tile_state_slot[batch] = hnb_rt::TileStateSlot{};
+}
+
+// Binds a checked launch once the plans of its slabs are fixed (fix_launch_plans): picks the module for those plans and the
+// tile size, writes the tile size and (`set_ranges`) the per-instance init thread ranges into the host frame block,
+// readies the batch's tile states and ordered-event scratch, and builds the kernel parameters.
+void bind_launch(hnb_ctx* c, LaunchPlan& lp, const hnb_batch_launch& bl, bool set_ranges) {
+    const Effect& fx = *lp.fx;
+    Slab& slab = *lp.slab;
+    const hnb_batch_info& bi = c->h_at<hnb_batch_info>(c->lay.off_batch_infos)[lp.batch];
+    const std::vector<Plane>* parent_plan = nullptr;  // a parent slab in the default cut needs no module of its own
+    if (lp.parent && !is_default_cut(lp.parent->planes, lp.parent->stride)) parent_plan = &lp.parent->planes;
+    lp.km = module_for_plan(c, *lp.fx, slab.planes, parent_plan);
+
+    const uint32_t sub_tile = 32u * fx.tile_k;
+    const uint32_t total_warps = uint32_t(lp.km->update_blocks_per_sm) * uint32_t(c->sm_count) * 8u;
+    const uint32_t tile = sub_tile * tile_chunks(c->tile_chunks_override, slab.capacity, bi.prefix_sum_count, sub_tile, total_warps,
+                                                 std::max(1u, fx.rows_per_lane / fx.tile_k));
+    // Tile size word shared with the bookkeeping kernels (hnb_tile_rows + flags)
+    const bool slot_order = (fx.flags & HNB_EFFECT_SLOT_ORDER) != 0;
+    const uint32_t tile_word = tile | (slot_order ? HNB_TILE_SLOT_ORDER : 0u);
+    if (c->h_at<uint32_t>(c->lay.off_tile_size)[lp.batch] != tile_word) {
+        c->h_at<uint32_t>(c->lay.off_tile_size)[lp.batch] = tile_word;
+        c->plan_dirty = true;
+    }
+    const bool consume = (fx.flags & HNB_EFFECT_CONSUME_GPU_SPAWN_EVENTS) != 0;
     if (set_ranges) {
         uint32_t* range = c->h_at<uint32_t>(c->lay.off_range);
         const uint32_t* sp = c->h_at<uint32_t>(c->lay.off_spawn_prefix);
         for (uint32_t i = 0; i < bi.prefix_sum_count; ++i) {
             uint32_t g = bi.prefix_sum_offset + i;
             uint32_t r = 0;
-            if (init_threads) {
-                uint32_t end = (i + 1 < bi.prefix_sum_count) ? sp[g + 1] : init_threads;
+            if (lp.init_threads) {
+                uint32_t end = (i + 1 < bi.prefix_sum_count) ? sp[g + 1] : lp.init_threads;
                 r = end > sp[g] ? end - sp[g] : 0;
                 if (consume && r) r |= 0x80000000u;
             }
@@ -619,7 +640,8 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
             if (r) c->plan_dirty = true;
         }
     }
-    ensure_tile_state(c, lp.batch, lp.slab->capacity / small_tile + bi.prefix_sum_count + 1);  // ceil(rows_i / tile) summed over the instances
+    const uint32_t max_tiles = slab.capacity / tile + bi.prefix_sum_count + 1;  // ceil(rows_i / tile) summed over the instances
+    ensure_tile_state(c, lp.batch, max_tiles);
     {
         // Slot-order state words carry only 6 bits of epoch: the array is zeroed when the slot's use changes (signature)
         // and at least every 64 frames of the slot (tile_state_rule.h). The signature alone is not enough: a batch slot
@@ -651,29 +673,26 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
     P.metadata = c->d_metadata.get();
     P.draw_args = c->draw_args();
     P.child_infos = c->d_child_infos.get();
-    P.properties = lp.fx->d_props.get();
-    P.properties_stride = lp.fx->props_stride;
-    P.slab = slab_view(*lp.slab);
+    P.properties = fx.d_props.get();
+    P.properties_stride = fx.props_stride;
+    P.slab = slab_view(slab);
     if (lp.parent) P.parent_slab = slab_view(*lp.parent);
     if (consume) P.consume_events = c->event_buffers[bl.consume_events].get();
     for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
-        if (bl.emit_events[i] != 0xFFFFFFFFu) {
-            if (bl.emit_events[i] >= c->event_buffers.size()) fail(HNB_ERR_INVALID_ARG, "invalid emit event buffer");
-            P.emit_events[i] = c->event_buffers[bl.emit_events[i]].get();
-            P.emit_events_capacity[i] = uint32_t(c->event_buffers[bl.emit_events[i]].size());
-        }
+        if (bl.emit_events[i] == 0xFFFFFFFFu) continue;
+        P.emit_events[i] = c->event_buffers[bl.emit_events[i]].get();
+        P.emit_events_capacity[i] = uint32_t(c->event_buffers[bl.emit_events[i]].size());
     }
-    if ((lp.fx->flags & HNB_EFFECT_ORDERED_EVENTS) && (lp.fx->flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS)) {
-        if (bi.prefix_sum_count != 1) fail(HNB_ERR_INVALID_ARG, "HNB_EFFECT_ORDERED_EVENTS needs a batch of exactly one instance");
+    if ((fx.flags & HNB_EFFECT_ORDERED_EVENTS) && (fx.flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS)) {
         for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
             if (!P.emit_events[i]) continue;
             // each allocated when missing: a frame that failed between the two allocations is completed by the next
-            if (!lp.slab->event_counts[i]) CUDA_CHECK(lp.slab->event_counts[i].alloc(lp.slab->capacity));
-            if (!lp.slab->event_block_sums[i]) CUDA_CHECK(lp.slab->event_block_sums[i].alloc(hnb::ordered_event_blocks(lp.slab->capacity) + 1));
-            P.event_counts[i] = lp.slab->event_counts[i].get();
+            if (!slab.event_counts[i]) CUDA_CHECK(slab.event_counts[i].alloc(slab.capacity));
+            if (!slab.event_block_sums[i]) CUDA_CHECK(slab.event_block_sums[i].alloc(hnb::ordered_event_blocks(slab.capacity) + 1));
+            P.event_counts[i] = slab.event_counts[i].get();
         }
     }
-    P.init_thread_count = init_threads;
+    P.init_thread_count = lp.init_threads;
     P.debug = c->d_debug.get();
     P.bi_spawner_base = bi.spawner_base;
     P.bi_prefix_sum_offset = bi.prefix_sum_offset;
@@ -683,29 +702,16 @@ LaunchPlan plan_batch(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
     P.mailbox_rows = c->mailbox_rows;
     P.mailbox_ring = c->mailbox_ring;
     P.tile_rows = tile_word;
-    lp.init_blocks = ceil_div(init_threads, 256 * hnb_rt::kInitItems);  // HNB_INIT_ITEMS logical init threads per CUDA thread
-    uint32_t max_tiles = lp.slab->capacity / small_tile + bi.prefix_sum_count + 1;
-    lp.update_blocks = std::min<uint32_t>(ceil_div(max_tiles, 8), uint32_t(lp.km->update_blocks_per_sm) * uint32_t(c->sm_count));
-    if (lp.update_blocks == 0) lp.update_blocks = 1;
-    if (lp.fx->props_size && !lp.fx->d_props) fail(HNB_ERR_NOT_READY, "effect uses properties but none were uploaded");
-    return lp;
+    lp.update_blocks = std::max(1u, std::min<uint32_t>(ceil_div(max_tiles, 8), uint32_t(lp.km->update_blocks_per_sm) * uint32_t(c->sm_count)));
 }
 
-// After every launch of a call has been planned and validated: the first bind of a slab fixes its plan (fix_plan; an
-// unbound parent slab keeps the default cut), which may move its records, so the launch parameters take the columns
-// again. A launch whose slab ended in another plan than it was planned for (two effects of different plans binding one
-// fresh slab in one frame, or no memory for the move) is planned again.
-void adopt_plans(hnb_ctx* c, LaunchPlan* plans, const hnb_batch_launch* batches, uint32_t n, bool set_ranges) {
-    for (uint32_t i = 0; i < n; ++i) {
-        fix_plan(c, *plans[i].slab, *plans[i].target);
-        if (plans[i].parent) fix_default_plan(c, *plans[i].parent);
-    }
-    for (uint32_t i = 0; i < n; ++i) {
-        LaunchPlan& lp = plans[i];
-        if (lp.slab->planes != *lp.target) lp = plan_batch(c, batches[i], set_ranges);
-        lp.params.slab = slab_view(*lp.slab);
-        if (lp.parent) lp.params.parent_slab = slab_view(*lp.parent);
-    }
+// A stand-alone pass's one launch: checked, then bound.
+LaunchPlan check_and_bind(hnb_ctx* c, const hnb_batch_launch& bl, bool set_ranges) {
+    LaunchPlan lp = check_launch(c, bl);
+    ensure_scratch(c);
+    fix_launch_plans(c, lp);
+    bind_launch(c, lp, bl, set_ranges);
+    return lp;
 }
 
 // hnb_init / hnb_update start with griddepcontrol.wait, so they may always be launched with programmatic stream
@@ -848,6 +854,39 @@ void check_coverage(hnb_ctx* c, const std::vector<LaunchPlan>& plans) {
     }
     for (uint32_t b = 0; b < c->B; ++b)
         if (!seen[b]) fail(HNB_ERR_NOT_READY, "every uploaded batch must be launched by hnb_simulate");
+}
+
+// The frame block reaches the device with ONE copy — or with none: when no table row, tile size or init range changed
+// since the last upload (a steady-state frame without spawns), the only new bytes are the 64-byte header (sim params,
+// epoch), and those ride in the bookkeeping kernel's parameter space. The frame is then a pure kernel chain, which
+// programmatic dependent launch pipelines against the previous frame.
+// ... or, third way, with the bookkeeping LAUNCH: when the frame has no init pass (nothing reads the tables before the
+// bookkeeping kernel) and the host-written part of the arena fits the kernel parameter space, it travels there and CTA 0
+// stores it into the device arena. A copy-engine operation between two kernels of the chain costs its own latency and the
+// programmatic overlap of the kernel behind it, every frame of a host that rewrites its tables every frame. With an init
+// pass the block needs a (one-CTA) kernel of its own at the head of the frame: init reads the tables first.
+// Returns what the bookkeeping launch carries in its parameter space: the header alone, header + tables, or nothing.
+std::pair<const void*, uint32_t> send_frame_block(hnb_ctx* c, std::vector<LaunchPlan>& plans) {
+    std::pair<const void*, uint32_t> carried{c->header(), uint32_t(sizeof(hnb::FrameHeader))};
+    if (c->dirty_tables || c->plan_dirty) {
+        const uint32_t bytes = uint32_t(c->lay.off_prefix_sum);
+        if (!c->param_upload || c->B == 0 || bytes > HNB_FRAME_BLOCK_MAX_BYTES) {
+            flush_arena(c, true);
+            c->frame_copies++;
+            carried = {nullptr, 0};
+        } else if (std::none_of(plans.begin(), plans.end(), [](const LaunchPlan& lp) { return lp.init_blocks != 0; })) {
+            carried = {c->h_arena.get(), bytes};
+        } else {
+            CUDA_CHECK(hnb::launch_frame_block(c->d_arena.get(), c->h_arena.get(), bytes, c->stream));
+            c->launches++;
+            for (auto& lp : plans) lp.params.late_tables = 1u;
+            carried = {nullptr, 0};
+        }
+        c->dirty_tables = false;
+        c->plan_dirty = false;
+    }
+    c->frames++;
+    return carried;
 }
 
 }  // namespace
@@ -1611,37 +1650,17 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
         if (n && !batches) fail(HNB_ERR_INVALID_ARG, "batches is NULL");
         CUDA_CHECK(cudaSetDevice(c->device));
         if (c->header()->sim.num_effects > c->E) fail(HNB_ERR_NOT_READY, "sim_params.num_effects exceeds the uploaded spawner table");
-        ensure_scratch(c);
+        // Every launch is checked before anything is written or enqueued: a bad frame is skipped as a whole.
         std::vector<LaunchPlan>& plans = c->frame_plans;  // reused from frame to frame: no allocation in steady state
         plans.clear();
         plans.reserve(n);
-        for (uint32_t i = 0; i < n; ++i) plans.push_back(plan_batch(c, batches[i], true));
-        check_coverage(c, plans);  // nothing has been enqueued yet: a bad frame is skipped as a whole
-        adopt_plans(c, plans.data(), batches, n, true);
+        for (uint32_t i = 0; i < n; ++i) plans.push_back(check_launch(c, batches[i]));
+        check_coverage(c, plans);
+        ensure_scratch(c);
+        for (const auto& lp : plans) fix_launch_plans(c, lp);
+        for (uint32_t i = 0; i < n; ++i) bind_launch(c, plans[i], batches[i], true);
         next_epoch(c);
-        // The frame block reaches the device with ONE copy — or with none: when no table row, tile size or init range
-        // changed since the last upload (a steady-state frame without spawns), the only new bytes are the 64-byte
-        // header (sim params, epoch), and those ride in the bookkeeping kernel's parameter space. The frame is then
-        // a pure kernel chain, which programmatic dependent launch pipelines against the previous frame.
-        // ... or, third way, with the bookkeeping LAUNCH: when the frame has no init pass (nothing reads the tables before the
-        // bookkeeping kernel) and the host-written part of the arena fits the kernel parameter space, it travels there and CTA 0
-        // stores it into the device arena. A copy-engine operation between two kernels of the chain costs its own latency and
-        // the programmatic overlap of the kernel behind it, every frame of a host that rewrites its tables every frame.
-        const bool copy_block = c->dirty_tables || c->plan_dirty;
-        bool any_init = false;
-        for (auto& lp : plans) any_init |= lp.init_blocks != 0;
-        const bool param_block = copy_block && c->param_upload && c->B > 0 && c->lay.off_prefix_sum <= HNB_FRAME_BLOCK_MAX_BYTES;
-        // with an init pass the block needs a (one-CTA) kernel of its own at the head of the frame: init reads the tables first
-        const bool block_kernel = param_block && any_init;
-        if (block_kernel) {
-            CUDA_CHECK(hnb::launch_frame_block(c->d_arena.get(), c->h_arena.get(), uint32_t(c->lay.off_prefix_sum), c->stream));
-            c->launches++;
-            for (auto& lp : plans) lp.params.late_tables = 1u;
-        }
-        if (copy_block && !param_block) flush_arena(c, true);
-        if (block_kernel) { c->dirty_tables = false; c->plan_dirty = false; }  // (stored by k_frame_block, enqueued above)
-        c->frames++;
-        c->frame_copies += (copy_block && !param_block) ? 1 : 0;
+        const auto [block, block_bytes] = send_frame_block(c, plans);
         // pass "hanabi:init" (mod.rs:7025-7179). Batches write disjoint slab rows and table rows; the only
         // cross-batch access is a child reading its parent's records, so frames with event-driven children keep
         // the reference's serial order.
@@ -1662,13 +1681,7 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
         // passes "hanabi:indirect_dispatch" + "hanabi:update_prefix_sum" (mod.rs:7182-7275), fused
         {
             PassRange range("hanabi:indirect_dispatch");  // + "hanabi:update_prefix_sum"
-            const void* block = nullptr;   // what rides in the kernel's parameter space: nothing / the 64-byte header / header + tables
-            uint32_t block_bytes = 0;
-            if (param_block && !block_kernel) { block = c->h_arena.get(); block_bytes = uint32_t(c->lay.off_prefix_sum); }
-            else if (block_kernel) { /* already stored by k_frame_block, header included */ }
-            else if (!copy_block) { block = c->header(); block_bytes = uint32_t(sizeof(hnb::FrameHeader)); }
             CUDA_CHECK(hnb::launch_bookkeeping(static_tables(c), c->header()->sim.num_effects, c->B, block, block_bytes, c->stream));
-            if (param_block && !block_kernel) { c->dirty_tables = false; c->plan_dirty = false; }  // the tables went with this launch
             c->launches += 1 + (c->d_child_infos.size() ? 1 : 0);
             std::fill(c->init_pending.begin(), c->init_pending.end(), 0);
         }
@@ -1685,8 +1698,7 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
         for (auto& lp : plans) {
             if (!(lp.fx->flags & HNB_EFFECT_ORDERED_EVENTS) || !(lp.fx->flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS)) continue;
             const hnb_batch_info& bi = c->h_at<hnb_batch_info>(c->lay.off_batch_infos)[lp.batch];
-            const hnb_spawner& sp = c->h_at<hnb_spawner>(c->lay.off_spawners)[bi.spawner_base];
-            if (sp.effect_metadata_index >= c->d_metadata.size()) fail(HNB_ERR_OUT_OF_RANGE, "spawner row points outside the metadata table");
+            const hnb_spawner& sp = c->h_at<hnb_spawner>(c->lay.off_spawners)[bi.spawner_base];  // row checked by check_coverage
             for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
                 if (!lp.params.event_counts[i]) continue;
                 hnb::EventAppendArgs a{};
@@ -1721,9 +1733,7 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
 int32_t hnb_pass_sort(hnb_ctx* c, const hnb_batch_launch* b) {
     return guarded([&] {
         if (!b) fail(HNB_ERR_INVALID_ARG, "batch is NULL");
-        ensure_scratch(c);
-        LaunchPlan lp = plan_batch(c, *b, false);
-        adopt_plans(c, &lp, b, 1, false);
+        LaunchPlan lp = check_and_bind(c, *b, false);
         flush_arena(c, false);
         launch_ribbon_sort(c, lp);
     });
@@ -1732,15 +1742,13 @@ int32_t hnb_pass_sort(hnb_ctx* c, const hnb_batch_launch* b) {
 int32_t hnb_pass_init(hnb_ctx* c, const hnb_batch_launch* b) {
     return guarded([&] {
         if (!b) fail(HNB_ERR_INVALID_ARG, "batch is NULL");
-        ensure_scratch(c);
         // The init kernel pops dead slots by rank from the counters as they stood at the START of the pass, and its
         // alive_count / particle_counter increments are applied by the indirect pass that follows (spawn_range[]): a
         // second stand-alone init of the same batch before that pass would pop the same slots and lose the first
         // launch's increments (the reference's atomics accumulate, vfx_init.wgsl:141-151). Refuse it.
         if (b->batch_info_index < c->init_pending.size() && c->init_pending[b->batch_info_index])
             fail(HNB_ERR_INVALID_ARG, "hnb_pass_init: this batch already has an init pass pending; run hnb_pass_indirect first");
-        LaunchPlan lp = plan_batch(c, *b, true);
-        adopt_plans(c, &lp, b, 1, true);
+        LaunchPlan lp = check_and_bind(c, *b, true);
         c->header()->num_batches = c->B;
         if (c->header()->epoch == 0) next_epoch(c);
         flush_arena(c, true);
@@ -1783,9 +1791,7 @@ int32_t hnb_pass_prefix_sum(hnb_ctx* c) {
 int32_t hnb_pass_update(hnb_ctx* c, const hnb_batch_launch* b) {
     return guarded([&] {
         if (!b) fail(HNB_ERR_INVALID_ARG, "batch is NULL");
-        ensure_scratch(c);
-        LaunchPlan lp = plan_batch(c, *b, false);
-        adopt_plans(c, &lp, b, 1, false);
+        LaunchPlan lp = check_and_bind(c, *b, false);
         next_epoch(c);
         flush_arena(c, false);
         CUDA_CHECK(hnb::launch_tile_prefix(static_tables(c), lp.batch, lp.params.tile_rows, c->stream));
@@ -1859,7 +1865,7 @@ int32_t hnb_read_tile_size(hnb_ctx* c, uint32_t row, uint32_t* out) {
     return guarded([&] {
         if (!out) fail(HNB_ERR_INVALID_ARG, "NULL argument");
         if (row >= c->B) fail(HNB_ERR_OUT_OF_RANGE, "batch row out of range");
-        *out = c->h_at<uint32_t>(c->lay.off_tile_size)[row];  // host copy of the word plan_batch passed to the batch's last launch
+        *out = c->h_at<uint32_t>(c->lay.off_tile_size)[row];  // host copy of the word bind_launch passed to the batch's last launch
     });
 }
 

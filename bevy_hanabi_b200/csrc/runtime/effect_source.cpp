@@ -339,7 +339,7 @@ std::string generate_effect_source(const hnb_effect_desc& d, const std::vector<P
             std::string item = e.substr(pos, end - pos);
             size_t eq = item.find('=');
             // The host sizes the dynamic shared memory and the grid from its own copy of these (update_smem_bytes,
-            // plan_batch): overriding them here would make the kernel's carve-up disagree with the launch. Ignored, loudly.
+            // bind_launch): overriding them here would make the kernel's carve-up disagree with the launch. Ignored, loudly.
             static const char* const kHostMirrored[] = {"HNB_SMEM_EFFECTS", "HNB_BLOCK", "HNB_WARPS", "HNB_ROWS_PER_LANE", "HNB_TILE_K",
                                                         "HNB_NUM_PLANES", "HNB_INIT_ITEMS", "HNB_MAX_CHUNKS", "HNB_INIT_SMEM_EFFECTS"};
             const std::string name = item.substr(0, eq);

@@ -30,7 +30,7 @@ inline uint32_t tile_state_run_epoch(uint32_t epoch) {
 }
 
 // Called for every planned run of a batch slot. `sig` describes what the run uses the slot for (nonzero for slot order,
-// see plan_batch; 0 for the other orders) and `run_epoch` is the run's epoch. Returns true when the slot's array must be
+// see bind_launch; 0 for the other orders) and `run_epoch` is the run's epoch. Returns true when the slot's array must be
 // zeroed before the run, and updates `s`.
 //  * A change of signature zeroes the array (another effect, slab, tile size or instance set).
 //  * Slot order zeroes it when the run is 64 or more epochs after the first run since the last zeroing.

@@ -20,7 +20,7 @@ SUB_TILE_C5 = 128  # rows of an update sub-tile for C5 records: 32 lanes x K = 4
 @pytest.fixture(params=[1, 2, 3, 4], ids=lambda n: f"{n}sub")
 def tiled_ctx(request, native, monkeypatch):
     """A fresh context on cuda:0 whose update tiles hold `tile_chunks` sub-tiles, forced with HNB_TILE_CHUNKS (None: the
-    slab-size rule of plan_batch, which picks 1 below one wave of resident warps, about 400 Ki rows for C5, so without the
+    slab-size rule of tile_chunks, which picks 1 below one wave of resident warps, about 400 Ki rows for C5, so without the
     override almost every row-exact test would run 1). The results are the same at every tile size by design, so after a
     forced run the fixture reads back the tile size of the last launch of batch `tile_batch` (default 0; its effect must
     have records of at most 36 bytes, as C5's, for 128-row sub-tiles) to prove that the size under test was the one that

@@ -372,7 +372,7 @@ class EmuWorld:
             per_block = 256 * self.lib.emu_init_items()
             self.lib.emu_init(C.byref(self.b), (threads + per_block - 1) // per_block)
         if self.static_lib is not None:
-            # ---- bookkeeping by the real fused kernel (k_bookkeeping): per-instance init thread ranges as plan_batch writes them
+            # ---- bookkeeping by the real fused kernel (k_bookkeeping): per-instance init thread ranges as bind_launch writes them
             for i in range(n):
                 end = int(self.spawn_prefix[i + 1]) if i + 1 < n else threads
                 self.spawn_range[i] = max(0, end - int(self.spawn_prefix[i])) if threads else 0

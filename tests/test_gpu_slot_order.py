@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 
 @at_tile_sizes("capacity,alive", [(8192, 5000), (8192, 8192), (8192, 1), (70, 70), (33, 0), (400_000, 380_000), (2_200_000, 2_000_001)])
 def test_c5_with_deaths(tiled_ctx, orc, capacity, alive):
-    """The sub-tile counts plan_batch picks (1 up to 8192 rows, more at 400 K and 2.2 M), then 2, 3 and 4 forced at every size
+    """The sub-tile counts tile_chunks picks (1 up to 8192 rows, more at 400 K and 2.2 M), then 2, 3 and 4 forced at every size
     (the bitmap words a warp owns: chunks x K of them), capacities that are no multiple of 32 or of the tile."""
     rng = np.random.default_rng(capacity + alive)
     ref = RefWorld(capacity, 8, [Instance(0, capacity, alive=alive, seed=42)])

@@ -5,7 +5,7 @@ published this frame when its epoch tag equals the frame's (`hnb_state_flag`). S
 default-order words 30 (relaxed order runs no look-back). So a word written 64 frames earlier, or any multiple, passes
 for current in slot order whenever the tile that wrote it was not rewritten since: the batch slot sat out, or served
 another instance with fewer tiles. The host zeroes an array before such a run (bevy_hanabi_b200/csrc/runtime/
-tile_state_rule.h, called by plan_batch).
+tile_state_rule.h, called by bind_launch).
 
 This model keeps one persistent state array per batch slot across frames, with per-frame geometry, and runs:
   * the real state words: `hnb_pack_state` / `hnb_state_flag` of the kernel header, from the g++ build tests/kernel_emu.py
@@ -79,7 +79,7 @@ def words():
 
 
 class RealRule:
-    """plan_batch's decision through the compiled header."""
+    """bind_launch's decision through the compiled header."""
 
     def __init__(self, lib):
         self.lib = lib
@@ -130,11 +130,11 @@ class Context:
         self.writer[slot][:] = [None] * self.cap
 
     def frame(self, batches, schedule="adversarial"):
-        """batches: [(slot, use)], use = dict(order="slot"|"default", sig=<what plan_batch hashes>, alive=[[per-tile survivors]
+        """batches: [(slot, use)], use = dict(order="slot"|"default", sig=<what bind_launch hashes>, alive=[[per-tile survivors]
         per instance], valid=[[per-tile valid rows]]). Returns {slot: [exclusive prefix per tile]}."""
         self.frame_no += 1
         run = self.rule.run_epoch(self.epoch)
-        for slot, use in batches:                             # plan_batch, before next_epoch
+        for slot, use in batches:                             # bind_launch, before next_epoch
             self._array(slot)
             sig = use["sig"] if use["order"] == "slot" else 0
             if self.rule.needs_clear(slot, sig, run):
