@@ -557,39 +557,53 @@ __device__ __forceinline__ void snapshot_column(const SnapshotArgs& a, u32 p, co
     }
 }
 
+// D of an emitting instance: the slots its last update freed sit at dead-stack positions n .. n+D of its slice
+// (deaths are pushed to dead[max_update-1-rank]), and a pending OnDie event may name any of them.
+__device__ __forceinline__ u32 last_dead_count(const EffectMetadata* md, u32 n, u32 rows) {
+    const u32 updated = md->max_update;
+    return updated > n ? min(updated - n, rows - n) : 0u;
+}
+
 // Header by the first 16 threads, then record i < n = min(alive_count, rows) from local row list_W[i] (clamped to the
-// slice as repack_source clamps it). Reads nothing but the metadata row, column W and the planes.
-__global__ void __launch_bounds__(RP_THREADS) k_snapshot_gather(SnapshotArgs a, u32* dst) {
+// slice as repack_source clamps it). Reads nothing but the metadata row, column W and the planes. DEAD (version 2): the
+// header names version 2 and D in word 6, and records n .. n+D come from local rows dead[first+i] - first.
+template <bool DEAD>
+__device__ __forceinline__ void snapshot_gather(const SnapshotArgs& a, const u32* dead, u32* dst) {
     const EffectMetadata* md = a.metadata;
     const u32 n = min(md->alive_count, a.rows);
+    const u32 d = DEAD ? last_dead_count(md, n, a.rows) : 0u;
     if (blockIdx.x == 0u && threadIdx.x < HNB_SNAPSHOT_HEADER_WORDS) {
         const u32 t = threadIdx.x;
         dst[t] = t == 0u ? HNB_SNAPSHOT_MAGIC_WORD
-               : t == 1u ? HNB_SNAPSHOT_VERSION_WORD
+               : t == 1u ? (DEAD ? HNB_SNAPSHOT_EVENTS_VERSION_WORD : HNB_SNAPSHOT_VERSION_WORD)
                : t == 2u ? a.stride_words * 4u
                : t == 3u ? n
                : t == 4u ? md->particle_counter
                : t == 5u ? a.rows
+               : t == 6u ? d
                : 0u;
     }
     const u32* list = md->indirect_write_index == 0u ? a.ping : a.pong;
     const u32 i0 = blockIdx.x * RP_ROWS_PER_BLOCK + threadIdx.x;
-    if (i0 >= n) return;
+    if (i0 >= n + d) return;
     u32 src[RP_ITEMS];
 #pragma unroll
     for (u32 k = 0; k < RP_ITEMS; ++k) {
         const u32 i = i0 + k * RP_THREADS;
-        src[k] = i < n ? min(list[a.first + i], a.rows - 1u) : 0u;
+        src[k] = i < n ? min(list[a.first + i], a.rows - 1u) : (DEAD && i < n + d) ? min(dead[a.first + i] - a.first, a.rows - 1u) : 0u;
     }
     for (u32 p = 0; p < a.num_planes; ++p) {
         switch (a.planes.words[p]) {
-        case 1: snapshot_column<1>(a, p, src, i0, n, dst); break;
-        case 2: snapshot_column<2>(a, p, src, i0, n, dst); break;
-        case 4: snapshot_column<4>(a, p, src, i0, n, dst); break;
-        default: snapshot_column<8>(a, p, src, i0, n, dst); break;
+        case 1: snapshot_column<1>(a, p, src, i0, n + d, dst); break;
+        case 2: snapshot_column<2>(a, p, src, i0, n + d, dst); break;
+        case 4: snapshot_column<4>(a, p, src, i0, n + d, dst); break;
+        default: snapshot_column<8>(a, p, src, i0, n + d, dst); break;
         }
     }
 }
+__global__ void __launch_bounds__(RP_THREADS) k_snapshot_gather(SnapshotArgs a, u32* dst) { snapshot_gather<false>(a, nullptr, dst); }
+// version 2: words 7-15 of the header and the events follow from k_events_translate
+__global__ void __launch_bounds__(RP_THREADS) k_snapshot_gather_dead(SnapshotArgs a, const u32* dead, u32* dst) { snapshot_gather<true>(a, dead, dst); }
 
 // m = min(count, rows, records the buffer holds); 0 for a header that is not a version-1 snapshot of this stride
 __device__ __forceinline__ u32 restore_count(const SnapshotArgs& a, const u32* src) {
@@ -599,46 +613,139 @@ __device__ __forceinline__ u32 restore_count(const SnapshotArgs& a, const u32* s
     return u32(m < fit ? m : fit);
 }
 
+// What a restore takes from a version-2 snapshot: live records [0, m) to rows [0, m) and dead records [n, n+dm) to rows
+// [m, m+dm), with m = min(n, rows, records the buffer holds) and dm = min(D, rows - m, dead records the buffer holds).
+// All zero for a header that is not a version-2 snapshot of this stride with `channels` event channels.
+struct RestoreSpan {
+    u32 n, d, m, dm;
+    bool ok;
+};
+__device__ __forceinline__ RestoreSpan restore_span(const SnapshotArgs& a, const u32* src, u32 channels) {
+    RestoreSpan s{0u, 0u, 0u, 0u, false};
+    if (src[0] != HNB_SNAPSHOT_MAGIC_WORD || src[1] != HNB_SNAPSHOT_EVENTS_VERSION_WORD || src[2] != a.stride_words * 4u ||
+        src[7] != channels)
+        return s;
+    s.ok = true;
+    s.n = src[3];
+    s.d = src[6];
+    const u64 fit = (a.src_bytes - HNB_SNAPSHOT_HEADER_WORDS * 4u) / (a.stride_words * 4u);
+    const u64 m = s.n < a.rows ? s.n : a.rows;
+    s.m = u32(m < fit ? m : fit);
+    const u64 dead_fit = fit > s.n ? fit - s.n : 0u;
+    const u64 dm = s.d < a.rows - s.m ? s.d : a.rows - s.m;
+    s.dm = u32(dm < dead_fit ? dm : dead_fit);
+    return s;
+}
+
+// rows i0 + k * RP_THREADS < m + dm of column p from records i (i < m) and n + i - m (the dead records)
 template <int W>
-__device__ __forceinline__ void restore_column(const SnapshotArgs& a, u32 p, u32 i0, u32 m, const u32* src) {
+__device__ __forceinline__ void restore_column(const SnapshotArgs& a, u32 p, u32 i0, u32 m, u32 dm, u32 n, const u32* src) {
     RepackPiece<W>* col = (RepackPiece<W>*)a.planes.ptr[p] + a.first;
     const u32 off = a.planes.word_off[p], al = snapshot_align(a.stride_words, off);
     RepackPiece<W> v[RP_ITEMS];
 #pragma unroll
     for (u32 k = 0; k < RP_ITEMS; ++k) {
         const u32 i = i0 + k * RP_THREADS;
-        if (i >= m) continue;
-        const u32* s = src + HNB_SNAPSHOT_HEADER_WORDS + u64(i) * a.stride_words + off;
+        if (i >= m + dm) continue;
+        const u32 r = i < m ? i : n + (i - m);
+        const u32* s = src + HNB_SNAPSHOT_HEADER_WORDS + u64(r) * a.stride_words + off;
         if (W >= 4 && al == 4u) snapshot_load<4>(s, v[k]);
         else if (W >= 2 && al >= 2u) snapshot_load<2>(s, v[k]);
         else snapshot_load<1>(s, v[k]);
     }
 #pragma unroll
     for (u32 k = 0; k < RP_ITEMS; ++k)
-        if (i0 + k * RP_THREADS < m) col[i0 + k * RP_THREADS] = v[k];
+        if (i0 + k * RP_THREADS < m + dm) col[i0 + k * RP_THREADS] = v[k];
 }
 
 // Record i < m -> local row i of every column; thread 0 writes alive_count = m, max_spawn = capacity - m (0 if the row's
 // capacity is below m) and, for an accepted header, particle_counter. k_repack_lists follows and reads m back.
-__global__ void __launch_bounds__(RP_THREADS) k_restore_scatter(SnapshotArgs a, const u32* src) {
-    const u32 m = restore_count(a, src);
+// DEAD (version 2): also dead record n + j -> row m + j for j < dm, and max_update = m + dm.
+template <bool DEAD>
+__device__ __forceinline__ void restore_scatter(const SnapshotArgs& a, const u32* src, u32 channels) {
+    u32 m, dm = 0u, n = 0u;
+    bool ok;
+    if (DEAD) {
+        const RestoreSpan s = restore_span(a, src, channels);
+        m = s.m; dm = s.dm; n = s.n; ok = s.ok;
+    } else {
+        m = restore_count(a, src);
+        ok = src[0] == HNB_SNAPSHOT_MAGIC_WORD && src[1] == HNB_SNAPSHOT_VERSION_WORD && src[2] == a.stride_words * 4u;
+    }
     const u32 i0 = blockIdx.x * RP_ROWS_PER_BLOCK + threadIdx.x;
     if (i0 == 0u) {
         EffectMetadata* md = a.metadata;
         md->alive_count = m;
         md->max_spawn = md->capacity > m ? md->capacity - m : 0u;
-        if (src[0] == HNB_SNAPSHOT_MAGIC_WORD && src[1] == HNB_SNAPSHOT_VERSION_WORD && src[2] == a.stride_words * 4u)
-            md->particle_counter = src[4];
+        if (ok) md->particle_counter = src[4];
+        if (DEAD) md->max_update = m + dm;
     }
-    if (i0 >= m) return;
+    if (i0 >= m + dm) return;
     for (u32 p = 0; p < a.num_planes; ++p) {
         switch (a.planes.words[p]) {
-        case 1: restore_column<1>(a, p, i0, m, src); break;
-        case 2: restore_column<2>(a, p, i0, m, src); break;
-        case 4: restore_column<4>(a, p, i0, m, src); break;
-        default: restore_column<8>(a, p, i0, m, src); break;
+        case 1: restore_column<1>(a, p, i0, m, dm, n, src); break;
+        case 2: restore_column<2>(a, p, i0, m, dm, n, src); break;
+        case 4: restore_column<4>(a, p, i0, m, dm, n, src); break;
+        default: restore_column<8>(a, p, i0, m, dm, n, src); break;
         }
     }
+}
+__global__ void __launch_bounds__(RP_THREADS) k_restore_scatter(SnapshotArgs a, const u32* src) { restore_scatter<false>(a, src, 0u); }
+__global__ void __launch_bounds__(RP_THREADS) k_restore_scatter_dead(SnapshotArgs a, const u32* src, u32 channels) {
+    restore_scatter<true>(a, src, channels);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Pending GPU spawn events of an emitting instance (hnb_slab_repack_events, hnb_instance_snapshot_events,
+// hnb_instance_restore_events). Between frames an event is an instance-local parent slot: a live slot or one of the D
+// slots the last update freed. The repack and the snapshot move slot src[i] to row / record i, so both translate an event
+// through inv[src[i]] = i.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ ChildInfo* channel_info(const EventChannels& ev, const EffectMetadata* md, u32 b) {
+    const u64 row = u64(md->base_child_index) + b;
+    return row < ev.num_child_infos ? &ev.child_infos[row] : nullptr;
+}
+// entries of channel b that hold an event: min(event_count, capacity)
+__device__ __forceinline__ u32 channel_stored(const EventChannels& ev, const EffectMetadata* md, u32 b) {
+    const ChildInfo* ci = channel_info(ev, md, b);
+    return ci ? min(u32(ci->event_count), ev.capacity[b]) : 0u;
+}
+
+// inv[src[i]] = i over the slice; before k_repack_lists, which rewrites the lists
+__global__ void __launch_bounds__(RP_THREADS) k_repack_inverse(RepackArgs a, u32* inv) {
+    const u32 n = min(a.metadata->alive_count, a.rows);
+    const u32* list = a.metadata->indirect_write_index == 0u ? a.ping : a.pong;
+    const u32 i = blockIdx.x * RP_THREADS + threadIdx.x;
+    if (i < a.rows) inv[repack_source(a, list, n, i)] = i;
+}
+
+// Entry k of channel b = blockIdx.x / blocks_per_channel. `snapshot` NULL (repack): e -> inv[e] in place. Otherwise the
+// entry goes to the snapshot as the record index inv[e], or 0xFFFFFFFF when that is not below n + D, after the channels
+// before it; block 0 writes header words 7-15. Clamped to the slice, like repack_source.
+__global__ void __launch_bounds__(RP_THREADS) k_events_translate(RepackArgs a, const u32* inv, EventChannels ev, u32 blocks_per_channel,
+                                                                 u32 stride_words, u32* snapshot) {
+    const EffectMetadata* md = a.metadata;
+    const u32 b = blockIdx.x / blocks_per_channel;
+    const u32 k = (blockIdx.x % blocks_per_channel) * RP_THREADS + threadIdx.x;
+    const u32 stored = channel_stored(ev, md, b);
+    if (!snapshot) {
+        if (k < stored) ev.buffer[b][k] = min(inv[min(ev.buffer[b][k], a.rows - 1u)], a.rows - 1u);
+        return;
+    }
+    const u32 n = min(md->alive_count, a.rows);
+    const u32 records = n + last_dead_count(md, n, a.rows);
+    if (blockIdx.x == 0u && threadIdx.x < 1u + 2u * HNB_MAX_EVENT_BINDINGS) {
+        const u32 t = threadIdx.x, c = (t - 1u) % HNB_MAX_EVENT_BINDINGS;
+        const ChildInfo* ci = c < ev.count ? channel_info(ev, md, c) : nullptr;
+        snapshot[7u + t] = t == 0u ? ev.count
+                         : t <= HNB_MAX_EVENT_BINDINGS ? (ci ? u32(ci->event_count) : 0u)
+                         : (c < ev.count ? channel_stored(ev, md, c) : 0u);
+    }
+    if (k >= stored) return;
+    u64 off = HNB_SNAPSHOT_HEADER_WORDS + u64(records) * stride_words;
+    for (u32 c = 0; c < b; ++c) off += channel_stored(ev, md, c);
+    const u32 r = inv[min(ev.buffer[b][k], a.rows - 1u)];
+    snapshot[off + k] = r < records ? r : 0xFFFFFFFFu;
 }
 
 // Order-independent checksum: sum over rows of a 64-bit mix of the row's AoS words and row index.
@@ -742,6 +849,48 @@ __global__ void __launch_bounds__(EV_THREADS) k_events_write(EventAppendArgs a) 
         const u32 particle_index = read_col[first + k];
         for (u32 i = 0; i < c[k] && pos + i < a.capacity; ++i) a.buffer[pos + i] = particle_index;
         pos += c[k];
+    }
+}
+
+// CTA b compacts channel b of a version-2 snapshot into its buffer: record index r -> row r (r < m) or m + r - n
+// (n <= r < n + dm), any other entry dropped, as is every entry past the capacity; order kept. event_count becomes the
+// stored unclamped count minus the dropped entries (0 for a rejected header). Reads nothing past src_bytes.
+__global__ void __launch_bounds__(EV_THREADS) k_restore_events(SnapshotArgs a, const u32* src, EventChannels ev) {
+    __shared__ u32 s_warp[EV_THREADS / 32];
+    __shared__ u32 s_carry;
+    const u32 b = blockIdx.x;
+    const RestoreSpan s = restore_span(a, src, ev.count);
+    ChildInfo* ci = channel_info(ev, a.metadata, b);
+    if (!s.ok) {
+        if (threadIdx.x == 0u && ci) ci->event_count = 0;
+        return;
+    }
+    const u32 unclamped = src[8u + b], stored = src[12u + b], cap = ev.capacity[b];
+    u64 off = HNB_SNAPSHOT_HEADER_WORDS + (u64(s.n) + s.d) * a.stride_words;
+    for (u32 c = 0; c < b; ++c) off += src[12u + c];
+    const u64 words = a.src_bytes / 4u;
+    const u32 readable = off < words ? (words - off < stored ? u32(words - off) : stored) : 0u;
+    if (threadIdx.x == 0u) s_carry = 0u;
+    __syncthreads();
+    for (u32 k0 = 0; k0 < readable; k0 += EV_THREADS) {
+        const u32 carry = s_carry;
+        if (carry >= cap) break;  // uniform: every thread read s_carry after the same barrier
+        const u32 k = k0 + threadIdx.x;
+        u32 row = 0xFFFFFFFFu;
+        if (k < readable) {
+            const u32 r = src[off + k];
+            if (r < s.m) row = r;
+            else if (r >= s.n && r - s.n < s.dm) row = s.m + (r - s.n);
+        }
+        u32 total;
+        const u32 pos = carry + ev_block_exclusive_scan(row != 0xFFFFFFFFu ? 1u : 0u, s_warp, &total);
+        if (row != 0xFFFFFFFFu && pos < cap) ev.buffer[b][pos] = row;
+        if (threadIdx.x == 0u) s_carry = carry + total;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0u && ci) {
+        const u32 dropped = stored - min(s_carry, cap);
+        ci->event_count = i32(unclamped >= dropped ? unclamped - dropped : 0u);
     }
 }
 
@@ -890,14 +1039,35 @@ cudaError_t launch_repack_lists(const RepackArgs& a, cudaStream_t st) {
     k_repack_lists<<<blocks_for(a.rows, RP_THREADS), RP_THREADS, 0, st>>>(a);
     return cudaGetLastError();
 }
-cudaError_t launch_snapshot_gather(const SnapshotArgs& a, u32* dst, cudaStream_t st) {
+cudaError_t launch_snapshot_gather(const SnapshotArgs& a, u32* dst, cudaStream_t st, const u32* dead) {
     if (a.rows == 0) return cudaSuccess;
-    k_snapshot_gather<<<blocks_for(a.rows, RP_ROWS_PER_BLOCK), RP_THREADS, 0, st>>>(a, dst);
+    if (dead) k_snapshot_gather_dead<<<blocks_for(a.rows, RP_ROWS_PER_BLOCK), RP_THREADS, 0, st>>>(a, dead, dst);
+    else k_snapshot_gather<<<blocks_for(a.rows, RP_ROWS_PER_BLOCK), RP_THREADS, 0, st>>>(a, dst);
     return cudaGetLastError();
 }
-cudaError_t launch_restore_scatter(const SnapshotArgs& a, const u32* src, cudaStream_t st) {
+cudaError_t launch_restore_scatter(const SnapshotArgs& a, const u32* src, cudaStream_t st, const u32* channels) {
     if (a.rows == 0) return cudaSuccess;
-    k_restore_scatter<<<blocks_for(a.rows, RP_ROWS_PER_BLOCK), RP_THREADS, 0, st>>>(a, src);
+    if (channels) k_restore_scatter_dead<<<blocks_for(a.rows, RP_ROWS_PER_BLOCK), RP_THREADS, 0, st>>>(a, src, *channels);
+    else k_restore_scatter<<<blocks_for(a.rows, RP_ROWS_PER_BLOCK), RP_THREADS, 0, st>>>(a, src);
+    return cudaGetLastError();
+}
+cudaError_t launch_repack_inverse(const RepackArgs& a, u32* inv, cudaStream_t st) {
+    if (a.rows == 0) return cudaSuccess;
+    k_repack_inverse<<<blocks_for(a.rows, RP_THREADS), RP_THREADS, 0, st>>>(a, inv);
+    return cudaGetLastError();
+}
+cudaError_t launch_events_translate(const RepackArgs& a, const u32* inv, const EventChannels& ev, u32 stride_words, u32* snapshot,
+                                    cudaStream_t st) {
+    if (a.rows == 0 || ev.count == 0) return cudaSuccess;
+    u32 widest = 1u;
+    for (u32 b = 0; b < ev.count; ++b) widest = std::max(widest, ev.capacity[b]);
+    const u32 per_channel = blocks_for(widest, RP_THREADS);
+    k_events_translate<<<per_channel * ev.count, RP_THREADS, 0, st>>>(a, inv, ev, per_channel, stride_words, snapshot);
+    return cudaGetLastError();
+}
+cudaError_t launch_restore_events(const SnapshotArgs& a, const u32* src, const EventChannels& ev, cudaStream_t st) {
+    if (a.rows == 0 || ev.count == 0) return cudaSuccess;
+    k_restore_events<<<ev.count, EV_THREADS, 0, st>>>(a, src, ev);
     return cudaGetLastError();
 }
 cudaError_t launch_measure_sm_clock(u64* out2, u64 window_ns, cudaStream_t st) {

@@ -101,10 +101,31 @@ struct SnapshotArgs {
     u32 first, rows;           // the slice
     u64 src_bytes;             // restore: bytes readable at the source (>= 64)
 };
-// header + records i < min(alive_count, rows) in alive-list order
-cudaError_t launch_snapshot_gather(const SnapshotArgs& a, u32* dst, cudaStream_t st);
-// records i < m to local rows i, and alive_count / max_spawn / particle_counter; enqueue launch_repack_lists after it
-cudaError_t launch_restore_scatter(const SnapshotArgs& a, const u32* src, cudaStream_t st);
+// header + records i < min(alive_count, rows) in alive-list order. `dead` (the slab's dead stack, row 0): a version-2
+// header, and the D records of the slots the last update freed after them; launch_events_translate completes it.
+cudaError_t launch_snapshot_gather(const SnapshotArgs& a, u32* dst, cudaStream_t st, const u32* dead = nullptr);
+// records i < m to local rows i, and alive_count / max_spawn / particle_counter; enqueue launch_repack_lists after it.
+// `channels` != NULL: a version-2 snapshot of that many event channels; also the dead records and max_update.
+cudaError_t launch_restore_scatter(const SnapshotArgs& a, const u32* src, cudaStream_t st, const u32* channels = nullptr);
+
+// The event buffers an emitting instance appends to (hnb_batch_launch.emit_events), channels b < count. Channel b's
+// pending count is child_infos[metadata->base_child_index + b].event_count (none when that row does not exist).
+#define HNB_SNAPSHOT_EVENTS_VERSION_WORD 2u
+struct EventChannels {
+    u32* buffer[HNB_MAX_EVENT_BINDINGS];
+    u32 capacity[HNB_MAX_EVENT_BINDINGS];
+    u32 count;
+    ChildInfo* child_infos;
+    u32 num_child_infos;
+};
+// inv[src[i]] = i for the repack's source rows (rows words); enqueue before launch_repack_lists
+cudaError_t launch_repack_inverse(const RepackArgs& a, u32* inv, cudaStream_t st);
+// every pending event e -> inv[e]: in place (`snapshot` NULL), or as record indices into a version-2 snapshot whose
+// records launch_snapshot_gather wrote (header words 7-15 and the entries)
+cudaError_t launch_events_translate(const RepackArgs& a, const u32* inv, const EventChannels& ev, u32 stride_words, u32* snapshot,
+                                    cudaStream_t st);
+// the events of a version-2 snapshot into the channels' buffers and event counts; after launch_restore_scatter
+cudaError_t launch_restore_events(const SnapshotArgs& a, const u32* src, const EventChannels& ev, cudaStream_t st);
 
 cudaError_t launch_indirect(const StaticTables& T, u32 num_effects, cudaStream_t st);
 cudaError_t launch_prefix_sum(const StaticTables& T, u32 num_batches, cudaStream_t st);

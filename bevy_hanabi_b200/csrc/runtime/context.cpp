@@ -1191,17 +1191,48 @@ int32_t hnb_slab_fill_c5_ex(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t cou
 // context does not keep up to 2 GiB between repacks that may be seconds apart.
 namespace {
 // The checks every call that rewrites or reads one instance's slice through its lists makes (`what`: the call's name).
+// `emit` NULL: a call that takes no event buffers, which refuses emitting effects. Otherwise the instance's event buffers
+// (hnb_batch_launch.emit_events): the effect must emit, with one distinct buffer per channel and UINT32_MAX past them.
 void check_instance_slice(hnb_ctx* c, const Slab& s, const Effect& fx, uint32_t metadata_row, uint32_t first, uint32_t rows,
-                          const char* what) {
+                          const char* what, const hnb_event_buffer* emit = nullptr) {
     const std::string w = what;
     if (uint64_t(first) + rows > s.capacity) fail(HNB_ERR_INVALID_ARG, w + ": rows outside the slab");
     if (metadata_row >= c->d_metadata.size()) fail(HNB_ERR_INVALID_ARG, w + ": metadata row out of range");
     if (fx.particle_stride != s.stride) fail(HNB_ERR_INVALID_ARG, w + ": effect particle stride does not match the slab");
     if (((fx.flags & HNB_EFFECT_SECTOR_PLANES) != 0) != s.sector_planes)
         fail(HNB_ERR_INVALID_ARG, w + ": effect and slab disagree on HNB_EFFECT_SECTOR_PLANES / HNB_SLAB_SECTOR_PLANES");
-    if (fx.flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS)
-        fail(HNB_ERR_INVALID_ARG, w + ": pending GPU spawn events name parent slots; an emitting effect cannot be " +
-                                      (w == "hnb_slab_repack" ? "repacked" : "snapshot or restored"));
+    const bool emits = (fx.flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS) != 0;
+    if (!emit) {
+        if (emits)
+            fail(HNB_ERR_INVALID_ARG, w + ": pending GPU spawn events name parent slots; an emitting effect cannot be " +
+                                          (w == "hnb_slab_repack" ? "repacked" : "snapshot or restored") + " without its event buffers");
+        return;
+    }
+    if (!emits) fail(HNB_ERR_INVALID_ARG, w + ": the effect does not have HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS");
+    const uint32_t channels = fx.desc->d.num_event_bindings;
+    if (channels > HNB_MAX_EVENT_BINDINGS) fail(HNB_ERR_INVALID_ARG, w + ": the effect has more event channels than emit_events holds");
+    for (uint32_t b = 0; b < HNB_MAX_EVENT_BINDINGS; ++b) {
+        if (b >= channels) {
+            if (emit[b] != 0xFFFFFFFFu) fail(HNB_ERR_INVALID_ARG, w + ": an event buffer is given for a channel the effect does not have");
+            continue;
+        }
+        if (emit[b] >= c->event_buffers.size()) fail(HNB_ERR_INVALID_ARG, w + ": a channel of the effect has no valid event buffer");
+        for (uint32_t o = 0; o < b; ++o)
+            if (emit[o] == emit[b]) fail(HNB_ERR_INVALID_ARG, w + ": the same event buffer is given for two channels");
+    }
+}
+
+// The checked event buffers of an emitting instance and the context's child-info rows their counts live in.
+hnb::EventChannels event_channels(hnb_ctx* c, const Effect& fx, const hnb_event_buffer* emit) {
+    hnb::EventChannels ev{};
+    ev.count = fx.desc->d.num_event_bindings;
+    for (uint32_t b = 0; b < ev.count; ++b) {
+        ev.buffer[b] = c->event_buffers[emit[b]].get();
+        ev.capacity[b] = uint32_t(c->event_buffers[emit[b]].size());
+    }
+    ev.child_infos = c->d_child_infos.get();
+    ev.num_child_infos = uint32_t(c->d_child_infos.size());
+    return ev;
 }
 
 hnb::RepackArgs repack_args(hnb_ctx* c, const Slab& s, uint32_t metadata_row, uint32_t first, uint32_t rows) {
@@ -1231,11 +1262,15 @@ hnb::SnapshotArgs snapshot_args(hnb_ctx* c, const Slab& s, uint32_t metadata_row
 }
 }  // namespace
 
-int32_t hnb_slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows) {
+namespace {
+// hnb_slab_repack and, with `emit`, hnb_slab_repack_events: the inverse permutation (for the events) and every column
+// gather read the lists, so the list writer goes last.
+int32_t slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                    const hnb_event_buffer* emit, const char* what) {
     return guarded([&] {
         Slab& s = get_slab(c, h);
         const Effect& fx = get_effect(c, e);
-        check_instance_slice(c, s, fx, metadata_row, first, rows, "hnb_slab_repack");
+        check_instance_slice(c, s, fx, metadata_row, first, rows, what, emit);
         if (rows == 0) return;
         fix_plan(c, s, fx.plan);
         CUDA_CHECK(cudaSetDevice(c->device));
@@ -1243,13 +1278,22 @@ int32_t hnb_slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_
         uint32_t widest = 0;
         for (const Plane& p : s.planes) widest = std::max(widest, p.width);
         void* scratch = nullptr;
-        CUDA_CHECK(cudaMallocAsync(&scratch, size_t(rows) * widest, c->stream));
+        CUDA_CHECK(cudaMallocAsync(&scratch, size_t(rows) * (widest + (emit ? 4 : 0)), c->stream));
+        uint32_t* inv = (uint32_t*)((char*)scratch + size_t(rows) * widest);
         cudaError_t err = cudaSuccess;
+        if (emit) {
+            err = hnb::launch_repack_inverse(a, inv, c->stream);
+            c->launches++;
+        }
         for (size_t p = 0; p < s.planes.size() && err == cudaSuccess; ++p) {
             const uint32_t width = s.planes[p].width;
             err = hnb::launch_repack_gather(a, s.column(p), scratch, width, c->stream);
             if (err == cudaSuccess)
                 err = cudaMemcpyAsync(s.column(p) + size_t(first) * width, scratch, size_t(rows) * width, cudaMemcpyDeviceToDevice, c->stream);
+            c->launches++;
+        }
+        if (emit && err == cudaSuccess) {
+            err = hnb::launch_events_translate(a, inv, event_channels(c, fx, emit), 0, nullptr, c->stream);
             c->launches++;
         }
         // the lists last: every gather reads them
@@ -1261,52 +1305,115 @@ int32_t hnb_slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_
     });
 }
 
-static_assert(HNB_SNAPSHOT_MAGIC == HNB_SNAPSHOT_MAGIC_WORD && HNB_SNAPSHOT_VERSION == HNB_SNAPSHOT_VERSION_WORD &&
-                  sizeof(hnb_instance_snapshot_header) == HNB_SNAPSHOT_HEADER_WORDS * 4,
-              "snapshot header of include/hanabi_b200.h and of the kernels");
-
-size_t hnb_instance_snapshot_bytes(uint32_t particle_stride, uint32_t rows) {
-    return sizeof(hnb_instance_snapshot_header) + size_t(rows) * particle_stride;
-}
-
-// One launch: the kernel reads n, W and particle_counter on the device, so the host never waits for them.
-int32_t hnb_instance_snapshot(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
-                              void* d_dst, size_t dst_bytes) {
+// hnb_instance_snapshot (one launch: the kernel reads n, W and particle_counter on the device, so the host never waits for
+// them) and, with `emit`, hnb_instance_snapshot_events (the records, then the inverse permutation in a stream-ordered
+// scratch of rows words, then the header's event words and the events).
+int32_t instance_snapshot(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                          const hnb_event_buffer* emit, void* d_dst, size_t dst_bytes, const char* what) {
     return guarded([&] {
         Slab& s = get_slab(c, h);
         const Effect& fx = get_effect(c, e);
-        check_instance_slice(c, s, fx, metadata_row, first, rows, "hnb_instance_snapshot");
-        if (!d_dst || ((uintptr_t)d_dst & 15u)) fail(HNB_ERR_INVALID_ARG, "hnb_instance_snapshot: d_dst is NULL or not 16-byte aligned");
-        if (dst_bytes < hnb_instance_snapshot_bytes(s.stride, rows))
-            fail(HNB_ERR_INVALID_ARG, "hnb_instance_snapshot: dst_bytes is below hnb_instance_snapshot_bytes(stride, rows)");
+        const std::string w = what;
+        check_instance_slice(c, s, fx, metadata_row, first, rows, what, emit);
+        if (!d_dst || ((uintptr_t)d_dst & 15u)) fail(HNB_ERR_INVALID_ARG, w + ": d_dst is NULL or not 16-byte aligned");
+        hnb::EventChannels ev{};
+        if (emit) {
+            ev = event_channels(c, fx, emit);
+            uint32_t capacity[HNB_MAX_EVENT_BINDINGS] = {};
+            for (uint32_t b = 0; b < ev.count; ++b) capacity[b] = ev.capacity[b];
+            if (dst_bytes < hnb_instance_snapshot_events_bytes(s.stride, rows, capacity))
+                fail(HNB_ERR_INVALID_ARG, w + ": dst_bytes is below hnb_instance_snapshot_events_bytes(stride, rows, capacities)");
+        } else if (dst_bytes < hnb_instance_snapshot_bytes(s.stride, rows)) {
+            fail(HNB_ERR_INVALID_ARG, w + ": dst_bytes is below hnb_instance_snapshot_bytes(stride, rows)");
+        }
         if (rows == 0) return;
         CUDA_CHECK(cudaSetDevice(c->device));
-        CUDA_CHECK(hnb::launch_snapshot_gather(snapshot_args(c, s, metadata_row, first, rows), (uint32_t*)d_dst, c->stream));
+        CUDA_CHECK(hnb::launch_snapshot_gather(snapshot_args(c, s, metadata_row, first, rows), (uint32_t*)d_dst, c->stream,
+                                               emit ? s.dead.get() : nullptr));
         c->launches++;
+        if (!emit) return;
+        const hnb::RepackArgs a = repack_args(c, s, metadata_row, first, rows);
+        void* inv = nullptr;
+        CUDA_CHECK(cudaMallocAsync(&inv, size_t(rows) * 4, c->stream));
+        cudaError_t err = hnb::launch_repack_inverse(a, (uint32_t*)inv, c->stream);
+        if (err == cudaSuccess) err = hnb::launch_events_translate(a, (const uint32_t*)inv, ev, s.stride / 4, (uint32_t*)d_dst, c->stream);
+        c->launches += 2;
+        const cudaError_t freed = cudaFreeAsync(inv, c->stream);
+        CUDA_CHECK(err);
+        CUDA_CHECK(freed);
     });
 }
 
-// Two launches: the records and the metadata words, then hnb_slab_repack's list writer, which reads m back from
-// alive_count.
-int32_t hnb_instance_restore(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
-                             const void* d_src, size_t src_bytes) {
+// hnb_instance_restore (two launches: the records and the metadata words, then hnb_slab_repack's list writer, which reads
+// m back from alive_count) and, with `emit`, hnb_instance_restore_events (then one CTA per channel for the events).
+int32_t instance_restore(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                         const hnb_event_buffer* emit, const void* d_src, size_t src_bytes, const char* what) {
     return guarded([&] {
         Slab& s = get_slab(c, h);
         const Effect& fx = get_effect(c, e);
-        check_instance_slice(c, s, fx, metadata_row, first, rows, "hnb_instance_restore");
-        if (!d_src || ((uintptr_t)d_src & 15u)) fail(HNB_ERR_INVALID_ARG, "hnb_instance_restore: d_src is NULL or not 16-byte aligned");
-        if (src_bytes < sizeof(hnb_instance_snapshot_header)) fail(HNB_ERR_INVALID_ARG, "hnb_instance_restore: src_bytes is below the 64-byte header");
+        const std::string w = what;
+        check_instance_slice(c, s, fx, metadata_row, first, rows, what, emit);
+        if (!d_src || ((uintptr_t)d_src & 15u)) fail(HNB_ERR_INVALID_ARG, w + ": d_src is NULL or not 16-byte aligned");
+        if (src_bytes < sizeof(hnb_instance_snapshot_header)) fail(HNB_ERR_INVALID_ARG, w + ": src_bytes is below the 64-byte header");
         if (rows == 0) return;
         CUDA_CHECK(cudaSetDevice(c->device));
         fix_plan(c, s, fx.plan);
         s.written = true;
         hnb::SnapshotArgs a = snapshot_args(c, s, metadata_row, first, rows);
         a.src_bytes = src_bytes;
-        CUDA_CHECK(hnb::launch_restore_scatter(a, (const uint32_t*)d_src, c->stream));
+        const hnb::EventChannels ev = emit ? event_channels(c, fx, emit) : hnb::EventChannels{};
+        CUDA_CHECK(hnb::launch_restore_scatter(a, (const uint32_t*)d_src, c->stream, emit ? &ev.count : nullptr));
         c->launches++;
         CUDA_CHECK(hnb::launch_repack_lists(repack_args(c, s, metadata_row, first, rows), c->stream));
         c->launches++;
+        if (!emit) return;
+        CUDA_CHECK(hnb::launch_restore_events(a, (const uint32_t*)d_src, ev, c->stream));
+        c->launches++;
     });
+}
+}  // namespace
+
+int32_t hnb_slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows) {
+    return slab_repack(c, h, e, metadata_row, first, rows, nullptr, "hnb_slab_repack");
+}
+int32_t hnb_slab_repack_events(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                               const hnb_event_buffer emit_events[HNB_MAX_EVENT_BINDINGS]) {
+    if (!emit_events) return guarded([] { fail(HNB_ERR_INVALID_ARG, "hnb_slab_repack_events: emit_events is NULL"); });
+    return slab_repack(c, h, e, metadata_row, first, rows, emit_events, "hnb_slab_repack_events");
+}
+
+static_assert(HNB_SNAPSHOT_MAGIC == HNB_SNAPSHOT_MAGIC_WORD && HNB_SNAPSHOT_VERSION == HNB_SNAPSHOT_VERSION_WORD &&
+                  HNB_SNAPSHOT_EVENTS_VERSION == HNB_SNAPSHOT_EVENTS_VERSION_WORD &&
+                  sizeof(hnb_instance_snapshot_header) == HNB_SNAPSHOT_HEADER_WORDS * 4,
+              "snapshot header of include/hanabi_b200.h and of the kernels");
+
+size_t hnb_instance_snapshot_bytes(uint32_t particle_stride, uint32_t rows) {
+    return sizeof(hnb_instance_snapshot_header) + size_t(rows) * particle_stride;
+}
+size_t hnb_instance_snapshot_events_bytes(uint32_t particle_stride, uint32_t rows, const uint32_t event_capacity[HNB_MAX_EVENT_BINDINGS]) {
+    size_t bytes = hnb_instance_snapshot_bytes(particle_stride, rows);
+    for (int b = 0; event_capacity && b < HNB_MAX_EVENT_BINDINGS; ++b) bytes += size_t(event_capacity[b]) * 4;
+    return bytes;
+}
+
+int32_t hnb_instance_snapshot(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                              void* d_dst, size_t dst_bytes) {
+    return instance_snapshot(c, h, e, metadata_row, first, rows, nullptr, d_dst, dst_bytes, "hnb_instance_snapshot");
+}
+int32_t hnb_instance_snapshot_events(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                                     const hnb_event_buffer emit_events[HNB_MAX_EVENT_BINDINGS], void* d_dst, size_t dst_bytes) {
+    if (!emit_events) return guarded([] { fail(HNB_ERR_INVALID_ARG, "hnb_instance_snapshot_events: emit_events is NULL"); });
+    return instance_snapshot(c, h, e, metadata_row, first, rows, emit_events, d_dst, dst_bytes, "hnb_instance_snapshot_events");
+}
+
+int32_t hnb_instance_restore(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                             const void* d_src, size_t src_bytes) {
+    return instance_restore(c, h, e, metadata_row, first, rows, nullptr, d_src, src_bytes, "hnb_instance_restore");
+}
+int32_t hnb_instance_restore_events(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                                    const hnb_event_buffer emit_events[HNB_MAX_EVENT_BINDINGS], const void* d_src, size_t src_bytes) {
+    if (!emit_events) return guarded([] { fail(HNB_ERR_INVALID_ARG, "hnb_instance_restore_events: emit_events is NULL"); });
+    return instance_restore(c, h, e, metadata_row, first, rows, emit_events, d_src, src_bytes, "hnb_instance_restore_events");
 }
 
 int32_t hnb_slab_checksum(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, uint64_t* out) {

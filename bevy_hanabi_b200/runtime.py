@@ -184,6 +184,14 @@ def initial_metadata(capacity: int, draw_index: int = 0, particle_stride_words: 
     return m
 
 
+def _channels(emit_events) -> C.Array:
+    """An instance's event buffers, channel by channel, as the four-entry emit_events array (N.INVALID = none)."""
+    buffers = list(emit_events)
+    if len(buffers) > 4:
+        raise ValueError("at most 4 event channels")
+    return (C.c_uint32 * 4)(*(buffers + [N.INVALID] * (4 - len(buffers))))
+
+
 class Context:
     """One simulation context on one GPU (≙ the render-world resources of HanabiPlugin)."""
 
@@ -323,6 +331,31 @@ class Context:
         or context whose effect has the snapshot's stride); its lists, claims and alive bits become what slab_repack
         leaves. `src_bytes`: bytes readable at `d_src` (>= 64). Only enqueues work."""
         check(lib.hnb_instance_restore(self._h, slab, effect, metadata_row, first, rows, d_src, src_bytes))
+
+    def slab_repack_events(self, slab: int, effect: int, metadata_row: int, first: int, rows: int, emit_events) -> None:
+        """slab_repack for an instance of an effect that emits GPU spawn events: `emit_events` (one event buffer per
+        channel of the effect, as given to its update launch) have their pending events rewritten to the rows their
+        parents moved to (hnb_slab_repack_events). Only enqueues work."""
+        check(lib.hnb_slab_repack_events(self._h, slab, effect, metadata_row, first, rows, _channels(emit_events)))
+
+    @staticmethod
+    def instance_snapshot_events_bytes(particle_stride: int, rows: int, event_capacities) -> int:
+        """Bytes a version-2 snapshot may need: the header, `rows` records and every channel's buffer capacity."""
+        caps = list(event_capacities) + [0] * (4 - len(event_capacities))
+        return lib.hnb_instance_snapshot_events_bytes(particle_stride, rows, (C.c_uint32 * 4)(*caps))
+
+    def instance_snapshot_events(self, slab: int, effect: int, metadata_row: int, first: int, rows: int, emit_events,
+                                 d_dst: int, dst_bytes: int) -> None:
+        """instance_snapshot for an emitting instance: a version-2 snapshot that also holds the records of the slots its
+        last update freed and the pending events of `emit_events` (hnb_instance_snapshot_events). Only enqueues work."""
+        check(lib.hnb_instance_snapshot_events(self._h, slab, effect, metadata_row, first, rows, _channels(emit_events), d_dst, dst_bytes))
+
+    def instance_restore_events(self, slab: int, effect: int, metadata_row: int, first: int, rows: int, emit_events,
+                                d_src: int, src_bytes: int) -> None:
+        """instance_restore of a version-2 snapshot: the pending events go into `emit_events` of this context, renamed to
+        the rows their parents were restored to, and into the event counts of the metadata row's child-info rows
+        (hnb_instance_restore_events). Only enqueues work."""
+        check(lib.hnb_instance_restore_events(self._h, slab, effect, metadata_row, first, rows, _channels(emit_events), d_src, src_bytes))
 
     def slab_checksum(self, slab: int, first: int, count: int, index_base: int = 0) -> int:
         out = C.c_uint64(0)

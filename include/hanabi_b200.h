@@ -167,6 +167,7 @@ HNB_API void hnb_ctx_frame_count(hnb_ctx* ctx, uint64_t* frames, uint64_t* frame
 /* ------------------------------------------------------------------------------------ */
 typedef uint32_t hnb_slab;
 typedef uint32_t hnb_effect;  /* a compiled effect registered with a context (section 4) */
+typedef uint32_t hnb_event_buffer;  /* an event buffer of GPU spawn events (section 5) */
 
 /**
  * Allocate a slab of `capacity_rows` particles whose reference AoS record is
@@ -311,6 +312,57 @@ HNB_API int32_t hnb_instance_snapshot(hnb_ctx* ctx, hnb_slab slab, hnb_effect ef
  */
 HNB_API int32_t hnb_instance_restore(hnb_ctx* ctx, hnb_slab slab, hnb_effect effect, uint32_t metadata_row, uint32_t first,
                                      uint32_t rows, const void* d_src, size_t src_bytes);
+
+/**
+ * Repack, snapshot and restore of an instance whose effect has HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS, together with the events
+ * it appended in its last update, which the children's next init consumes. Between frames a pending event is an
+ * instance-local parent slot: a live slot, or one of the D = min(max_update - n, rows - n) slots the last update freed,
+ * which sit at dead-stack positions n .. n+D of the slice (an OnDie parent keeps its record there). Each call takes
+ * `emit_events`, the instance's hnb_batch_launch.emit_events: a valid event buffer for every channel b <
+ * num_event_bindings, each buffer once, and 0xFFFFFFFF for the other channels. Channel b's pending count is the context's
+ * child_infos[base_child_index + b].event_count, base_child_index read from the DEVICE metadata row (a channel whose row
+ * does not exist has none). The calls keep every rule of the calls without events (between frames, work only enqueued,
+ * nothing read out of the slice) and return HNB_ERR_INVALID_ARG, with nothing enqueued, on the same inputs, and also when
+ * the effect does not emit or `emit_events` does not match its channels.
+ *
+ * hnb_slab_repack_events does what hnb_slab_repack does, and rewrites entries [0, min(event_count, capacity)) of every
+ * channel in place as e -> inv[e], where inv[src[i]] = i: each event names the row its parent's record moved to.
+ * event_count (its overflow surplus included) and the order of the entries do not change. Its scratch grows by rows x 4
+ * bytes.
+ *
+ * hnb_instance_snapshot_events writes a version-2 snapshot (HNB_SNAPSHOT_EVENTS_VERSION) into `d_dst`, of at least
+ * hnb_instance_snapshot_events_bytes(stride, rows, capacities) bytes (event_capacity[b]: the capacity of channel b's
+ * buffer, 0 past the effect's channels):
+ *   - header words 0-5 as in version 1; reserved[0] = D, reserved[1] = the channel count C, reserved[2 + b] = channel b's
+ *     unclamped event_count and reserved[6 + b] = e_b = min(event_count, capacity) (0 past C);
+ *   - the n live records in alive-list order, as in version 1, then D dead records: record n + j is local row
+ *     dead[first + n + j] - first;
+ *   - then, channel after channel, e_b entries: the record index of the event's slot, or 0xFFFFFFFF when that slot is
+ *     not one of the n + D records.
+ * The first 64 + (n + D) * stride + 4 * sum(e_b) bytes are the complete snapshot. The call takes a scratch of rows x 4
+ * bytes with cudaMallocAsync on the context stream and releases it the same way.
+ *
+ * hnb_instance_restore_events restores a version-2 snapshot whose stride and channel count match the effect. With m as
+ * for version 1, live record i < m goes to row i and dead record n + j to row m + j for j < D', where D' = min(D, rows - m,
+ * dead records within src_bytes). The lists, dead stack, claims and alive bits are those of hnb_instance_restore; the
+ * metadata row gets what hnb_instance_restore writes, plus max_update = m + D'. Record index r becomes row r (r < m) or
+ * m + r - n (n <= r < n + D'); any other entry is dropped, and so is every entry past the destination buffer's capacity
+ * or past src_bytes. The kept entries fill the channel's buffer in their order, and this context's
+ * child_infos[base_child_index + b].event_count becomes the stored unclamped count minus the dropped entries. A header
+ * that does not match restores an empty instance with event_count = 0 on every channel. Restoring into X's own slice
+ * leaves what hnb_slab_repack_events(X) leaves, except on rows >= n + D.
+ */
+#define HNB_SNAPSHOT_EVENTS_VERSION 2u
+HNB_API int32_t hnb_slab_repack_events(hnb_ctx* ctx, hnb_slab slab, hnb_effect effect, uint32_t metadata_row, uint32_t first,
+                                       uint32_t rows, const hnb_event_buffer emit_events[4]);
+/** Bytes a version-2 snapshot of a `rows`-row slice may need: 64 + rows * particle_stride + 4 * sum(event_capacity[b]). */
+HNB_API size_t hnb_instance_snapshot_events_bytes(uint32_t particle_stride, uint32_t rows, const uint32_t event_capacity[4]);
+HNB_API int32_t hnb_instance_snapshot_events(hnb_ctx* ctx, hnb_slab slab, hnb_effect effect, uint32_t metadata_row,
+                                             uint32_t first, uint32_t rows, const hnb_event_buffer emit_events[4], void* d_dst,
+                                             size_t dst_bytes);
+HNB_API int32_t hnb_instance_restore_events(hnb_ctx* ctx, hnb_slab slab, hnb_effect effect, uint32_t metadata_row,
+                                            uint32_t first, uint32_t rows, const hnb_event_buffer emit_events[4],
+                                            const void* d_src, size_t src_bytes);
 /** 64-bit FNV-style checksum of the AoS bytes of rows [first,first+count), computed on device
  *  (order-independent sum of per-row hashes), for whole-slab comparisons at sizes the host
  *  cannot download cheaply. */
@@ -513,7 +565,6 @@ HNB_API int32_t hnb_upload_properties(hnb_ctx* ctx, hnb_effect effect, uint32_t 
                                       const void* blob, uint32_t bytes);
 
 /* GPU spawn events (reference src/render/event.rs) */
-typedef uint32_t hnb_event_buffer;
 /** Allocate an event buffer of `capacity` SpawnEvent entries (reference hard-codes 256, event.rs:266). */
 HNB_API int32_t hnb_event_buffer_create(hnb_ctx* ctx, uint32_t capacity, hnb_event_buffer* out);
 HNB_API int32_t hnb_child_info_insert(hnb_ctx* ctx, uint32_t row, const hnb_child_info* info);

@@ -643,7 +643,63 @@ def c3_chain():
         ctx.close()
 
 
-SCENARIOS = {"c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
+def emitter_relocation():
+    """hnb_slab_repack_events, hnb_instance_snapshot_events and hnb_instance_restore_events on an emitting parent of 16 Mi
+    slots in a churned state, with two channels of 512 Ki entries, both full and overflowing (channel 0: Always, count 1;
+    channel 1: OnDie, count 4). The first repack runs on the churned lists (one window); snapshot and restore (into a
+    second slab) are best of 5."""
+    _card()
+    P, CAP = 16 << 20, 1 << 19
+    w = G.ExprWriter()
+    asset = (G.EffectAsset(P, w.module, name="relocated_emitter")
+             .init(G.SetAttributeModifier(A.POSITION, w.rand(G.VEC3) * w.lit(2.) - w.lit(1.)))
+             .init(G.SetAttributeModifier(A.VELOCITY, w.rand(G.VEC3) - w.lit(0.5)))
+             .init(G.SetAttributeModifier(A.AGE, w.lit(0.)))
+             .init(G.SetAttributeModifier(A.LIFETIME, w.lit(0.1).uniform(w.lit(0.5))))
+             .update(G.EmitSpawnEventModifier(G.ALWAYS, w.lit(G.U32(1)), 0))
+             .update(G.EmitSpawnEventModifier(G.ON_DIE, w.lit(G.U32(4)), 1)))
+    fx = asset.generate(num_event_bindings=2)
+    stride = fx.particle_stride
+    ctx = hb.Context(0, stream.cuda_stream)
+    slab, effect = ctx.slab_create(P, stride), ctx.effect_compile(fx)
+    ev = [ctx.event_buffer_create(CAP) for _ in range(4)]
+    for row in range(4):
+        ctx.child_info_insert(row, 0, 0)
+    for row in (0, 1):
+        md = R.initial_metadata(P, row, stride // 4)
+        md.base_child_index = 2 * row
+        ctx.metadata_insert(row, md)
+        ctx.draw_args_insert(row)
+    ctx.upload_batches([N.BatchInfo(0, 0, 0, 0, 0, 1)], [0])
+    dt, rate = 1 / 60, P // 24
+    for f in range(40):  # lifetimes of 6 to 30 frames: the list is a permutation of the slice by now
+        ctx.set_sim_params(dt, f * dt, 1)
+        ctx.upload_spawners([R.make_spawner(spawn=rate, seed=100 + f)])
+        ctx.simulate([N.BatchLaunch.make(effect, slab, 0, rate, emit_events=ev[:2])])
+    ctx.sync()
+    alive = ctx.read_metadata(0).alive_count
+    counts = [ctx.read_child_info(k).event_count for k in (0, 1)]
+    assert min(counts) > CAP, counts
+    events = 12 * 2 * CAP  # per entry: the entry read and written, one inverse word read
+    rp = _events_ms(lambda: ctx.slab_repack_events(slab, effect, 0, 0, P, ev[:2]), reps=1)
+    report(f"emitter_relocation: repack of {P >> 20} Mi rows, {alive >> 10} Ki alive, 2 x {CAP >> 10} Ki events", rp,
+           _repack_bytes(ctx, slab, P, alive) + 8 * P + events, "one window; bytes: repack + inverse + events")
+    nbytes = ctx.instance_snapshot_events_bytes(stride, P, [CAP, CAP])
+    buf = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
+    dst = ctx.slab_create(P, stride)
+    snap = _events_ms(lambda: ctx.instance_snapshot_events(slab, effect, 0, 0, P, ev[:2], buf.data_ptr(), nbytes))
+    rest = _events_ms(lambda: ctx.instance_restore_events(dst, effect, 1, 0, P, ev[2:], buf.data_ptr(), nbytes))
+    md = ctx.read_metadata(1)
+    records = md.max_update
+    restored = [ctx.read_child_info(k).event_count for k in (2, 3)]
+    report("emitter_relocation: snapshot", snap, (4 + 2 * stride) * records + 8 * P + events, f"{records >> 10} Ki records, best of 5")
+    report("emitter_relocation: restore", rest, (8 + 2 * stride) * records + 4 * (P - alive) + P // 8 + 8 * 2 * CAP,
+           f"into another slab, best of 5; event counts {counts} -> {restored}, alive {alive} -> {md.alive_count}")
+    del buf
+    ctx.close()
+
+
+SCENARIOS = {"c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "emitter_relocation": emitter_relocation, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
 if __name__ == "__main__":
     for name in (sys.argv[1:] or list(SCENARIOS)):
         try:
