@@ -291,15 +291,18 @@ int32_t hnb_asset_generate(const hnb_asset* a, const hnb_asset* parent, uint32_t
         auto g = std::make_unique<hnb_generated>();
         g->src = a->a.generate(parent ? &parent_layout : nullptr, num_event_bindings);
         g->name = a->a.name;
-        auto fill = [](const ParticleLayout& pl, std::vector<hnb_attr_layout>& v, const std::set<Attribute>* writes) {
+        auto fill = [](const ParticleLayout& pl, std::vector<hnb_attr_layout>& v, const std::set<Attribute>* writes, bool lifetime_reap_only) {
             for (const auto& l : pl.layout) {
                 if (l.is_pad) continue;
-                const bool read_only = writes && !writes->count(attribute_by_name(l.name));
-                v.push_back({static_name(l.name), l.type.code, l.offset, read_only ? uint32_t(HNB_ATTR_UPDATE_READ_ONLY) : 0u});
+                const Attribute a = attribute_by_name(l.name);
+                const bool read_only = writes && !writes->count(a);
+                uint32_t flags = read_only ? uint32_t(HNB_ATTR_UPDATE_READ_ONLY) : 0u;
+                if (read_only && lifetime_reap_only && a == attr::LIFETIME) flags |= HNB_ATTR_REAP_ONLY;
+                v.push_back({static_name(l.name), l.type.code, l.offset, flags});
             }
         };
-        fill(g->src.particle_layout, g->attrs, &g->src.update_writes);
-        if (g->src.parent_layout) fill(*g->src.parent_layout, g->parent_attrs, nullptr);
+        fill(g->src.particle_layout, g->attrs, &g->src.update_writes, g->src.lifetime_reap_only);
+        if (g->src.parent_layout) fill(*g->src.parent_layout, g->parent_attrs, nullptr, false);
         *out = g.release();
     });
 }

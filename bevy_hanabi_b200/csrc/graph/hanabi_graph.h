@@ -269,6 +269,7 @@ struct EffectShaderSource {  // what generate() substitutes into the kernel temp
     std::string init_code, init_extra, sim_space_code, age_code, reap_code, update_code, update_extra;
     uint32_t flags = 0;  // HNB_EFFECT_* layout flags
     std::set<Attribute> update_writes;  // attributes the update body assigns; the others are HNB_ATTR_UPDATE_READ_ONLY
+    bool lifetime_reap_only = false;    // LIFETIME gets HNB_ATTR_REAP_ONLY (see EffectAsset::generate)
     std::optional<ParticleLayout> parent_layout;
     uint32_t num_event_bindings = 0;
 };

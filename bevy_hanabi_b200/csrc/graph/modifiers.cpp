@@ -420,6 +420,10 @@ EffectShaderSource EffectAsset::generate(const ParticleLayout* parent_layout, ui
 
     // aging / reaping (lib.rs:1223-1264)
     const bool has_age = out.particle_layout.contains(attr::AGE), has_lifetime = out.particle_layout.contains(attr::LIFETIME);
+    // The lifetime is read only by the standard age and reap code below: no update modifier writes AGE or LIFETIME, and no
+    // other update code mentions the lifetime (a textual test, so it errs on the side of leaving the flag off).
+    out.lifetime_reap_only = has_age && has_lifetime && !out.update_writes.count(attr::AGE) && !out.update_writes.count(attr::LIFETIME) &&
+                             out.update_code.find("lifetime") == std::string::npos && out.update_extra.find("lifetime") == std::string::npos;
     if (has_age) {
         if (has_lifetime) out.age_code += "\n    const bool was_alive = particle.age < particle.lifetime; (void)was_alive;";
         else out.age_code += "\n    const bool was_alive = true; (void)was_alive;";  // the reference leaves it undeclared (latent bug)

@@ -12,6 +12,7 @@
 //   hnb_store_written                          the update's store: only the columns holding a word it may write
 //   hnb_init_body(Particle&, Ctx&)            = {{INIT_CODE}} + PREV/NEXT reset + {{SIM_SPACE}}
 //   hnb_update_body(Particle&, Ctx&) -> bool  = {{AGE_CODE}} {{REAP_CODE}} {{UPDATE_CODE}}, returns is_alive
+//   [HNB_LIFE_FLOOR: hnb_load_raw_but_life / hnb_load_life / hnb_raw_age / hnb_raw_life]  (lifetime floors)
 //
 // Design (DESIGN.md §kernels):
 //   * update is a persistent, single-pass "process + stable compaction" kernel with WARP-AUTONOMOUS
@@ -60,6 +61,12 @@ namespace hnb {
 #ifndef HNB_SLOT_ORDER
 #define HNB_SLOT_ORDER 0  // 1 (HNB_EFFECT_SLOT_ORDER): the update pass walks the instance's SLOTS in ascending order, guided by
                           // the slab's alive bitmap, instead of walking the alive list. See "slot order" below.
+#endif
+#ifndef HNB_LIFE_FLOOR
+#define HNB_LIFE_FLOOR 0  // 1 (generated for HNB_ATTR_REAP_ONLY lifetimes in a column of their own): see "lifetime floors" below
+#endif
+#if HNB_LIFE_FLOOR && (HNB_SLOT_ORDER || HNB_RELAXED_ORDER)
+#error "lifetime floors are kept by the ordered update pass only"
 #endif
 
 // --- tile state word of the decoupled look-back ---
@@ -284,6 +291,10 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK) hnb_init(const BatchPara
         hnb_raw_zero(raw);
         hnb_pack<true>(particle, raw);  // init also stores PREV/NEXT (vfx_init.wgsl:175-181)
         hnb_store_raw(raw, P.slab, base_particle + particle_index);
+#if HNB_LIFE_FLOOR
+        // the slot's lifetime changed: its group's floor proves nothing until an update stores a new one
+        if (P.life_floor) P.life_floor[(base_particle + particle_index) >> 5u] = __uint_as_float(HNB_LIFE_FLOOR_NONE);
+#endif
     }
 }
 
@@ -664,11 +675,23 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
             pidx_next[k] = row < trust_r ? row : (row < max_update ? read_col[row] : 0u);
         }
 #endif
+#if HNB_LIFE_FLOOR
+        // Lifetime floors (DESIGN.md §3). In a tile wholly below trust_r every row holds its own index, so when the instance
+        // starts on a 32-row group, row group k of a sub-tile is one slab group, and it lies wholly inside the instance's
+        // slice (its rows are below max_update <= capacity): a group shared by two instances is neither read nor stored.
+        // P.life_floor is NULL when the slab uses no floors. Any other tile loads whole records, as without floors.
+        const bool floors = P.life_floor != nullptr && tile_known && (base_particle & 31u) == 0u;  // warp-uniform
+#endif
 #pragma unroll 1
         for (u32 j = 0; j < chunks; ++j) {
             u32 pidx[HNB_TILE_K];
             bool valid[HNB_TILE_K];
             RawParticle raw[HNB_TILE_K];
+#if HNB_LIFE_FLOOR
+            // lane k < HNB_TILE_K holds the floor of the sub-tile's row group k: one coalesced load
+            const u32 g_first = ((base_particle + row0) >> 5u) + j * HNB_TILE_K;  // slab group of row group 0
+            const u32 my_floor = floors && lane < HNB_TILE_K ? __float_as_uint(P.life_floor[g_first + lane]) : HNB_LIFE_FLOOR_NONE;
+#endif
             // gather the particle records (all loads in flight before any use)
 #if HNB_SLOT_ORDER
 #pragma unroll
@@ -688,7 +711,14 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
                 pidx[k] = pidx_next[k];
                 pidx_stash[j * HNB_TILE_K + k][lane] = pidx[k];
                 valid[k] = row < max_update;
+#if HNB_LIFE_FLOOR
+                if (valid[k]) {
+                    hnb_load_raw_but_life(raw[k], P.slab, base_particle + pidx[k]);
+                    if (!floors) hnb_load_life(raw[k], P.slab, base_particle + pidx[k]);  // (with floors: below)
+                }
+#else
                 if (valid[k]) hnb_load_raw(raw[k], P.slab, base_particle + pidx[k]);
+#endif
                 else hnb_raw_zero(raw[k]);
             }
             // prefetch the alive-list entries of the next sub-tile (coalesced u32)
@@ -709,6 +739,35 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
 #pragma unroll
             for (int k = 0; k < HNB_TILE_K; ++k) {
                 bool alive = false;
+#if HNB_LIFE_FLOOR
+                if (floors) {
+                    // The floor F of a group is at most the lifetime of each of its particles, so `age < F && age + dt < F`
+                    // (the fp32 sums the age code computes) proves `age < lifetime` both times the body compares them. A proven
+                    // row takes F as its lifetime: every use of it is one of those comparisons (HNB_ATTR_REAP_ONLY), and the
+                    // lifetime column is never stored. Any other row loads its lifetime here. A NaN on either side proves
+                    // nothing. (Deciding every row of the sub-tile before the first body, to issue these loads together,
+                    // costs registers that hnb_update does not have at 3 CTAs per SM.)
+                    const f32 F = __uint_as_float(__shfl_sync(0xffffffffu, my_floor, k));
+                    bool proven = false;
+                    if (valid[k]) {
+                        const f32 age = hnb_raw_age(raw[k]);
+                        proven = age < F && age + hnb_ctx.sim->delta_time < F;
+                        if (proven) hnb_raw_life(raw[k]) = F;
+                        else hnb_load_life(raw[k], P.slab, base_particle + pidx[k]);
+                    }
+                    // Every row (all are valid below trust_r) loaded its lifetime: store their minimum as the group's floor,
+                    // a NaN anywhere making it NaN (fminf would drop it).
+                    if (__ballot_sync(0xffffffffu, proven) == 0u) {
+                        f32 m = valid[k] ? hnb_raw_life(raw[k]) : __uint_as_float(0x7f800000u);
+#pragma unroll
+                        for (int d = 16; d > 0; d >>= 1) {
+                            const f32 o = __shfl_xor_sync(0xffffffffu, m, d);
+                            m = (m != m || m < o) ? m : o;
+                        }
+                        if (lane == 0) P.life_floor[g_first + k] = m;
+                    }
+                }
+#endif
                 if (valid[k]) {
                     Particle particle;
                     hnb_unpack(raw[k], particle);

@@ -139,6 +139,12 @@ struct BatchParams {
     // this batch's GpuBatchInfo words the kernels need (the host knows them when it launches: no dependent load for them)
     u32 bi_spawner_base, bi_prefix_sum_offset, bi_prefix_sum_count;
     u32 first_md_index, _pad1;       // effect_metadata_index of the batch's first instance (used when the batch has exactly one)          // 1: the host-written tables are stored by the kernel just ahead (k_frame_block): read them after the wait
+    // Lifetime floors of the slab (HNB_LIFE_FLOOR effects, DESIGN.md §3): one f32 per 32 slab rows, a lower bound of the
+    // lifetimes of the group's particles, or HNB_LIFE_FLOOR_NONE. NULL: the slab uses no floors. Kept out of SlabView so
+    // that the parameter offsets, and the code, of effects without floors stay as they were.
+    f32* life_floor;
 };
+// All bits set: a NaN, against which every comparison is false, so it proves nothing (0.0 would: ages can be negative).
+#define HNB_LIFE_FLOOR_NONE 0xffffffffu
 
 }  // namespace hnb

@@ -97,6 +97,11 @@ struct Slab {
     DeviceArray<uint32_t> ping, pong, dead;
     DeviceArray<uint32_t> alive_bits;  // one bit per row (HNB_EFFECT_SLOT_ORDER effects keep it current)
     DeviceArray<unsigned long long> ident_claim;  // [2]: identity claims of ping / pong (hnb_claim_pack)
+    // Lifetime floors (DESIGN.md §3): one f32 per 32 rows, HNB_LIFE_FLOOR_NONE (all bits set) until an update of an effect
+    // with floors stores one. Every other writer of records clears the groups it touches (clear_life_floors). `floors_off`:
+    // the update passes get no floors any more, because a view was handed out or a module without floors was bound.
+    DeviceArray<uint32_t> life_floor;
+    bool floors_off = false;
     // HNB_EFFECT_ORDERED_EVENTS scratch, allocated on first use: per channel the per-row event counts and their block sums
     DeviceArray<uint32_t> event_counts[HNB_MAX_EVENT_BINDINGS];
     DeviceArray<uint32_t> event_block_sums[HNB_MAX_EVENT_BINDINGS];
@@ -106,6 +111,7 @@ struct KernelModule {
     CUmodule mod = nullptr;
     CUfunction init = nullptr, update = nullptr;
     int update_blocks_per_sm = 1;
+    bool life_floor = false;  // generated with HNB_LIFE_FLOOR: keeps the slab's lifetime floors (and clears them on init)
     std::string log;
 };
 
@@ -388,6 +394,15 @@ hnb::PlaneSet plane_set(const std::vector<Plane>& planes, char* block, uint32_t 
 }
 hnb::PlaneSet plane_set(const Slab& s) { return plane_set(s.planes, s.d_block.get(), s.capacity); }
 
+// Sets the lifetime floors of every 32-row group that rows [first, first + count) touch to HNB_LIFE_FLOOR_NONE, in stream
+// order: for writers of records other than the update pass (DESIGN.md §3).
+void clear_life_floors(hnb_ctx* c, const Slab& s, uint32_t first, uint32_t count) {
+    if (count == 0) return;
+    const size_t g0 = first / 32u, g1 = (size_t(first) + count + 31u) / 32u;
+    CUDA_CHECK(cudaMemsetAsync(s.life_floor.get() + g0, 0xff, (g1 - g0) * sizeof(uint32_t), c->stream));
+}
+void clear_life_floors(hnb_ctx* c, const Slab& s) { clear_life_floors(c, s, 0, s.capacity); }
+
 // AoS records <-> columns go through a device staging buffer in chunks of this size.
 constexpr size_t kChunkBytes = size_t(64) << 20;
 
@@ -416,6 +431,7 @@ void fix_plan(hnb_ctx* c, Slab& s, const std::vector<Plane>& plan) {
         }
         CUDA_CHECK(cudaStreamSynchronize(c->stream));  // the old block and the staging buffer are released below
         s.d_block.swap(next);
+        clear_life_floors(c, s);
     }
     s.planes = plan;
     s.plan_fixed = true;
@@ -468,6 +484,7 @@ KernelModule* get_module(hnb_ctx* c, const std::string& source, const std::strin
     r = c->drv.ModuleGetFunction(&km->update, km->mod, "hnb_update");
     if (r != CUDA_SUCCESS) fail(HNB_ERR_CUDA, "cuModuleGetFunction(hnb_update): " + cu_error_string(c->drv, r));
     km->update_blocks_per_sm = 1;  // depends on the effect's dynamic shared memory (set_update_smem)
+    km->life_floor = source.find("\n#define HNB_LIFE_FLOOR 1\n") != std::string::npos;
     KernelModule* out = km.get();
     c->modules.emplace(hash, std::move(km));
     return out;
@@ -677,6 +694,10 @@ void bind_launch(hnb_ctx* c, LaunchPlan& lp, const hnb_batch_launch& bl, bool se
     P.properties_stride = fx.props_stride;
     P.slab = slab_view(slab);
     if (lp.parent) P.parent_slab = slab_view(*lp.parent);
+    // A module without floors neither keeps nor clears them, and it may write lifetimes: once one runs on the slab, no update
+    // reads a floor of it again.
+    if (!lp.km->life_floor) slab.floors_off = true;
+    P.life_floor = slab.floors_off ? nullptr : reinterpret_cast<float*>(slab.life_floor.get());
     if (consume) P.consume_events = c->event_buffers[bl.consume_events].get();
     for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
         if (bl.emit_events[i] == 0xFFFFFFFFu) continue;
@@ -974,6 +995,8 @@ int32_t hnb_slab_create_ex(hnb_ctx* c, uint32_t capacity_rows, uint32_t stride, 
         CUDA_CHECK(grow(s.alive_bits, size_t(capacity_rows) / 32 + 2, 0, c->stream));
         CUDA_CHECK(s.ident_claim.alloc(2));
         clear_ident_claims(c, s);
+        CUDA_CHECK(s.life_floor.alloc(size_t(capacity_rows) / 32 + 1));
+        clear_life_floors(c, s);
         CUDA_CHECK(hnb::launch_slab_reset(s.ping.get(), s.pong.get(), s.dead.get(), 0, capacity_rows, c->stream));
         c->launches++;
         s.live = true;
@@ -995,6 +1018,7 @@ int32_t hnb_slab_reset_rows(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t cou
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
         clear_ident_claims(c, s);
+        clear_life_floors(c, s, first, count);
         CUDA_CHECK(hnb::launch_slab_reset(s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
         CUDA_CHECK(hnb::launch_bits_range(s.alive_bits.get(), first, count, false, c->stream));
         c->launches += 2;
@@ -1006,6 +1030,7 @@ int32_t hnb_slab_rebuild_alive_bits(hnb_ctx* c, hnb_slab h, uint32_t first, uint
         Slab& s = get_slab(c, h);
         check_rows(s, first, rows);
         if (column > 1 || alive_count > rows) fail(HNB_ERR_INVALID_ARG, "bad alive-list column or count");
+        clear_life_floors(c, s, first, rows);  // slots may become alive whose lifetimes no floor covers
         CUDA_CHECK(hnb::launch_bits_range(s.alive_bits.get(), first, rows, false, c->stream));
         CUDA_CHECK(hnb::launch_bits_from_list(s.alive_bits.get(), (column ? s.pong : s.ping).get() + first, first, alive_count, c->stream));
         c->launches += rows ? 1 + (alive_count ? 1 : 0) : 0;
@@ -1020,6 +1045,7 @@ void transfer_aos(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, void* 
     check_rows(s, first, count);
     if (count == 0) return;
     s.written |= upload;
+    if (upload) clear_life_floors(c, s, first, count);
     const uint32_t rows_per_chunk = (uint32_t)std::max<size_t>(1, kChunkBytes / s.stride);
     DeviceArray<char> staging;
     CUDA_CHECK(staging.alloc(size_t(std::min(rows_per_chunk, count)) * s.stride));
@@ -1059,6 +1085,7 @@ int32_t hnb_slab_upload_indirect(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_
         CUDA_CHECK(stage.alloc(size_t(count) * 3));
         CUDA_CHECK(cudaMemcpyAsync(stage.get(), rows, size_t(count) * 12, cudaMemcpyHostToDevice, c->stream));
         clear_ident_claims(c, s);
+        clear_life_floors(c, s, first, count);
         CUDA_CHECK(hnb::launch_indirect_deinterleave(stage.get(), s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
         c->launches++;
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
@@ -1099,6 +1126,7 @@ int32_t hnb_slab_import_aos_device(hnb_ctx* c, hnb_slab h, uint32_t first, uint3
         if (count && !d_src) fail(HNB_ERR_INVALID_ARG, "d_src is NULL");
         if ((uintptr_t)d_src & 3u) fail(HNB_ERR_INVALID_ARG, "d_src must be 4-byte aligned (16-byte aligned for full speed)");
         s.written = true;
+        clear_life_floors(c, s, first, count);
         CUDA_CHECK(hnb::launch_aos_to_planes((const uint32_t*)d_src, plane_set(s), first, count, s.stride / 4, c->stream));
         c->launches += count ? 1 : 0;
     });
@@ -1118,6 +1146,7 @@ int32_t hnb_slab_import_indirect_device(hnb_ctx* c, hnb_slab h, uint32_t first, 
         check_rows(s, first, count);
         if (count && !d_src) fail(HNB_ERR_INVALID_ARG, "d_src is NULL");
         clear_ident_claims(c, s);
+        clear_life_floors(c, s, first, count);
         CUDA_CHECK(hnb::launch_indirect_deinterleave((const uint32_t*)d_src, s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
         c->launches += count ? 1 : 0;
     });
@@ -1127,6 +1156,7 @@ int32_t hnb_slab_device_view(hnb_ctx* c, hnb_slab h, hnb_slab_view* out) {
         Slab& s = get_slab(c, h);
         if (!out) fail(HNB_ERR_INVALID_ARG, "out is NULL");
         fix_default_plan(c, s);  // handed-out columns never move: an unbound slab keeps the default cut from now on
+        s.floors_off = true;     // records written through the view would not clear the floors
         memset(out, 0, sizeof(*out));
         out->capacity_rows = s.capacity;
         out->particle_stride = s.stride;
@@ -1179,6 +1209,7 @@ int32_t hnb_slab_fill_c5_ex(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t cou
         if (s.stride != 32) fail(HNB_ERR_LAYOUT, "hnb_slab_fill_c5 needs the 32-byte {position,age,velocity,lifetime} layout");
         if (s.sector_planes) fail(HNB_ERR_LAYOUT, "hnb_slab_fill_c5 writes the default or a column plan; spawn through the init pass or use hnb_slab_upload_aos");
         s.written = true;
+        clear_life_floors(c, s, first, count);
         CUDA_CHECK(hnb::launch_fill_c5(plane_set(s), s.ping.get(), s.pong.get(), s.ident_claim.get(), first, count, seed, lo, hi,
                                        logical_first, c->stream));
         CUDA_CHECK(hnb::launch_bits_range(s.alive_bits.get(), first, count, true, c->stream));
@@ -1275,6 +1306,7 @@ int32_t slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row,
         fix_plan(c, s, fx.plan);
         CUDA_CHECK(cudaSetDevice(c->device));
         const hnb::RepackArgs a = repack_args(c, s, metadata_row, first, rows);
+        clear_life_floors(c, s, first, rows);
         uint32_t widest = 0;
         for (const Plane& p : s.planes) widest = std::max(widest, p.width);
         void* scratch = nullptr;
@@ -1359,6 +1391,7 @@ int32_t instance_restore(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata
         CUDA_CHECK(cudaSetDevice(c->device));
         fix_plan(c, s, fx.plan);
         s.written = true;
+        clear_life_floors(c, s, first, rows);
         hnb::SnapshotArgs a = snapshot_args(c, s, metadata_row, first, rows);
         a.src_bytes = src_bytes;
         const hnb::EventChannels ev = emit ? event_channels(c, fx, emit) : hnb::EventChannels{};

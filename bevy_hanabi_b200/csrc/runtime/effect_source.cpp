@@ -263,6 +263,50 @@ bool has_attr(const hnb_effect_desc& d, const char* name) {
 
 const char* nz(const char* s) { return s ? s : ""; }
 
+const hnb_attr_layout* find_attr(const hnb_effect_desc& d, const char* name) {
+    for (uint32_t i = 0; i < d.n_attrs; ++i)
+        if (!strcmp(d.attrs[i].name, name)) return &d.attrs[i];
+    return nullptr;
+}
+
+// Lifetime floors (DESIGN.md §3): the column of `planes` that holds the lifetime and nothing else, when the update pass of
+// this effect may prove particles alive from a floor instead of loading it; -1 otherwise. That needs an f32 lifetime flagged
+// HNB_ATTR_REAP_ONLY and read-only (so the column is never stored and only the standard age / reap code compares it), an f32
+// age, and the ordered pass (the floor is kept per 32 rows of an identity-claimed tile). Slot order keeps none: there
+// inits clear the floors of many groups every frame, and the lifetime loads those groups then need, issued behind the
+// age, cost more than the floors save.
+int life_floor_plane(const hnb_effect_desc& d, const std::vector<Plane>& planes, bool sector) {
+    if (sector || (d.flags & (HNB_EFFECT_RELAXED_ORDER | HNB_EFFECT_SLOT_ORDER))) return -1;
+    const hnb_attr_layout* life = find_attr(d, "lifetime");
+    const hnb_attr_layout* age = find_attr(d, "age");
+    const uint32_t need = HNB_ATTR_UPDATE_READ_ONLY | HNB_ATTR_REAP_ONLY;
+    if (!life || !age || life->value_type != HNB_FLOAT || age->value_type != HNB_FLOAT || (life->flags & need) != need) return -1;
+    for (size_t p = 0; p < planes.size(); ++p)
+        if (planes[p].offset == life->offset && planes[p].width == 4) return int(p);
+    return -1;
+}
+
+// The accessors hnb_update uses with HNB_LIFE_FLOOR: every column load but the lifetime's, the lifetime load, the age word
+// and the lifetime word of a RawParticle.
+void gen_life_floor_code(std::ostringstream& o, const hnb_effect_desc& d, const std::vector<Plane>& planes, int life_plane) {
+    const uint32_t age_off = find_attr(d, "age")->offset;
+    size_t age_plane = 0;
+    while (!(planes[age_plane].offset <= age_off && age_off < planes[age_plane].offset + planes[age_plane].width)) ++age_plane;
+    o << "#define HNB_LIFE_FLOOR 1\n";
+    o << "HNB_DI void hnb_load_raw_but_life(RawParticle& r, const SlabView& s, u32 row) {\n";
+    for (size_t p = 0; p < planes.size(); ++p) {
+        if (int(p) == life_plane) continue;
+        const char* t = planes[p].width == 16 ? "float4" : planes[p].width == 8 ? "float2" : "f32";
+        o << "    r.q" << p << " = HNB_LOAD_PLANE(" << t << ", s.planes[" << p << "], row);\n";
+    }
+    o << "}\n";
+    o << "HNB_DI void hnb_load_life(RawParticle& r, const SlabView& s, u32 row) { r.q" << life_plane << " = HNB_LOAD_PLANE(f32, s.planes["
+      << life_plane << "], row); }\n";
+    o << "HNB_DI f32 hnb_raw_age(const RawParticle& r) { return "
+      << raw_word(planes[age_plane], age_plane, (age_off - planes[age_plane].offset) / 4) << "; }\n";
+    o << "HNB_DI f32& hnb_raw_life(RawParticle& r) { return r.q" << life_plane << "; }\n";
+}
+
 }  // namespace
 
 uint32_t rows_per_lane() {
@@ -371,6 +415,7 @@ std::string generate_effect_source(const hnb_effect_desc& d, const std::vector<P
          "#endif\n";
     // {{ATTRIBUTES}} / {{PROPERTIES}} / {{PARENT_ATTRIBUTES}}
     gen_layout_code(o, "", "Particle", d.attrs, d.n_attrs, d.particle_stride, planes, true, sector);
+    if (const int life_plane = life_floor_plane(d, planes, sector); life_plane >= 0) gen_life_floor_code(o, d, planes, life_plane);
     // a parent slab is read in the default cut (emitting effects keep it: column_plan), or in the plan its first bound
     // effect gave it
     if (read_parent)

@@ -395,7 +395,10 @@ typedef struct hnb_slab_view {
  * generated for that cut. Take the view after the first hnb_simulate that binds the slab to see the effect's own plan.
  * Writing the index columns (ping / pong) through it is not supported: the update pass may
  * skip alive-list loads and stores where it knows a column to be the identity, and a write through the view does not
- * drop that knowledge. Use hnb_slab_import_indirect_device or hnb_slab_upload_indirect to change the lists. */
+ * drop that knowledge. Use hnb_slab_import_indirect_device or hnb_slab_upload_indirect to change the lists.
+ * The same holds for records: the update pass of an effect with HNB_ATTR_REAP_ONLY keeps a lifetime floor per 32 rows,
+ * and every call of this API that writes records clears the floors it covers. A write through the view would not, so a
+ * slab whose view has been handed out stops using floors for good. */
 HNB_API int32_t hnb_slab_device_view(hnb_ctx* ctx, hnb_slab slab, hnb_slab_view* out);
 /** Rows [first,first+count) as AoS records into `d_dst` (count * particle_stride bytes). */
 HNB_API int32_t hnb_slab_export_aos_device(hnb_ctx* ctx, hnb_slab slab, uint32_t first, uint32_t count, void* d_dst);
@@ -444,6 +447,15 @@ typedef struct hnb_attr_layout {
  * (hnb_asset_generate) sets the flag from the code it emits. Ignored for parent layouts.
  */
 enum { HNB_ATTR_UPDATE_READ_ONLY = 1u << 0 };
+/**
+ * HNB_ATTR_REAP_ONLY (on "lifetime" only, together with HNB_ATTR_UPDATE_READ_ONLY): the update reads the lifetime only in
+ * the standard age and reap code (`was_alive = age < lifetime; age = age + delta_time; is_alive = age < lifetime`), no
+ * other code of the update body (update code, UPDATE_EXTRA) reads it and nothing else writes AGE. When, in addition, the
+ * lifetime sits in a 4-byte column of its own, the update pass keeps a lifetime floor per 32 slab rows and skips the
+ * lifetime load of every particle the floor proves alive this frame (DESIGN.md §3). The results are bit-identical
+ * either way. The graph lowering sets the flag; hand-written descriptors that set it must honour the conditions.
+ */
+enum { HNB_ATTR_REAP_ONLY = 1u << 1 };
 
 enum {
     HNB_EFFECT_LOCAL_SPACE = 1u << 0,          /* LayoutFlags::LOCAL_SPACE_SIMULATION */
