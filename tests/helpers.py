@@ -404,15 +404,16 @@ class Lockstep:
     """A GpuWorld and the oracle world it must equal, stepped frame by frame and compared after every frame.
 
     `asset`: an authored effect, stepped by the numpy interpreter with the per-instance property records `props`. Without
-    it the world runs C5 (recipes.c5_lowered) under the C oracle's update body with ACCEL_DRAG; `init` adds the constant
-    init of c5_init(). `relaxed`: lists and dead stacks are compared as sets, then the oracle adopts the device's lists
+    it the world runs C5 under the C oracle's update body with ACCEL_DRAG, on the device the hand-lowered recipes.c5_lowered
+    or `effect`, an already compiled C5 module (the authored recipes.c5_asset); `init` adds the constant init of c5_init().
+    `relaxed`: lists and dead stacks are compared as sets, then the oracle adopts the device's lists
     (the next frame reads them in the order the device wrote them). `rtol`: fp32 attributes within `rtol` of their
     magnitude, and the device restarts every compared frame from the oracle's records (the bound is a per-step bound:
     libm-level differences are amplified from frame to frame by non-smooth dynamics). `seeds(n, f)`: the spawner seeds of
     frame f, or None to keep them."""
 
     def __init__(self, ctx, orc, ref, asset=None, *, props=None, init=False, sector=False, slot=False, relaxed=False,
-                 fast_math=False, rtol=0.0, seeds=None):
+                 fast_math=False, rtol=0.0, seeds=None, effect=None):
         from bevy_hanabi_b200 import recipes
         from oracle.hanabi_oracle import EffectOracle
         from tests.effects import ACCEL_DRAG, c5_init
@@ -436,7 +437,7 @@ class Lockstep:
             self.eo = EffectOracle(asset, dict(enumerate(props)) if props else None)
             lowered = asset.generate(sector_planes=sector, slot_order=slot, relaxed_order=relaxed, fast_math=fast_math)
             self.mask, self.float_attrs = float_word_mask(asset)
-        self.gpu = GpuWorld(ctx, ref, lowered, property_blobs=blobs, sector_planes=sector)
+        self.gpu = GpuWorld(ctx, ref, lowered, property_blobs=blobs, sector_planes=sector, effect=effect)
 
     def step(self, f, spawns=None):
         """Frame `f` on both sides, without a comparison. `spawns`: per instance, or None to keep the spawn counts."""
@@ -533,10 +534,11 @@ def table_world(name, caps, batches=None, align=1, dead_perm_seed=None):
     return ref
 
 
-def filled_c5(ctx, orc, insts, fills, batches=None, dead_perm_seed=None, parities=None):
+def filled_c5(ctx, orc, insts, fills, batches=None, dead_perm_seed=None, parities=None, effect=None):
     """A Lockstep of C5 with its init over `insts`. `fills`: (first, count, seed, lifetime_lo, lifetime_hi) ranges filled
     by hnb_slab_fill_c5 on the device and orc_fill_c5 in the oracle, after the world was uploaded; the last fill holds the
-    claim. `parities`: the alive-list column each instance's first frame appends to (metadata indirect_write_index)."""
+    claim. `parities`: the alive-list column each instance's first frame appends to (metadata indirect_write_index).
+    `effect`: the compiled C5 module the device runs (Lockstep's)."""
     ref = RefWorld(sum(i.capacity for i in insts), 8, insts, batches=batches)
     for i, parity in enumerate(parities or []):
         ref.metadata[i].indirect_write_index = parity
@@ -545,7 +547,7 @@ def filled_c5(ctx, orc, insts, fills, batches=None, dead_perm_seed=None, paritie
         for inst in insts:
             rows = slice(inst.slab_offset + inst.alive, inst.slab_offset + inst.capacity)
             ref.indirect[rows, 2] = rng.permutation(ref.indirect[rows, 2])
-    lock = Lockstep(ctx, orc, ref, init=True)
+    lock = Lockstep(ctx, orc, ref, init=True, effect=effect)
     for first, count, seed, lo, hi in fills:
         orc.orc_fill_c5(O.ptr(ref.particles), O.ptr(ref.indirect), first, count, seed, lo, hi)
         ctx.slab_fill_c5(lock.gpu.slab, first, count, seed, lo, hi)
