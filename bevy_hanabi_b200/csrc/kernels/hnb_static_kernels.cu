@@ -894,6 +894,153 @@ __global__ void __launch_bounds__(EV_THREADS) k_restore_events(SnapshotArgs a, c
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Bounds of every instance of a batch (hnb_batch_bounds): a pure read of the `position` column(s). One persistent launch
+// reduces all instances, one small launch writes the records.
+//
+// Floats are compared through the usual order-preserving key (bounds_key), so -0 < +0, the infinities take part and the
+// result is the same whatever the order of the reduction. A NaN is skipped. Every partial result is kept as a MAXIMUM:
+// `hi` of the keys and `lo` of the inverted keys. No float has key 0 or 0xFFFFFFFF (those bit patterns are NaNs), so 0
+// means "no value" in both, and an accumulator of zeroes is the reset state.
+// ---------------------------------------------------------------------------------------------
+#define BD_THREADS 256
+#define BD_ITEMS 4  // rows per thread in flight (as RP_ITEMS)
+#define BD_TILE (BD_THREADS * BD_ITEMS)
+
+__device__ __forceinline__ u32 bounds_key(u32 bits) { return bits ^ ((bits >> 31u) ? 0xFFFFFFFFu : 0x80000000u); }
+__device__ __forceinline__ u32 bounds_bits(u32 key) { return key ^ ((key >> 31u) ? 0x80000000u : 0xFFFFFFFFu); }
+
+struct BoundsAcc { u32 lo[3], hi[3]; };
+__device__ __forceinline__ void bounds_take(BoundsAcc& r, int c, u32 bits) {
+    if ((bits & 0x7FFFFFFFu) > 0x7F800000u) return;  // NaN
+    const u32 k = bounds_key(bits);
+    r.lo[c] = max(r.lo[c], ~k);
+    r.hi[c] = max(r.hi[c], k);
+}
+
+// Instance j of the batch as the device tables of the last simulated frame describe it, every word clamped: the spawner
+// and metadata rows to their tables, the slice to the slab, n = min(alive_count, rows) as hnb_instance_snapshot defines it.
+struct BoundsInstance { u32 first, rows, n, w; };
+__device__ __forceinline__ u32 bounds_count(const BoundsArgs& a) { return min(a.batch_info->prefix_sum_count, a.max_instances); }
+__device__ __forceinline__ BoundsInstance bounds_instance(const BoundsArgs& a, u32 j) {
+    const u64 row = u64(a.batch_info->spawner_base) + j;
+    const Spawner* sp = &a.spawners[row < a.num_spawners ? row : a.num_spawners - 1u];
+    const EffectMetadata* md = &a.metadata[min(sp->effect_metadata_index, a.num_metadata - 1u)];
+    BoundsInstance b;
+    b.first = min(sp->slab_offset, a.capacity_rows);
+    b.rows = min(md->capacity, a.capacity_rows - b.first);
+    b.n = min(md->alive_count, b.rows);
+    b.w = md->indirect_write_index == 0u ? 0u : 1u;
+    return b;
+}
+
+// Persistent grid. Every CTA walks the instances (their descriptions staged BD_THREADS at a time in shared memory, so the
+// dependent table loads of 1024 instances cost four rounds, not 1024) and takes the tiles t with t + j = blockIdx (mod
+// gridDim) of instance j: one 64 Mi-row instance and 1024 instances of 64 tiles both spread evenly, with no prefix of
+// counts the host would have to know. Rows below the identity claim of column W take pidx = i without a list load; the
+// slab's two claim words are read once per thread, they do not change under the kernel.
+// FAST: position's three words sit in one 16-byte column, or in one half of a 32-byte sector-plane column: one 16-byte
+// load per row. Otherwise one 4-byte load per word from whatever columns the plan gave them.
+// Per (warp, instance) that had a tile: registers -> shuffles -> six atomicMax into the accumulator by lanes 0-5. The
+// warps of a CTA never wait for one another inside a staging round, so one warp's gather overlaps another's reduction.
+template <bool FAST>
+__global__ void __launch_bounds__(BD_THREADS) k_bounds_reduce(BoundsArgs a) {
+    __shared__ u32 s_first[BD_THREADS], s_rows[BD_THREADS], s_n[BD_THREADS], s_w[BD_THREADS];
+    const u32 count = bounds_count(a);
+    const u32 tid = threadIdx.x, lane = tid & 31u, G = gridDim.x;
+    const u64 claim0 = hnb_claim_load(&a.claim[0]), claim1 = hnb_claim_load(&a.claim[1]);
+    u32 rot = 0u;  // j mod G of the instance at hand
+    for (u32 chunk = 0; chunk < count; chunk += BD_THREADS) {
+        __syncthreads();
+        if (chunk + tid < count) {
+            const BoundsInstance b = bounds_instance(a, chunk + tid);
+            s_first[tid] = b.first; s_rows[tid] = b.rows; s_n[tid] = b.n; s_w[tid] = b.w;
+        }
+        __syncthreads();
+        const u32 staged = min(count - chunk, u32(BD_THREADS));
+        for (u32 jj = 0; jj < staged; ++jj, rot = rot + 1u == G ? 0u : rot + 1u) {
+            const u32 n = s_n[jj], tiles = (n + BD_TILE - 1u) / BD_TILE;
+            u32 t = blockIdx.x >= rot ? blockIdx.x - rot : blockIdx.x + G - rot;
+            if (t >= tiles) continue;
+            const u32 first = s_first[jj], last_row = s_rows[jj] - 1u, w = s_w[jj];
+            const u32* list = (w == 0u ? a.ping : a.pong) + first;
+            const u32 claimed = min(hnb_claim_len(w == 0u ? claim0 : claim1, first), n);
+            BoundsAcc r = {{0u, 0u, 0u}, {0u, 0u, 0u}};
+            for (; t < tiles; t += G) {
+                const u32 i0 = t * BD_TILE + tid;
+                u32 p[BD_ITEMS];
+#pragma unroll
+                for (u32 k = 0; k < BD_ITEMS; ++k) {
+                    const u32 i = i0 + k * BD_THREADS;
+                    p[k] = i < claimed ? i : (i < n ? min(list[i], last_row) : 0u);
+                }
+                if (FAST) {
+                    const RepackPiece<4>* col = (const RepackPiece<4>*)a.col[0];
+                    const u32 quads = a.col_words[0] >> 2u, quad = a.col_lane[0] >> 2u;
+                    RepackPiece<4> v[BD_ITEMS];
+#pragma unroll
+                    for (u32 k = 0; k < BD_ITEMS; ++k)
+                        if (i0 + k * BD_THREADS < n) v[k] = col[(u64(first) + p[k]) * quads + quad];
+#pragma unroll
+                    for (u32 k = 0; k < BD_ITEMS; ++k) {
+                        if (i0 + k * BD_THREADS >= n) continue;
+#pragma unroll
+                        for (int c = 0; c < 3; ++c) bounds_take(r, c, v[k].w[c]);
+                    }
+                } else {
+                    u32 v[BD_ITEMS][3];
+#pragma unroll
+                    for (u32 k = 0; k < BD_ITEMS; ++k) {
+                        if (i0 + k * BD_THREADS >= n) continue;
+#pragma unroll
+                        for (int c = 0; c < 3; ++c) v[k][c] = a.col[c][(u64(first) + p[k]) * a.col_words[c] + a.col_lane[c]];
+                    }
+#pragma unroll
+                    for (u32 k = 0; k < BD_ITEMS; ++k) {
+                        if (i0 + k * BD_THREADS >= n) continue;
+#pragma unroll
+                        for (int c = 0; c < 3; ++c) bounds_take(r, c, v[k][c]);
+                    }
+                }
+            }
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+#pragma unroll
+                for (int d = 16; d > 0; d >>= 1) {
+                    r.lo[c] = max(r.lo[c], __shfl_xor_sync(0xffffffffu, r.lo[c], d));
+                    r.hi[c] = max(r.hi[c], __shfl_xor_sync(0xffffffffu, r.hi[c], d));
+                }
+            }
+            // every lane holds the warp's six maxima: lane s < 6 publishes slot s (0: a warp whose rows had no value)
+            const u32 m = lane == 0u ? r.lo[0] : lane == 1u ? r.lo[1] : lane == 2u ? r.lo[2] : lane == 3u ? r.hi[0] : lane == 4u ? r.hi[1] : r.hi[2];
+            if (lane < 6u && m) atomicMax(&a.acc[u64(chunk + jj) * 8u + (lane < 3u ? lane : lane + 1u)], u64(m));
+        }
+    }
+}
+
+// Record j of every instance the call covers (those past the batch's device-side count get an empty one), and the
+// accumulator back to zeroes for the next call.
+__global__ void __launch_bounds__(BD_THREADS) k_bounds_write(BoundsArgs a) {
+    const u32 j = blockIdx.x * BD_THREADS + threadIdx.x;
+    if (j >= a.max_instances) return;
+    const u32 n = j < bounds_count(a) ? bounds_instance(a, j).n : 0u;
+    u64* acc = a.acc + u64(j) * 8u;
+    RepackPiece<4> lo, hi;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const u32 l = u32(acc[c]), h = u32(acc[4 + c]);
+        lo.w[c] = l ? bounds_bits(~l) : 0x7F800000u;  // +inf: no value
+        hi.w[c] = h ? bounds_bits(h) : 0xFF800000u;   // -inf
+        acc[c] = 0ull;
+        acc[4 + c] = 0ull;
+    }
+    lo.w[3] = n;
+    hi.w[3] = 0u;
+    RepackPiece<4>* out = (RepackPiece<4>*)a.out + u64(j) * 2u;
+    out[0] = lo;
+    out[1] = hi;
+}
+
 // Effective SM clock: cycles elapsed on one SM over ~`window_ns` of the global timer.
 __global__ void k_measure_sm_clock(u64* out, u64 window_ns) {
     u64 t0, t1;
@@ -1068,6 +1215,31 @@ cudaError_t launch_events_translate(const RepackArgs& a, const u32* inv, const E
 cudaError_t launch_restore_events(const SnapshotArgs& a, const u32* src, const EventChannels& ev, cudaStream_t st) {
     if (a.rows == 0 || ev.count == 0) return cudaSuccess;
     k_restore_events<<<ev.count, EV_THREADS, 0, st>>>(a, src, ev);
+    return cudaGetLastError();
+}
+// CTAs of k_bounds_reduce<FAST> that one SM holds
+template <bool FAST> static cudaError_t bounds_blocks_per_sm(int* out) {
+    static int cached = 0;
+    if (cached == 0) {
+        int n = 0;
+        const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_bounds_reduce<FAST>, BD_THREADS, 0);
+        if (e != cudaSuccess) return e;
+        cached = std::max(n, 1);
+    }
+    *out = cached;
+    return cudaSuccess;
+}
+cudaError_t launch_batch_bounds(const BoundsArgs& a, bool fast, u32 sm_count, cudaStream_t st) {
+    if (a.max_instances == 0) return cudaSuccess;
+    int per_sm = 1;
+    const cudaError_t e = fast ? bounds_blocks_per_sm<true>(&per_sm) : bounds_blocks_per_sm<false>(&per_sm);
+    if (e != cudaSuccess) return e;
+    // no more CTAs than the slab can have tiles: a small batch is a small launch
+    const u64 max_tiles = u64(a.capacity_rows) / BD_TILE + a.max_instances;
+    const unsigned grid = (unsigned)std::min<u64>(max_tiles, u64(sm_count) * u64(per_sm));
+    if (fast) k_bounds_reduce<true><<<grid, BD_THREADS, 0, st>>>(a);
+    else k_bounds_reduce<false><<<grid, BD_THREADS, 0, st>>>(a);
+    k_bounds_write<<<blocks_for(a.max_instances, BD_THREADS), BD_THREADS, 0, st>>>(a);
     return cudaGetLastError();
 }
 cudaError_t launch_measure_sm_clock(u64* out2, u64 window_ns, cudaStream_t st) {

@@ -127,6 +127,33 @@ cudaError_t launch_events_translate(const RepackArgs& a, const u32* inv, const E
 // the events of a version-2 snapshot into the channels' buffers and event counts; after launch_restore_scatter
 cudaError_t launch_restore_events(const SnapshotArgs& a, const u32* src, const EventChannels& ev, cudaStream_t st);
 
+// Bounds of every instance of one batch (hnb_batch_bounds): per component of `position`, the minimum and maximum over the
+// instance's live particles in the total order of bounds_key. Everything about the instances is read on the device; the
+// host only names the batch's row, the slab's columns and where `position` sits in them.
+struct BoundsArgs {
+    const BatchInfo* batch_info;     // the batch's row of the device frame block (spawner_base, prefix_sum_count)
+    const Spawner* spawners;         // device spawner table, `num_spawners` rows
+    const EffectMetadata* metadata;  // device metadata table, `num_metadata` rows
+    u32 num_spawners, num_metadata;
+    const u32* ping;                 // alive-list columns of the slab (row 0)
+    const u32* pong;
+    const u64* claim;                // [2]: the slab's identity claims, only read
+    u32 capacity_rows;               // rows of the slab
+    u32 max_instances;               // records `out` and `acc` hold for this call
+    // Word c of `position` is word col_lane[c] of the col_words[c]-word elements of column col[c] (row 0 of the slab).
+    // The fast kernel needs the three words in one column at a 16-byte boundary: col[0], col_words[0] and col_lane[0].
+    const u32* col[3];
+    u32 col_words[3], col_lane[3];
+    // 8 slots per instance, all zero between calls: max(~key) of x y z, -, max(key) of x y z, -. A slot is a 64-bit word
+    // with the 32-bit key in its low half: 64 bits is the atomicMax width the project's kernels and their CPU emulation use.
+    u64* acc;
+    void* out;                       // hnb_instance_bounds records (32 bytes each, 16-byte aligned)
+};
+// One persistent launch that reduces every instance into `acc`, then one that writes the records and zeroes `acc` again.
+// `fast`: position's three words share one 16- or 32-byte column. `sm_count`: SMs of the device.
+cudaError_t launch_batch_bounds(const BoundsArgs& a, bool fast, u32 sm_count, cudaStream_t st);
+#define HNB_BATCH_BOUNDS_LAUNCHES 2u
+
 cudaError_t launch_indirect(const StaticTables& T, u32 num_effects, cudaStream_t st);
 cudaError_t launch_prefix_sum(const StaticTables& T, u32 num_batches, cudaStream_t st);
 cudaError_t launch_tile_prefix(const StaticTables& T, u32 batch_index, u32 tile, cudaStream_t st);

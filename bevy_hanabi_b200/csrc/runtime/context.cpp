@@ -259,6 +259,7 @@ struct hnb_ctx {
     uint32_t mailbox_rows = 0, mailbox_ring = 0;
     bool plan_dirty = false;  // bind_launch changed a tile-size or range word of the host frame block since the last upload
     uint64_t frame_copies = 0, frames = 0;  // hnb_simulate calls that needed the host->device copy of the frame block / all calls
+    DeviceArray<unsigned long long> d_bounds_acc;  // hnb_batch_bounds: 8 slots per instance of the largest batch seen, zero between calls
     DeviceArray<unsigned long long> d_debug;  // 16 diagnostic counters + a 64-frame timeline ring of 4 words (HNB_PROFILE kernels)
 
     hnb::FrameHeader* header() { return reinterpret_cast<hnb::FrameHeader*>(h_arena.get()); }
@@ -1867,6 +1868,63 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
             for (auto& lp : plans)
                 if (lp.fx->flags & HNB_EFFECT_RIBBONS) launch_ribbon_sort(c, lp);
         }
+    });
+}
+
+static_assert(sizeof(hnb_instance_bounds) == 32, "hnb_instance_bounds is two 16-byte stores");
+
+// Everything is checked on the host before anything is enqueued; what the instances look like (counts, W, slab offsets,
+// metadata rows) is read by the kernels from the device tables of the last simulated frame, clamped there.
+int32_t hnb_batch_bounds(hnb_ctx* c, const hnb_batch_launch* b, hnb_instance_bounds* d_out, uint32_t out_rows) {
+    return guarded([&] {
+        const std::string w = "hnb_batch_bounds";
+        if (!b) fail(HNB_ERR_INVALID_ARG, w + ": batch is NULL");
+        const Slab& s = get_slab(c, b->slab);
+        const Effect& fx = get_effect(c, b->effect);
+        if (b->batch_info_index >= c->B) fail(HNB_ERR_INVALID_ARG, w + ": batch_info_index is not an uploaded batch row");
+        const hnb_batch_info& bi = c->h_at<hnb_batch_info>(c->lay.off_batch_infos)[b->batch_info_index];
+        if (uint64_t(bi.spawner_base) + bi.prefix_sum_count > c->E)
+            fail(HNB_ERR_INVALID_ARG, w + ": the batch references instances outside the uploaded spawner table");
+        if (fx.particle_stride != s.stride) fail(HNB_ERR_INVALID_ARG, w + ": effect particle stride does not match the slab");
+        if (((fx.flags & HNB_EFFECT_SECTOR_PLANES) != 0) != s.sector_planes)
+            fail(HNB_ERR_INVALID_ARG, w + ": effect and slab disagree on HNB_EFFECT_SECTOR_PLANES / HNB_SLAB_SECTOR_PLANES");
+        const hnb_attr_layout* position = nullptr;
+        for (const hnb_attr_layout& a : fx.desc->attrs)
+            if (a.name && std::string(a.name) == "position") position = &a;
+        if (!position || position->value_type != HNB_VEC3 || (position->offset & 3u) || uint64_t(position->offset) + 12 > s.stride)
+            fail(HNB_ERR_INVALID_ARG, w + ": the effect has no `position` attribute of type HNB_VEC3 inside its record");
+        if (!d_out || ((uintptr_t)d_out & 15u)) fail(HNB_ERR_INVALID_ARG, w + ": d_out is NULL or not 16-byte aligned");
+        if (out_rows < bi.prefix_sum_count) fail(HNB_ERR_INVALID_ARG, w + ": out_rows is below the batch's instance count");
+        if (bi.prefix_sum_count == 0) return;
+        if (c->d_metadata.size() == 0) fail(HNB_ERR_INVALID_ARG, w + ": no metadata row was inserted");
+        CUDA_CHECK(cudaSetDevice(c->device));
+        if (c->d_bounds_acc.size() < size_t(bi.prefix_sum_count) * 8)
+            CUDA_CHECK(grow(c->d_bounds_acc, std::max<size_t>(bi.prefix_sum_count, c->d_metadata.size()) * 8, 0, c->stream));
+
+        hnb::BoundsArgs a{};
+        a.batch_info = c->d_at<hnb::BatchInfo>(c->lay.off_batch_infos) + b->batch_info_index;
+        a.spawners = c->d_at<hnb::Spawner>(c->lay.off_spawners);
+        a.metadata = c->d_metadata.get();
+        a.num_spawners = c->E;
+        a.num_metadata = uint32_t(c->d_metadata.size());
+        a.ping = s.ping.get();
+        a.pong = s.pong.get();
+        a.claim = s.ident_claim.get();
+        a.capacity_rows = s.capacity;
+        a.max_instances = bi.prefix_sum_count;
+        // position in the slab's CURRENT columns: a plan may cut its three words apart
+        const hnb::PlaneSet ps = plane_set(s);
+        for (uint32_t k = 0; k < 3; ++k) {
+            const uint32_t word = position->offset / 4 + k, p = ps.word_to_plane[word];
+            a.col[k] = static_cast<const uint32_t*>(ps.ptr[p]);
+            a.col_words[k] = ps.words[p];
+            a.col_lane[k] = word - ps.word_off[p];
+        }
+        const bool fast = a.col[2] == a.col[0] && (a.col_lane[0] & 3u) == 0 && (a.col_words[0] & 3u) == 0;
+        a.acc = c->d_bounds_acc.get();
+        a.out = d_out;
+        CUDA_CHECK(hnb::launch_batch_bounds(a, fast, uint32_t(c->sm_count), c->stream));
+        c->launches += HNB_BATCH_BOUNDS_LAUNCHES;
     });
 }
 

@@ -14,6 +14,10 @@ from ._native import (BatchInfo, BatchLaunch, ChildInfo, DispatchIndirectArgs, D
                       EffectMetadata, SimParams, Spawner, Transform, check, lib)
 
 
+# hnb_instance_bounds as a numpy record
+BOUNDS_DTYPE = np.dtype([("min", np.float32, 3), ("count", np.uint32), ("max", np.float32, 3), ("reserved", np.uint32)])
+
+
 @dataclass
 class AttrField:
     """One field of the reference AoS ``Particle`` record."""
@@ -356,6 +360,17 @@ class Context:
         the rows their parents were restored to, and into the event counts of the metadata row's child-info rows
         (hnb_instance_restore_events). Only enqueues work."""
         check(lib.hnb_instance_restore_events(self._h, slab, effect, metadata_row, first, rows, _channels(emit_events), d_src, src_bytes))
+
+    def batch_bounds(self, launch: BatchLaunch, d_out: int, out_rows: int) -> None:
+        """Write the bounds of every instance of `launch`'s batch (the descriptor of the last simulate) to `d_out`: one
+        32-byte hnb_instance_bounds record per instance, `out_rows` of them at a 16-byte aligned address this device can
+        write (device_alloc, a torch tensor's data_ptr(), or pinned host memory). Call after simulate and before the next
+        frame's tables are uploaded; nothing of the instances changes; only enqueues work (hnb_batch_bounds)."""
+        check(lib.hnb_batch_bounds(self._h, C.byref(launch), d_out, out_rows))
+
+    def download_bounds(self, d_out: int, rows: int) -> np.ndarray:
+        """Wait for the context stream and return `rows` records batch_bounds wrote to device memory, as BOUNDS_DTYPE."""
+        return self.device_download(d_out, rows * BOUNDS_DTYPE.itemsize).view(BOUNDS_DTYPE)
 
     def slab_checksum(self, slab: int, first: int, count: int, index_base: int = 0) -> int:
         out = C.c_uint64(0)

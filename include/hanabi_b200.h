@@ -609,6 +609,57 @@ typedef struct hnb_batch_launch {
  */
 HNB_API int32_t hnb_simulate(hnb_ctx* ctx, const hnb_batch_launch* batches, uint32_t n);
 
+/**
+ * Bounds of one instance's live particles: the axis-aligned box of the `position` attribute. 32 bytes.
+ * A component no particle gave a value (an empty instance, or a NaN in every particle) has min = +inf and max = -inf.
+ */
+typedef struct hnb_instance_bounds {
+    float min[3];
+    uint32_t count;    /* n = min(alive_count, capacity): the particles the box covers */
+    float max[3];
+    uint32_t reserved; /* 0 */
+} hnb_instance_bounds;
+
+/**
+ * Compute the bounds of every instance of one batch on the device: what frustum culling, LOD or a slice allocator asks
+ * about an instance each frame, without a read-back of counts and without exporting records.
+ *
+ * `batch` is the launch descriptor passed to the last hnb_simulate; its `effect`, `slab` and `batch_info_index` are
+ * used. Record j of `d_out` receives the bounds of the batch's j-th instance (spawner row spawner_base + j), for every
+ * instance of the batch, in one call. `d_out` holds `out_rows` records and is 16-byte-aligned memory the context's device
+ * can write: device memory (hnb_device_alloc, for culling on the GPU) or pinned host memory (hnb_host_alloc; the host
+ * reads it after hnb_sync or an event of its own on the context stream).
+ *
+ * Per instance, with W = indirect_write_index, n = min(alive_count, capacity) and list = alive-list column W, all read on
+ * the DEVICE from the tables of the last simulated frame (the live set hnb_instance_snapshot defines):
+ *   - min[c] / max[c] are the minimum / maximum of component c of `position` AS STORED, over local rows list[first+i],
+ *     i < n, each clamped to the slice. Stored means simulation space: an HNB_EFFECT_LOCAL_SPACE effect gives a local
+ *     box, to which the caller applies the emitter transform.
+ *   - The order is the total order of the key  bits ^ (sign ? 0xFFFFFFFF : 0x80000000)  compared as unsigned: -0 < +0,
+ *     and the infinities take part. The result does not depend on scheduling: it is bit-exact. A NaN component is skipped.
+ *   - count = n, whatever the components hold.
+ *   - Particle extent is NOT included: neither `size` attributes nor render-time size modifiers. The caller inflates
+ *     the box by the effect's largest particle size.
+ * Nothing of the instance is modified: no record, list, identity claim, lifetime floor, alive bit, metadata word, draw
+ * argument or mailbox word. The call reads the slab in whatever column plan it has; it neither fixes the plan of a slab
+ * that has none yet nor turns lifetime floors off. Every kind of effect is accepted (emitting parents, ribbons, slot
+ * order, relaxed order, sector planes).
+ *
+ * Call window: between hnb_simulate calls, and BEFORE the next frame's hnb_upload_spawners / hnb_upload_batches. The
+ * device keeps the simulated frame's tables until the next hnb_simulate copies new ones; the instance count used to check
+ * `out_rows` is the host's batch row. Work is only enqueued on the context stream (two launches), after every launch of
+ * the previous hnb_simulate; no synchronisation, and no allocation after the first call (a per-context accumulator of
+ * 64 bytes per instance, which grows only when a larger batch is seen).
+ *
+ * HNB_ERR_INVALID_ARG, with nothing enqueued: `batch` NULL; invalid effect or slab handle; batch_info_index not an
+ * uploaded batch row, or the row's instances outside the uploaded spawner table; no metadata row inserted; the effect's
+ * stride or HNB_EFFECT_SECTOR_PLANES flag not matching the slab; an effect without a `position` attribute of type
+ * HNB_VEC3 at a 4-byte-aligned offset inside the record; `d_out` NULL or not 16-byte aligned; `out_rows` below the
+ * batch's instance count. A batch of zero instances is a no-op. Whatever the device tables hold, no access leaves the slab
+ * or d_out[0, out_rows): instance count, table rows, slab offset, capacity and list entries are clamped on the device.
+ */
+HNB_API int32_t hnb_batch_bounds(hnb_ctx* ctx, const hnb_batch_launch* batch, hnb_instance_bounds* d_out, uint32_t out_rows);
+
 /* Individual passes, as exercised one by one by the reference's shader contract tests
  * (src/render/shader_contract_tests.rs). They run the un-fused kernels. */
 HNB_API int32_t hnb_pass_init(hnb_ctx* ctx, const hnb_batch_launch* batch);

@@ -457,6 +457,90 @@ def snapshot_restore():
     ctx.close()
 
 
+def _timed_bounds(label, ctx, launch, instances, bytes_, extra=""):
+    """hnb_batch_bounds of `launch`'s batch into a device buffer: one warm-up call, then the best of 5 CUDA-event windows.
+    `bytes_`: what the pass must read (16 B of position per live particle, 4 B of list where no claim covers the row)."""
+    out = torch.empty(32 * instances, dtype=torch.uint8, device="cuda")
+    ctx.batch_bounds(launch, out.data_ptr(), instances)
+    ms = _events_ms(lambda: ctx.batch_bounds(launch, out.data_ptr(), instances))
+    rec = np.frombuffer(out.cpu().numpy().tobytes(), dtype=R.BOUNDS_DTYPE)
+    report(f"bounds: {label}", ms, bytes_, f"{ms * 1e3:.1f} us per call, {int(rec['count'].sum()) >> 10} Ki particles in {instances} records, best of 5{extra}")
+    return rec
+
+
+def bounds():
+    """hnb_batch_bounds: the filled 64 Mi C5 instance under its claim (16 B per particle), the same size spawned by one
+    init burst (identity list without a claim: 20 B), C4's topology in one call, the 16 Mi-slot churn steady state
+    (gathers through a permuted list) and one small instance (latency), beside a 2 GiB device-to-device copy."""
+    _card()
+    a = torch.empty(2 << 30, dtype=torch.uint8, device="cuda")
+    b = torch.empty_like(a)
+    ms = _events_ms(lambda: b.copy_(a))
+    report("bounds: 2 GiB device-to-device copy", ms, 2 * a.numel(), "torch copy_ (reads 2 GiB and writes 2 GiB), best of 5")
+    del a, b
+    torch.cuda.empty_cache()
+
+    P = 64 << 20
+    ctx = hb.Context(0, stream.cuda_stream)
+    effect = ctx.effect_compile(recipes.c5_lowered())
+    slab = ctx.slab_create(P, 32)
+    ctx.slab_fill_c5(slab, 0, P, 42, 1e9, 1e9)
+    single_instance(ctx, P, 32, alive=P)
+    la = N.BatchLaunch.make(effect, slab, 0, 0)
+    ctx.simulate([la])
+    rec = _timed_bounds("C5 64Mi filled, claim over every row", ctx, la, 1, 16 * P)
+    assert rec["count"][0] == P and (rec["min"][0] < -0.99).all() and (rec["max"][0] > 0.99).all()
+    ctx.slab_destroy(slab)
+    slab = ctx.slab_create(P, 32)
+    single_instance(ctx, P, 32, alive=0, spawn=P)
+    ctx.simulate([N.BatchLaunch.make(effect, slab, 0, P)])
+    ctx.upload_spawners([R.make_spawner(spawn=0, seed=43)])
+    la = N.BatchLaunch.make(effect, slab, 0, 0)
+    ctx.simulate([la])
+    rec = _timed_bounds("C5 64Mi from one init burst, no claim", ctx, la, 1, 20 * P)
+    assert rec["count"][0] == P
+    ctx.close()
+    torch.cuda.empty_cache()
+
+    n_inst, cap = 1024, 65536
+    ctx = hb.Context(0, stream.cuda_stream)
+    effect = ctx.effect_compile(recipes.c5_lowered())
+    slab = ctx.slab_create(n_inst * cap, 32)
+    sp = []
+    for i in range(n_inst):
+        ctx.slab_fill_c5(slab, i * cap, cap, 7000 + i, 1e9, 1e9)  # the last fill holds the slab's claim
+        m = R.initial_metadata(cap, i, 8)
+        m.alive_count, m.max_spawn = cap, 0
+        ctx.metadata_insert(i, m)
+        ctx.draw_args_insert(i)
+        sp.append(R.make_spawner(seed=i, effect_metadata_index=i, draw_indirect_index=i, slab_offset=i * cap))
+    ctx.upload_spawners(sp)
+    ctx.upload_batches([N.BatchInfo(0, 0, 0, 0, 0, n_inst)], [0] * n_inst)
+    ctx.set_sim_params(1 / 60, 0.0, n_inst)
+    la = N.BatchLaunch.make(effect, slab, 0, 0)
+    ctx.simulate([la])
+    rec = _timed_bounds("C4 shape: 1024 x 65536 in one batch", ctx, la, n_inst, 20 * n_inst * cap - 4 * cap)
+    assert (rec["count"] == cap).all()
+    ctx.close()
+    torch.cuda.empty_cache()
+
+    for cap in (4096, 16 << 10):
+        ctx = hb.Context(0, stream.cuda_stream)
+        slab = ctx.slab_create(cap, 32)
+        ctx.slab_fill_c5(slab, 0, cap, 100, 1e9, 1e9)
+        single_instance(ctx, cap, 32, alive=cap)
+        la = N.BatchLaunch.make(ctx.effect_compile(recipes.c5_lowered()), slab, 0, 0)
+        ctx.simulate([la])
+        _timed_bounds(f"one instance of {cap >> 10} Ki particles (latency)", ctx, la, 1, 16 * cap)
+        ctx.close()
+
+    P, ctx, slab, effect, stride, dt, rate = _churned()
+    alive = ctx.read_metadata(0).alive_count
+    _timed_bounds(f"churned {P >> 20} Mi slots, {alive >> 10} Ki alive, permuted list", ctx, N.BatchLaunch.make(effect, slab, 0, rate), 1, 20 * alive,
+                  "; GB/s counts 4 B of list + 16 B of position, the gather moves whole 32 B sectors")
+    ctx.close()
+
+
 def fresh_sector():
     """Cost of sector planes when access IS coalesced: C5 recipe burst + update, like `c5_init`, on a sector slab."""
     w = G.ExprWriter()
@@ -699,7 +783,7 @@ def emitter_relocation():
     ctx.close()
 
 
-SCENARIOS = {"c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "emitter_relocation": emitter_relocation, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
+SCENARIOS = {"c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "bounds": bounds, "emitter_relocation": emitter_relocation, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
 if __name__ == "__main__":
     for name in (sys.argv[1:] or list(SCENARIOS)):
         try:
