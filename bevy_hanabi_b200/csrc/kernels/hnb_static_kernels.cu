@@ -1041,6 +1041,373 @@ __global__ void __launch_bounds__(BD_THREADS) k_bounds_write(BoundsArgs a) {
     out[1] = hi;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Draw order of every instance of a batch (hnb_batch_depth_order): the live entries of each instance sorted back to
+// front by the depth of `position` against the instance's plane. A pure read of the instance, like bounds.
+//
+// Sort key: ~bounds_key(depth bits), and 0xFFFFFFFF for a NaN depth. Ascending keys are descending depths in bounds'
+// total order; no non-NaN depth has key 0xFFFFFFFF (bounds_key 0 is the NaN 0xFFFFFFFF), so NaNs go last. Every sort
+// below is stable and starts from the live entries in ascending i, so equal keys keep ascending i.
+//
+// Tiles of DO_TILE rows belong to one instance (tile t of instance j: rows [t*DO_TILE, (t+1)*DO_TILE) of its live list).
+// Thirteen launches, whatever the batch holds:
+//   k_do_plan      tiles per instance and their prefix over the batch (one CTA), digit totals zeroed (every CTA)
+//   k_do_keys      per tile: entries, positions, keys. An instance of one tile is sorted whole in shared memory (four
+//                  8-bit LSD passes) and written to the order; a larger one writes (key, entry) at its own slab rows of
+//                  scratch buffer 0, the tile's digit-0 histogram, and the instance's totals of all four digits
+//   4 x (k_do_scan, k_do_scatter), with k_do_hist before the scan of passes 1-3: an LSD pass over 8 bits. The scan
+//                  makes the per-tile histograms exclusive offsets in (digit, tile) order, one warp per (instance,
+//                  digit); the scatter ranks each tile's digits stably and moves its pairs to the other buffer, or
+//                  writes the entries to the order in the instance's last pass that runs.
+// A pass whose digit is the same for all n keys of an instance (one total equals n) does not run for it; an instance
+// for which no pass runs has its scratch entries copied to the order by the last scatter.
+// ---------------------------------------------------------------------------------------------
+#define DO_THREADS 256  // also the number of digit values: thread d owns digit d in every histogram step
+#define DO_WARPS (DO_THREADS / 32)
+#define DO_ITEMS 16
+#define DO_WARP_ROWS (32 * DO_ITEMS)
+#define DO_TILE (DO_THREADS * DO_ITEMS)
+#define DO_CTAS_PER_SM 4  // tile kernels loop over tiles: more CTAs than fit would only wait
+
+// ((a*x + b*y) + c*z) + d, every step rounded on its own (no contraction).
+#ifdef __CUDA_ARCH__
+__device__ __forceinline__ float do_mul(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ float do_add(float a, float b) { return __fadd_rn(a, b); }
+#else
+__device__ __forceinline__ float do_mul(float a, float b) { return a * b; }
+__device__ __forceinline__ float do_add(float a, float b) { return a + b; }
+#endif
+__device__ __forceinline__ u32 depth_sort_key(const float* plane, u32 x, u32 y, u32 z) {
+    const float depth = do_add(do_add(do_add(do_mul(plane[0], __uint_as_float(x)), do_mul(plane[1], __uint_as_float(y))),
+                                      do_mul(plane[2], __uint_as_float(z))), plane[3]);
+    const u32 bits = __float_as_uint(depth);
+    return (bits & 0x7FFFFFFFu) > 0x7F800000u ? 0xFFFFFFFFu : ~bounds_key(bits);
+}
+
+// Instance j as k_do_plan recorded it: 8 words.
+struct DepthInstance { u32 first, n, tile_base, tiles, w, rows, mask; };
+__device__ __forceinline__ DepthInstance do_instance(const DepthOrderArgs& a, u32 j) {
+    const u32* in = a.info + u64(j) * 8u;
+    return DepthInstance{in[0], in[1], in[2], in[3], in[4], in[5], in[6]};
+}
+// The instance that owns tile g of the call: the largest j with tile_base <= g (tile_base is non-decreasing in j, and
+// instances without tiles share the base of the next one). The caller checks g - tile_base < tiles.
+__device__ __forceinline__ u32 do_find(const DepthOrderArgs& a, u32 count, u32 g) {
+    u32 lo = 0u, hi = count - 1u;
+    while (lo < hi) {
+        const u32 mid = hi - (hi - lo) / 2u;
+        if (a.info[u64(mid) * 8u + 2u] <= g) lo = mid;
+        else hi = mid - 1u;
+    }
+    return lo;
+}
+// The buffer pass p reads: one flip per pass that ran before it.
+__device__ __forceinline__ u32 do_src(u32 mask, u32 pass) { return __popc(mask & ((1u << pass) - 1u)) & 1u; }
+
+// Stable rank of every item of a tile among the items of its digit. Item k of a warp is tile row
+// warp * DO_WARP_ROWS + k * 32 + lane, so a warp ranks its items k = 0, 1, ... in turn with __match_any_sync, and the
+// per-warp digit counts are then scanned in warp order. Digit 256 marks an item past the instance's end (no rank).
+// On return rank[k] is the number of earlier items of the tile with the same digit, and s_tot[d] the tile's count of d.
+__device__ __forceinline__ void do_rank(const u32 (&dig)[DO_ITEMS], u32 (&rank)[DO_ITEMS], u32* s_cnt, u32* s_tot) {
+    const u32 tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    __syncthreads();  // the previous tile's readers of s_cnt are done
+    for (u32 k = tid; k < DO_WARPS * 256u; k += DO_THREADS) s_cnt[k] = 0u;
+    __syncthreads();
+    u32* cnt = s_cnt + warp * 256u;
+    const u32 lt = (1u << lane) - 1u;
+#pragma unroll
+    for (u32 k = 0; k < DO_ITEMS; ++k) {
+        const u32 peers = __match_any_sync(0xffffffffu, dig[k]);
+        const u32 before = dig[k] < 256u ? cnt[dig[k]] : 0u;
+        rank[k] = before + __popc(peers & lt);
+        __syncwarp();
+        if (dig[k] < 256u && (peers & lt) == 0u) cnt[dig[k]] = before + __popc(peers);
+        __syncwarp();
+    }
+    __syncthreads();
+    u32 run = 0u;
+    for (u32 w = 0; w < DO_WARPS; ++w) {
+        const u32 c = s_cnt[w * 256u + tid];
+        s_cnt[w * 256u + tid] = run;
+        run += c;
+    }
+    s_tot[tid] = run;
+    __syncthreads();
+#pragma unroll
+    for (u32 k = 0; k < DO_ITEMS; ++k)
+        if (dig[k] < 256u) rank[k] += s_cnt[warp * 256u + dig[k]];
+}
+
+// Exclusive prefix of v over the CTA's threads in thread order.
+__device__ __forceinline__ u32 do_block_exclusive(u32 v, u32* s_warp) {
+    const u32 tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    u32 x = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const u32 y = __shfl_up_sync(0xffffffffu, x, d);
+        if (lane >= u32(d)) x += y;
+    }
+    __syncthreads();  // s_warp of an earlier call is read
+    if (lane == 31u) s_warp[warp] = x;
+    __syncthreads();
+    u32 before = 0u;
+    for (u32 w = 0; w < warp; ++w) before += s_warp[w];
+    return before + x - v;
+}
+
+// Tiles per instance and their prefix over the batch, kept in `info` for the later launches (CTA 0); the digit totals
+// of the call's instances back to zero (every CTA). An instance whose tiles would pass `max_tiles` (only possible when
+// the tables describe overlapping slices) gets none: it is not sorted, and nothing outside the buffers is touched.
+__global__ void __launch_bounds__(DO_THREADS) k_do_plan(DepthOrderArgs a) {
+    __shared__ u32 s_warp[DO_WARPS];
+    const u32 count = bounds_count(a.src), tid = threadIdx.x;
+    for (u64 k = u64(blockIdx.x) * DO_THREADS + tid; k < u64(count) * 1024u; k += u64(gridDim.x) * DO_THREADS) a.totals[k] = 0u;
+    if (blockIdx.x != 0u) return;
+    u64 carry = 0u;
+    for (u32 chunk = 0; chunk < count; chunk += DO_THREADS) {
+        const u32 j = chunk + tid;
+        BoundsInstance b = {0u, 0u, 0u, 0u};
+        if (j < count) b = bounds_instance(a.src, j);
+        const u32 tiles = u32((u64(b.n) + DO_TILE - 1u) / DO_TILE);
+        const u32 excl = do_block_exclusive(tiles, s_warp);
+        const u64 base = carry + excl;
+        if (j < count) {
+            u32* in = a.info + u64(j) * 8u;
+            const bool fits = base + tiles <= a.max_tiles;
+            in[0] = b.first; in[1] = b.n; in[2] = u32(base < a.max_tiles ? base : a.max_tiles); in[3] = fits ? tiles : 0u;
+            in[4] = b.w; in[5] = b.rows; in[6] = 0u; in[7] = 0u;
+        }
+        __syncthreads();
+        if (tid == DO_THREADS - 1u) s_warp[0] = excl + tiles;
+        __syncthreads();
+        carry += s_warp[0];
+    }
+    if (tid == 0u) *a.total_tiles = u32(carry < a.max_tiles ? carry : a.max_tiles);
+}
+
+// Entry, position and key of every live row of the tile; rows below the identity claim of column W load no list entry.
+template <bool FAST>
+__device__ __forceinline__ void do_tile_keys(const DepthOrderArgs& a, const DepthInstance& in, u32 claimed, const float* plane,
+                                             u32 i0, u32 (&key)[DO_ITEMS], u32 (&val)[DO_ITEMS]) {
+    const BoundsArgs& s = a.src;
+    const u32* list = (in.w == 0u ? s.ping : s.pong) + in.first;
+    const u32 last_row = in.rows - 1u;
+#pragma unroll
+    for (u32 k = 0; k < DO_ITEMS; ++k) {
+        const u32 i = i0 + k * 32u;
+        val[k] = i < claimed ? i : (i < in.n ? min(list[i], last_row) : 0u);
+    }
+    if (FAST) {
+        const RepackPiece<4>* col = (const RepackPiece<4>*)s.col[0];
+        const u32 quads = s.col_words[0] >> 2u, quad = s.col_lane[0] >> 2u;
+        RepackPiece<4> v[DO_ITEMS];
+#pragma unroll
+        for (u32 k = 0; k < DO_ITEMS; ++k)
+            if (i0 + k * 32u < in.n) v[k] = col[(u64(in.first) + val[k]) * quads + quad];
+#pragma unroll
+        for (u32 k = 0; k < DO_ITEMS; ++k)
+            key[k] = i0 + k * 32u < in.n ? depth_sort_key(plane, v[k].w[0], v[k].w[1], v[k].w[2]) : 0xFFFFFFFFu;
+    } else {
+        u32 v[DO_ITEMS][3];
+#pragma unroll
+        for (u32 k = 0; k < DO_ITEMS; ++k) {
+            if (i0 + k * 32u >= in.n) continue;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) v[k][c] = s.col[c][(u64(in.first) + val[k]) * s.col_words[c] + s.col_lane[c]];
+        }
+#pragma unroll
+        for (u32 k = 0; k < DO_ITEMS; ++k)
+            key[k] = i0 + k * 32u < in.n ? depth_sort_key(plane, v[k][0], v[k][1], v[k][2]) : 0xFFFFFFFFu;
+    }
+}
+
+// Persistent grid over the call's tiles (the count is read from the plan). One-tile instances are sorted here whole;
+// larger ones get their pairs, histograms and totals for the passes.
+template <bool FAST>
+__global__ void __launch_bounds__(DO_THREADS) k_do_keys(DepthOrderArgs a) {
+    __shared__ u32 s_key[DO_TILE], s_val[DO_TILE];
+    __shared__ u32 s_cnt[DO_WARPS * 256], s_tot[256], s_warp[DO_WARPS];
+    const u32 count = bounds_count(a.src), total = *a.total_tiles, tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    const u64 claim0 = hnb_claim_load(&a.src.claim[0]), claim1 = hnb_claim_load(&a.src.claim[1]);
+    for (u32 g = blockIdx.x; g < total; g += gridDim.x) {
+        const u32 j = do_find(a, count, g);
+        const DepthInstance in = do_instance(a, j);
+        const u32 t = g - in.tile_base;
+        if (t >= in.tiles) continue;  // CTA-uniform
+        const u32 claimed = min(hnb_claim_len(in.w == 0u ? claim0 : claim1, in.first), in.n);
+        const u32 r0 = warp * DO_WARP_ROWS + lane, i0 = t * DO_TILE + r0;
+        u32 key[DO_ITEMS], val[DO_ITEMS];
+        do_tile_keys<FAST>(a, in, claimed, a.planes + u64(j) * 4u, i0, key, val);
+        if (in.tiles == 1u) {
+            u32 dig[DO_ITEMS], rank[DO_ITEMS];
+            for (u32 pass = 0; pass < 4u; ++pass) {
+#pragma unroll
+                for (u32 k = 0; k < DO_ITEMS; ++k) dig[k] = i0 + k * 32u < in.n ? (key[k] >> (8u * pass)) & 255u : 256u;
+                do_rank(dig, rank, s_cnt, s_tot);
+                const u32 base = do_block_exclusive(s_tot[tid], s_warp);
+                __syncthreads();  // every thread has read s_tot
+                s_tot[tid] = base;
+                __syncthreads();
+#pragma unroll
+                for (u32 k = 0; k < DO_ITEMS; ++k) {
+                    if (dig[k] >= 256u) continue;
+                    const u32 r = s_tot[dig[k]] + rank[k];
+                    s_key[r] = key[k];
+                    s_val[r] = val[k];
+                }
+                __syncthreads();
+#pragma unroll
+                for (u32 k = 0; k < DO_ITEMS; ++k) {
+                    if (r0 + k * 32u >= in.n) continue;
+                    key[k] = s_key[r0 + k * 32u];
+                    val[k] = s_val[r0 + k * 32u];
+                }
+            }
+#pragma unroll
+            for (u32 k = 0; k < DO_ITEMS; ++k)
+                if (r0 + k * 32u < in.n) a.order[u64(in.first) + r0 + k * 32u] = val[k];
+            continue;
+        }
+        __syncthreads();  // the previous tile's readers of s_cnt are done
+        for (u32 k = tid; k < 4u * 256u; k += DO_THREADS) s_cnt[k] = 0u;
+        __syncthreads();
+#pragma unroll
+        for (u32 k = 0; k < DO_ITEMS; ++k) {
+            const u32 i = i0 + k * 32u;
+            if (i >= in.n) continue;
+            a.keys[0][u64(in.first) + i] = key[k];
+            a.vals[0][u64(in.first) + i] = val[k];
+#pragma unroll
+            for (u32 p = 0; p < 4u; ++p) atomicAdd(&s_cnt[p * 256u + ((key[k] >> (8u * p)) & 255u)], 1u);
+        }
+        __syncthreads();
+        a.hist[u64(in.tile_base) * 256u + u64(tid) * in.tiles + t] = s_cnt[tid];
+#pragma unroll
+        for (u32 p = 0; p < 4u; ++p)
+            if (s_cnt[p * 256u + tid]) atomicAdd(&a.totals[u64(j) * 1024u + p * 256u + tid], s_cnt[p * 256u + tid]);
+    }
+}
+
+// Pass `pass`, one warp per (instance, digit d): the row of tile counts of d becomes exclusive offsets into the
+// instance's order, starting at the count of the smaller digits. Pass 0 also decides, from the totals, which passes run.
+__global__ void __launch_bounds__(DO_THREADS) k_do_scan(DepthOrderArgs a, u32 pass) {
+    const u32 lane = threadIdx.x & 31u;
+    const u64 row = u64(blockIdx.x) * DO_WARPS + (threadIdx.x >> 5);
+    const u32 count = bounds_count(a.src);
+    if (row >= u64(count) * 256u) return;  // warp-uniform
+    const u32 j = u32(row >> 8), d = u32(row & 255u);
+    const DepthInstance in = do_instance(a, j);
+    if (in.tiles < 2u) return;
+    const u32* tot = a.totals + u64(j) * 1024u;
+    u32 run;
+    if (pass == 0u) {
+        u32 mask = 0u;
+        for (u32 p = 0; p < 4u; ++p) {
+            bool constant = false;
+#pragma unroll
+            for (u32 q = 0; q < 8u; ++q) constant |= tot[p * 256u + q * 32u + lane] == in.n;
+            if (__ballot_sync(0xffffffffu, constant) == 0u) mask |= 1u << p;
+        }
+        if (d == 0u && lane == 0u) a.info[u64(j) * 8u + 6u] = mask;
+        run = mask & 1u;
+    } else {
+        run = (in.mask >> pass) & 1u;
+    }
+    if (!run) return;
+    u32 base = 0u;
+#pragma unroll
+    for (u32 q = 0; q < 8u; ++q) {
+        const u32 e = q * 32u + lane;
+        if (e < d) base += tot[pass * 256u + e];
+    }
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) base += __shfl_xor_sync(0xffffffffu, base, s);
+    u32* h = a.hist + u64(in.tile_base) * 256u + u64(d) * in.tiles;
+    for (u32 t0 = 0; t0 < in.tiles; t0 += 256u) {
+        u32 v[8];
+#pragma unroll
+        for (u32 q = 0; q < 8u; ++q) v[q] = t0 + q * 32u + lane < in.tiles ? h[t0 + q * 32u + lane] : 0u;
+#pragma unroll
+        for (u32 q = 0; q < 8u; ++q) {
+            u32 x = v[q];
+#pragma unroll
+            for (int s = 1; s < 32; s <<= 1) {
+                const u32 y = __shfl_up_sync(0xffffffffu, x, s);
+                if (lane >= u32(s)) x += y;
+            }
+            if (t0 + q * 32u + lane < in.tiles) h[t0 + q * 32u + lane] = base + x - v[q];
+            base += __shfl_sync(0xffffffffu, x, 31);
+        }
+    }
+}
+
+// Pass `pass` over every tile of the instances it runs for: stable digit ranks within the tile plus the tile's offsets
+// give each pair its place in the instance's slice of the other buffer (of the order, in the last pass that runs).
+// Places are clamped to the instance's n: only tables that describe overlapping slices could produce another.
+__global__ void __launch_bounds__(DO_THREADS) k_do_scatter(DepthOrderArgs a, u32 pass) {
+    __shared__ u32 s_cnt[DO_WARPS * 256], s_tot[256];
+    const u32 count = bounds_count(a.src), total = *a.total_tiles, tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    for (u32 g = blockIdx.x; g < total; g += gridDim.x) {
+        const DepthInstance in = do_instance(a, do_find(a, count, g));
+        const u32 t = g - in.tile_base;
+        if (in.tiles < 2u || t >= in.tiles) continue;  // CTA-uniform
+        const u32 i0 = t * DO_TILE + warp * DO_WARP_ROWS + lane;
+        if (!((in.mask >> pass) & 1u)) {
+            if (pass == 3u && in.mask == 0u) {  // every digit constant: the keys are all equal, the entries in order
+#pragma unroll
+                for (u32 k = 0; k < DO_ITEMS; ++k) {
+                    const u32 i = i0 + k * 32u;
+                    if (i < in.n) a.order[u64(in.first) + i] = a.vals[0][u64(in.first) + i];
+                }
+            }
+            continue;
+        }
+        const u32 src = do_src(in.mask, pass), last = (in.mask >> (pass + 1u)) == 0u;
+        u32 key[DO_ITEMS], val[DO_ITEMS], dig[DO_ITEMS], rank[DO_ITEMS];
+#pragma unroll
+        for (u32 k = 0; k < DO_ITEMS; ++k) {
+            const u32 i = i0 + k * 32u;
+            key[k] = i < in.n ? a.keys[src][u64(in.first) + i] : 0u;
+            val[k] = i < in.n ? a.vals[src][u64(in.first) + i] : 0u;
+            dig[k] = i < in.n ? (key[k] >> (8u * pass)) & 255u : 256u;
+        }
+        do_rank(dig, rank, s_cnt, s_tot);
+        s_tot[tid] = a.hist[u64(in.tile_base) * 256u + u64(tid) * in.tiles + t];
+        __syncthreads();
+#pragma unroll
+        for (u32 k = 0; k < DO_ITEMS; ++k) {
+            if (dig[k] >= 256u) continue;
+            const u64 r = u64(in.first) + min(s_tot[dig[k]] + rank[k], in.n - 1u);
+            if (last) {
+                a.order[r] = val[k];
+            } else {
+                a.keys[src ^ 1u][r] = key[k];
+                a.vals[src ^ 1u][r] = val[k];
+            }
+        }
+    }
+}
+
+// Tile histograms of pass `pass` (1-3) over the buffer that pass reads.
+__global__ void __launch_bounds__(DO_THREADS) k_do_hist(DepthOrderArgs a, u32 pass) {
+    __shared__ u32 s_cnt[256];
+    const u32 count = bounds_count(a.src), total = *a.total_tiles, tid = threadIdx.x;
+    for (u32 g = blockIdx.x; g < total; g += gridDim.x) {
+        const DepthInstance in = do_instance(a, do_find(a, count, g));
+        const u32 t = g - in.tile_base;
+        if (in.tiles < 2u || t >= in.tiles || !((in.mask >> pass) & 1u)) continue;  // CTA-uniform
+        const u32* keys = a.keys[do_src(in.mask, pass)] + in.first;
+        __syncthreads();
+        s_cnt[tid] = 0u;
+        __syncthreads();
+        const u32 end = u64(t + 1u) * DO_TILE < in.n ? (t + 1u) * DO_TILE : in.n;
+        for (u32 i = t * DO_TILE + tid; i < end; i += DO_THREADS)
+            atomicAdd(&s_cnt[(keys[i] >> (8u * pass)) & 255u], 1u);
+        __syncthreads();
+        a.hist[u64(in.tile_base) * 256u + u64(tid) * in.tiles + t] = s_cnt[tid];
+    }
+}
+
 // Effective SM clock: cycles elapsed on one SM over ~`window_ns` of the global timer.
 __global__ void k_measure_sm_clock(u64* out, u64 window_ns) {
     u64 t0, t1;
@@ -1240,6 +1607,23 @@ cudaError_t launch_batch_bounds(const BoundsArgs& a, bool fast, u32 sm_count, cu
     if (fast) k_bounds_reduce<true><<<grid, BD_THREADS, 0, st>>>(a);
     else k_bounds_reduce<false><<<grid, BD_THREADS, 0, st>>>(a);
     k_bounds_write<<<blocks_for(a.max_instances, BD_THREADS), BD_THREADS, 0, st>>>(a);
+    return cudaGetLastError();
+}
+u64 depth_order_max_tiles(u32 capacity_rows, u32 max_instances) { return u64(capacity_rows) / DO_TILE + max_instances; }
+cudaError_t launch_batch_depth_order(const DepthOrderArgs& a, bool fast, u32 sm_count, cudaStream_t st) {
+    if (a.src.max_instances == 0) return cudaSuccess;
+    // tile kernels: no more CTAs than the call can have tiles; the plan zeroes 1024 totals per instance
+    const unsigned tiles = (unsigned)std::max<u64>(1, std::min<u64>(a.max_tiles, u64(sm_count) * DO_CTAS_PER_SM));
+    const unsigned plan = std::min(blocks_for(u64(a.src.max_instances) * 1024u, DO_THREADS * 16u), 1024u);
+    const unsigned rows = blocks_for(u64(a.src.max_instances) * 256u, DO_WARPS);
+    k_do_plan<<<plan, DO_THREADS, 0, st>>>(a);
+    if (fast) k_do_keys<true><<<tiles, DO_THREADS, 0, st>>>(a);
+    else k_do_keys<false><<<tiles, DO_THREADS, 0, st>>>(a);
+    for (u32 pass = 0; pass < 4u; ++pass) {
+        if (pass) k_do_hist<<<tiles, DO_THREADS, 0, st>>>(a, pass);
+        k_do_scan<<<rows, DO_THREADS, 0, st>>>(a, pass);
+        k_do_scatter<<<tiles, DO_THREADS, 0, st>>>(a, pass);
+    }
     return cudaGetLastError();
 }
 cudaError_t launch_measure_sm_clock(u64* out2, u64 window_ns, cudaStream_t st) {

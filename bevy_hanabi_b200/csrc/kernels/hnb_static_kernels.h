@@ -154,6 +154,28 @@ struct BoundsArgs {
 cudaError_t launch_batch_bounds(const BoundsArgs& a, bool fast, u32 sm_count, cudaStream_t st);
 #define HNB_BATCH_BOUNDS_LAUNCHES 2u
 
+// Draw order of every instance of one batch (hnb_batch_depth_order): per instance, its live entries sorted by the depth of
+// `position` against the instance's plane, farthest first, NaN last, ties in list order, written at its own slab rows of
+// `order`. The instances and `position` are found as BoundsArgs describes (its acc and out are not used).
+struct DepthOrderArgs {
+    BoundsArgs src;
+    const float* planes;  // (a, b, c, d) per instance of the batch
+    u32* order;           // d_order: indexed by slab row
+    // Scratch, one context-owned buffer: 16 bytes per slab row, 1 KiB per tile of the call, 4 KiB + 32 bytes per instance.
+    u32* keys[2];         // LSD pass buffers of (key, entry), indexed by slab row
+    u32* vals[2];
+    u32* hist;            // 256 words per tile: instance j's block at 256 * tile_base, digit-major [digit][tile]
+    u32* totals;          // [instance][pass][digit]: digit counts of each instance of more than one tile
+    u32* info;            // 8 words per instance (k_do_plan): first, n, tile_base, tiles, W, rows, mask of passes that run
+    u32* total_tiles;     // [1]: tiles of the call
+    u32 max_tiles;        // depth_order_max_tiles(capacity_rows, max_instances): `hist` holds 256 words per tile
+};
+// Tiles a call can have: disjoint slices of n_j rows need sum ceil(n_j / tile) <= capacity_rows / tile + instances.
+u64 depth_order_max_tiles(u32 capacity_rows, u32 max_instances);
+// A fixed sequence of launches whatever the batch holds. `fast`: position's three words share one 16- or 32-byte column.
+cudaError_t launch_batch_depth_order(const DepthOrderArgs& a, bool fast, u32 sm_count, cudaStream_t st);
+#define HNB_BATCH_DEPTH_ORDER_LAUNCHES 13u
+
 cudaError_t launch_indirect(const StaticTables& T, u32 num_effects, cudaStream_t st);
 cudaError_t launch_prefix_sum(const StaticTables& T, u32 num_batches, cudaStream_t st);
 cudaError_t launch_tile_prefix(const StaticTables& T, u32 batch_index, u32 tile, cudaStream_t st);

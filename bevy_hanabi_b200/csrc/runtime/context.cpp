@@ -260,6 +260,7 @@ struct hnb_ctx {
     bool plan_dirty = false;  // bind_launch changed a tile-size or range word of the host frame block since the last upload
     uint64_t frame_copies = 0, frames = 0;  // hnb_simulate calls that needed the host->device copy of the frame block / all calls
     DeviceArray<unsigned long long> d_bounds_acc;  // hnb_batch_bounds: 8 slots per instance of the largest batch seen, zero between calls
+    DeviceArray<uint32_t> d_depth_scratch;  // hnb_batch_depth_order: pass buffers, histograms and instance plan of the largest call seen
     DeviceArray<unsigned long long> d_debug;  // 16 diagnostic counters + a 64-frame timeline ring of 4 words (HNB_PROFILE kernels)
 
     hnb::FrameHeader* header() { return reinterpret_cast<hnb::FrameHeader*>(h_arena.get()); }
@@ -1873,26 +1874,64 @@ int32_t hnb_simulate(hnb_ctx* c, const hnb_batch_launch* batches, uint32_t n) {
 
 static_assert(sizeof(hnb_instance_bounds) == 32, "hnb_instance_bounds is two 16-byte stores");
 
+// The checks hnb_batch_bounds and hnb_batch_depth_order share, and where `position` sits in the slab's current columns.
 // Everything is checked on the host before anything is enqueued; what the instances look like (counts, W, slab offsets,
 // metadata rows) is read by the kernels from the device tables of the last simulated frame, clamped there.
+struct BatchPosition {
+    const Slab* slab;
+    const Effect* effect;
+    const hnb_batch_info* batch;  // the host's row: its prefix_sum_count sizes the call
+    const hnb_attr_layout* position;
+};
+static BatchPosition check_batch_position(hnb_ctx* c, const hnb_batch_launch* b, const std::string& w) {
+    if (!b) fail(HNB_ERR_INVALID_ARG, w + ": batch is NULL");
+    const Slab& s = get_slab(c, b->slab);
+    const Effect& fx = get_effect(c, b->effect);
+    if (b->batch_info_index >= c->B) fail(HNB_ERR_INVALID_ARG, w + ": batch_info_index is not an uploaded batch row");
+    const hnb_batch_info& bi = c->h_at<hnb_batch_info>(c->lay.off_batch_infos)[b->batch_info_index];
+    if (uint64_t(bi.spawner_base) + bi.prefix_sum_count > c->E)
+        fail(HNB_ERR_INVALID_ARG, w + ": the batch references instances outside the uploaded spawner table");
+    if (fx.particle_stride != s.stride) fail(HNB_ERR_INVALID_ARG, w + ": effect particle stride does not match the slab");
+    if (((fx.flags & HNB_EFFECT_SECTOR_PLANES) != 0) != s.sector_planes)
+        fail(HNB_ERR_INVALID_ARG, w + ": effect and slab disagree on HNB_EFFECT_SECTOR_PLANES / HNB_SLAB_SECTOR_PLANES");
+    const hnb_attr_layout* position = nullptr;
+    for (const hnb_attr_layout& a : fx.desc->attrs)
+        if (a.name && std::string(a.name) == "position") position = &a;
+    if (!position || position->value_type != HNB_VEC3 || (position->offset & 3u) || uint64_t(position->offset) + 12 > s.stride)
+        fail(HNB_ERR_INVALID_ARG, w + ": the effect has no `position` attribute of type HNB_VEC3 inside its record");
+    return BatchPosition{&s, &fx, &bi, position};
+}
+// The device side of a checked batch with at least one instance. `fast`: position's three words share one 16-byte quad.
+static hnb::BoundsArgs batch_position_args(hnb_ctx* c, const hnb_batch_launch* b, const BatchPosition& bp, bool* fast) {
+    const Slab& s = *bp.slab;
+    hnb::BoundsArgs a{};
+    a.batch_info = c->d_at<hnb::BatchInfo>(c->lay.off_batch_infos) + b->batch_info_index;
+    a.spawners = c->d_at<hnb::Spawner>(c->lay.off_spawners);
+    a.metadata = c->d_metadata.get();
+    a.num_spawners = c->E;
+    a.num_metadata = uint32_t(c->d_metadata.size());
+    a.ping = s.ping.get();
+    a.pong = s.pong.get();
+    a.claim = s.ident_claim.get();
+    a.capacity_rows = s.capacity;
+    a.max_instances = bp.batch->prefix_sum_count;
+    // position in the slab's CURRENT columns: a plan may cut its three words apart
+    const hnb::PlaneSet ps = plane_set(s);
+    for (uint32_t k = 0; k < 3; ++k) {
+        const uint32_t word = bp.position->offset / 4 + k, p = ps.word_to_plane[word];
+        a.col[k] = static_cast<const uint32_t*>(ps.ptr[p]);
+        a.col_words[k] = ps.words[p];
+        a.col_lane[k] = word - ps.word_off[p];
+    }
+    *fast = a.col[2] == a.col[0] && (a.col_lane[0] & 3u) == 0 && (a.col_words[0] & 3u) == 0;
+    return a;
+}
+
 int32_t hnb_batch_bounds(hnb_ctx* c, const hnb_batch_launch* b, hnb_instance_bounds* d_out, uint32_t out_rows) {
     return guarded([&] {
         const std::string w = "hnb_batch_bounds";
-        if (!b) fail(HNB_ERR_INVALID_ARG, w + ": batch is NULL");
-        const Slab& s = get_slab(c, b->slab);
-        const Effect& fx = get_effect(c, b->effect);
-        if (b->batch_info_index >= c->B) fail(HNB_ERR_INVALID_ARG, w + ": batch_info_index is not an uploaded batch row");
-        const hnb_batch_info& bi = c->h_at<hnb_batch_info>(c->lay.off_batch_infos)[b->batch_info_index];
-        if (uint64_t(bi.spawner_base) + bi.prefix_sum_count > c->E)
-            fail(HNB_ERR_INVALID_ARG, w + ": the batch references instances outside the uploaded spawner table");
-        if (fx.particle_stride != s.stride) fail(HNB_ERR_INVALID_ARG, w + ": effect particle stride does not match the slab");
-        if (((fx.flags & HNB_EFFECT_SECTOR_PLANES) != 0) != s.sector_planes)
-            fail(HNB_ERR_INVALID_ARG, w + ": effect and slab disagree on HNB_EFFECT_SECTOR_PLANES / HNB_SLAB_SECTOR_PLANES");
-        const hnb_attr_layout* position = nullptr;
-        for (const hnb_attr_layout& a : fx.desc->attrs)
-            if (a.name && std::string(a.name) == "position") position = &a;
-        if (!position || position->value_type != HNB_VEC3 || (position->offset & 3u) || uint64_t(position->offset) + 12 > s.stride)
-            fail(HNB_ERR_INVALID_ARG, w + ": the effect has no `position` attribute of type HNB_VEC3 inside its record");
+        const BatchPosition bp = check_batch_position(c, b, w);
+        const hnb_batch_info& bi = *bp.batch;
         if (!d_out || ((uintptr_t)d_out & 15u)) fail(HNB_ERR_INVALID_ARG, w + ": d_out is NULL or not 16-byte aligned");
         if (out_rows < bi.prefix_sum_count) fail(HNB_ERR_INVALID_ARG, w + ": out_rows is below the batch's instance count");
         if (bi.prefix_sum_count == 0) return;
@@ -1901,30 +1940,54 @@ int32_t hnb_batch_bounds(hnb_ctx* c, const hnb_batch_launch* b, hnb_instance_bou
         if (c->d_bounds_acc.size() < size_t(bi.prefix_sum_count) * 8)
             CUDA_CHECK(grow(c->d_bounds_acc, std::max<size_t>(bi.prefix_sum_count, c->d_metadata.size()) * 8, 0, c->stream));
 
-        hnb::BoundsArgs a{};
-        a.batch_info = c->d_at<hnb::BatchInfo>(c->lay.off_batch_infos) + b->batch_info_index;
-        a.spawners = c->d_at<hnb::Spawner>(c->lay.off_spawners);
-        a.metadata = c->d_metadata.get();
-        a.num_spawners = c->E;
-        a.num_metadata = uint32_t(c->d_metadata.size());
-        a.ping = s.ping.get();
-        a.pong = s.pong.get();
-        a.claim = s.ident_claim.get();
-        a.capacity_rows = s.capacity;
-        a.max_instances = bi.prefix_sum_count;
-        // position in the slab's CURRENT columns: a plan may cut its three words apart
-        const hnb::PlaneSet ps = plane_set(s);
-        for (uint32_t k = 0; k < 3; ++k) {
-            const uint32_t word = position->offset / 4 + k, p = ps.word_to_plane[word];
-            a.col[k] = static_cast<const uint32_t*>(ps.ptr[p]);
-            a.col_words[k] = ps.words[p];
-            a.col_lane[k] = word - ps.word_off[p];
-        }
-        const bool fast = a.col[2] == a.col[0] && (a.col_lane[0] & 3u) == 0 && (a.col_words[0] & 3u) == 0;
+        bool fast = false;
+        hnb::BoundsArgs a = batch_position_args(c, b, bp, &fast);
         a.acc = c->d_bounds_acc.get();
         a.out = d_out;
         CUDA_CHECK(hnb::launch_batch_bounds(a, fast, uint32_t(c->sm_count), c->stream));
         c->launches += HNB_BATCH_BOUNDS_LAUNCHES;
+    });
+}
+
+int32_t hnb_batch_depth_order(hnb_ctx* c, const hnb_batch_launch* b, const float* d_planes, uint32_t plane_rows, uint32_t* d_order,
+                              uint32_t order_rows) {
+    return guarded([&] {
+        const std::string w = "hnb_batch_depth_order";
+        // a ribbon effect is refused before anything else about it is checked
+        if (b && (get_effect(c, b->effect).flags & HNB_EFFECT_RIBBONS))
+            fail(HNB_ERR_INVALID_ARG, w + ": a ribbon effect is drawn in ribbon order, not in depth order");
+        const BatchPosition bp = check_batch_position(c, b, w);
+        const hnb_batch_info& bi = *bp.batch;
+        if (!d_planes || ((uintptr_t)d_planes & 15u)) fail(HNB_ERR_INVALID_ARG, w + ": d_planes is NULL or not 16-byte aligned");
+        if (plane_rows < bi.prefix_sum_count) fail(HNB_ERR_INVALID_ARG, w + ": plane_rows is below the batch's instance count");
+        if (!d_order) fail(HNB_ERR_INVALID_ARG, w + ": d_order is NULL");
+        if (order_rows < bp.slab->capacity) fail(HNB_ERR_INVALID_ARG, w + ": order_rows is below the slab's capacity");
+        if (bi.prefix_sum_count == 0) return;
+        if (c->d_metadata.size() == 0) fail(HNB_ERR_INVALID_ARG, w + ": no metadata row was inserted");
+        CUDA_CHECK(cudaSetDevice(c->device));
+        // scratch: four words per slab row, 256 per tile, 1024 + 8 per instance, the tile count
+        const size_t rows = bp.slab->capacity, inst = bi.prefix_sum_count;
+        const size_t max_tiles = hnb::depth_order_max_tiles(bp.slab->capacity, bi.prefix_sum_count);
+        const size_t words = 4 * rows + 256 * max_tiles + 1032 * inst + 1;
+        if (c->d_depth_scratch.size() < words) CUDA_CHECK(grow(c->d_depth_scratch, words, 0, c->stream));
+
+        bool fast = false;
+        hnb::DepthOrderArgs a{};
+        a.src = batch_position_args(c, b, bp, &fast);
+        a.planes = d_planes;
+        a.order = d_order;
+        uint32_t* p = c->d_depth_scratch.get();
+        for (int k = 0; k < 2; ++k) {
+            a.keys[k] = p + (2 * k) * rows;
+            a.vals[k] = p + (2 * k + 1) * rows;
+        }
+        a.hist = p + 4 * rows;
+        a.totals = a.hist + 256 * max_tiles;
+        a.info = a.totals + 1024 * inst;
+        a.total_tiles = a.info + 8 * inst;
+        a.max_tiles = uint32_t(max_tiles);
+        CUDA_CHECK(hnb::launch_batch_depth_order(a, fast, uint32_t(c->sm_count), c->stream));
+        c->launches += HNB_BATCH_DEPTH_ORDER_LAUNCHES;
     });
 }
 

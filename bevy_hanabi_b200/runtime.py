@@ -368,6 +368,14 @@ class Context:
         frame's tables are uploaded; nothing of the instances changes; only enqueues work (hnb_batch_bounds)."""
         check(lib.hnb_batch_bounds(self._h, C.byref(launch), d_out, out_rows))
 
+    def batch_depth_order(self, launch: BatchLaunch, d_planes: int, plane_rows: int, d_order: int, order_rows: int) -> None:
+        """Sort every instance of `launch`'s batch (the descriptor of the last simulate) back to front: d_order[first + r]
+        receives the r-th farthest live entry of the instance, by the depth of `position` against plane j = d_planes[4j:4j+4]
+        (float32 a, b, c, d; 16-byte aligned). `d_order` (uint32, `order_rows` >= the slab's capacity, indexed by slab row)
+        and `d_planes` are device or pinned host memory. Same call window as batch_bounds; nothing of the instances
+        changes; only enqueues work (hnb_batch_depth_order)."""
+        check(lib.hnb_batch_depth_order(self._h, C.byref(launch), d_planes, plane_rows, d_order, order_rows))
+
     def download_bounds(self, d_out: int, rows: int) -> np.ndarray:
         """Wait for the context stream and return `rows` records batch_bounds wrote to device memory, as BOUNDS_DTYPE."""
         return self.device_download(d_out, rows * BOUNDS_DTYPE.itemsize).view(BOUNDS_DTYPE)

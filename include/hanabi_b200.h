@@ -660,6 +660,44 @@ typedef struct hnb_instance_bounds {
  */
 HNB_API int32_t hnb_batch_bounds(hnb_ctx* ctx, const hnb_batch_launch* batch, hnb_instance_bounds* d_out, uint32_t out_rows);
 
+/**
+ * Sort every instance's live particles back to front on the device, in one call per batch: the draw order that
+ * alpha-blended particles need, without a read-back of counts and without exporting records.
+ *
+ * `batch`, the live set and the call window are those of hnb_batch_bounds. For the batch's j-th instance (spawner row
+ * spawner_base + j), with first = its slab offset, n = min(alive_count, capacity), list = alive-list column W
+ * (W = indirect_write_index) and the live entries e_i = list[first + i], i < n, each clamped to the slice (entries under
+ * the identity claim of column W are i, and are not loaded), all read on the DEVICE from the tables of the last
+ * simulated frame:
+ *   - Plane j is d_planes[4j .. 4j+3] = (a, b, c, d). The depth of entry e is ((a*x + b*y) + c*z) + d, with (x, y, z) its
+ *     `position` AS STORED and every operation one fp32 round-to-nearest step (no contraction). With a camera's forward
+ *     axis f and eye p, the plane (f, -f.p) gives view depth; for an HNB_EFFECT_LOCAL_SPACE effect, pass that plane
+ *     transformed into the emitter's space.
+ *   - d_order[first + r] = e_pi(r) for r < n, where pi sorts by depth DESCENDING (farthest first) in the total order of
+ *     the key  bits ^ (sign ? 0xFFFFFFFF : 0x80000000)  (so -0 < +0 and the infinities take part), NaN depths after all
+ *     others, and equal depths in ascending i (stable). The result depends on device state alone: it is bit-exact.
+ * d_order is indexed by slab row like the alive-list columns: a renderer binds it in place of the column the draw reads
+ * (render_indirect_read_index) and keeps the draw-indirect instance_count. Nothing outside d_order[first, first + n) of
+ * each instance is written, so one buffer of the slab's capacity per view serves every batch of the slab.
+ *
+ * Nothing of the instance is modified: no record, list, identity claim, lifetime floor, alive bit, metadata word, draw
+ * argument or mailbox word. The call reads the slab in whatever column plan it has; it neither fixes the plan of a slab
+ * that has none yet nor turns lifetime floors off. Every effect hnb_batch_bounds accepts is accepted (emitting parents,
+ * slot order, relaxed order, sector planes) except an HNB_EFFECT_RIBBONS effect, whose draw follows ribbon order.
+ *
+ * d_planes and d_order are memory the context's device can read / write: device memory or pinned host memory
+ * (hnb_host_alloc). Work is only enqueued on the context stream (HNB_BATCH_DEPTH_ORDER_LAUNCHES = 13 launches, whatever
+ * the batch holds); no synchronisation, and no allocation once a context-owned scratch buffer (16 bytes per slab row,
+ * 1 KiB per 4096 live rows and about 4 KiB per instance) has grown to the largest call seen.
+ *
+ * HNB_ERR_INVALID_ARG, with nothing enqueued: every refusal of hnb_batch_bounds; an HNB_EFFECT_RIBBONS effect; `d_planes`
+ * NULL or not 16-byte aligned; `plane_rows` below the batch's instance count; `d_order` NULL; `order_rows` below the
+ * slab's capacity. A batch of zero instances is a no-op. Whatever the device tables hold, no access leaves the slab,
+ * d_planes[0, 4 * plane_rows) or d_order[0, order_rows).
+ */
+HNB_API int32_t hnb_batch_depth_order(hnb_ctx* ctx, const hnb_batch_launch* batch, const float* d_planes, uint32_t plane_rows,
+                                      uint32_t* d_order, uint32_t order_rows);
+
 /* Individual passes, as exercised one by one by the reference's shader contract tests
  * (src/render/shader_contract_tests.rs). They run the un-fused kernels. */
 HNB_API int32_t hnb_pass_init(hnb_ctx* ctx, const hnb_batch_launch* batch);

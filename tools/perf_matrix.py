@@ -541,6 +541,101 @@ def bounds():
     ctx.close()
 
 
+def _timed_depth_order(label, ctx, launch, instances, rows, alive, claimed, extra=""):
+    """hnb_batch_depth_order of `launch`'s batch into a device order buffer of `rows`: one warm-up call, then the best of 5
+    CUDA-event windows. GB/s counts what any depth sort must move: 16 B of position (and 4 B of list where no claim covers
+    the row) read and a 4 B entry written per live particle."""
+    order = torch.empty(rows, dtype=torch.int32, device="cuda")
+    planes = torch.tensor([[0.48, -0.6, 0.64, 0.25]] * instances, dtype=torch.float32, device="cuda")
+    ctx.batch_depth_order(launch, planes.data_ptr(), instances, order.data_ptr(), rows)
+    ms = _events_ms(lambda: ctx.batch_depth_order(launch, planes.data_ptr(), instances, order.data_ptr(), rows))
+    report(f"depth_order: {label}", ms, (20 if claimed else 24) * alive, f"{ms * 1e3:.1f} us per call, {alive >> 10} Ki particles, best of 5{extra}")
+    return order
+
+
+def depth_order():
+    """hnb_batch_depth_order: the filled 64 Mi C5 instance under its claim, the same size spawned by one init burst, C4's
+    topology in one call, the 16 Mi-slot churn steady state and single instances of 4 Ki and 16 Ki (latency), beside a
+    2 GiB device-to-device copy and torch's stable argsort (CUB radix sort) of the same 64 Mi depths, already computed."""
+    _card()
+    a = torch.empty(2 << 30, dtype=torch.uint8, device="cuda")
+    b = torch.empty_like(a)
+    ms = _events_ms(lambda: b.copy_(a))
+    report("depth_order: 2 GiB device-to-device copy", ms, 2 * a.numel(), "torch copy_ (reads 2 GiB and writes 2 GiB), best of 5")
+    del a, b
+    torch.cuda.empty_cache()
+
+    P = 64 << 20
+    ctx = hb.Context(0, stream.cuda_stream)
+    effect = ctx.effect_compile(recipes.c5_lowered())
+    slab = ctx.slab_create(P, 32)
+    ctx.slab_fill_c5(slab, 0, P, 42, 1e9, 1e9)
+    single_instance(ctx, P, 32, alive=P)
+    la = N.BatchLaunch.make(effect, slab, 0, 0)
+    ctx.simulate([la])
+    order = _timed_depth_order("C5 64Mi filled, claim over every row", ctx, la, 1, P, P, True)
+    view = ctx.slab_device_view(slab)
+    col = torch.as_tensor(_DeviceColumn(view.planes[0], (P, 4)), device="cuda")
+    depth = ((col[:, 0] * 0.48 + col[:, 1] * -0.6) + col[:, 2] * 0.64) + 0.25
+    ms = _events_ms(lambda: torch.argsort(depth, descending=True, stable=True))
+    report("depth_order: torch.argsort(stable=True) of the 64Mi depths", ms, 8 * P, "CUB radix sort of float32 keys with int64 indices, best of 5")
+    del order, depth, col
+    ctx.slab_destroy(slab)
+    slab = ctx.slab_create(P, 32)
+    single_instance(ctx, P, 32, alive=0, spawn=P)
+    ctx.simulate([N.BatchLaunch.make(effect, slab, 0, P)])
+    ctx.upload_spawners([R.make_spawner(spawn=0, seed=43)])
+    la = N.BatchLaunch.make(effect, slab, 0, 0)
+    ctx.simulate([la])
+    _timed_depth_order("C5 64Mi from one init burst, no claim", ctx, la, 1, P, P, False)
+    ctx.close()
+    torch.cuda.empty_cache()
+
+    n_inst, cap = 1024, 65536
+    ctx = hb.Context(0, stream.cuda_stream)
+    effect = ctx.effect_compile(recipes.c5_lowered())
+    slab = ctx.slab_create(n_inst * cap, 32)
+    sp = []
+    for i in range(n_inst):
+        ctx.slab_fill_c5(slab, i * cap, cap, 7000 + i, 1e9, 1e9)  # the last fill holds the slab's claim
+        m = R.initial_metadata(cap, i, 8)
+        m.alive_count, m.max_spawn = cap, 0
+        ctx.metadata_insert(i, m)
+        ctx.draw_args_insert(i)
+        sp.append(R.make_spawner(seed=i, effect_metadata_index=i, draw_indirect_index=i, slab_offset=i * cap))
+    ctx.upload_spawners(sp)
+    ctx.upload_batches([N.BatchInfo(0, 0, 0, 0, 0, n_inst)], [0] * n_inst)
+    ctx.set_sim_params(1 / 60, 0.0, n_inst)
+    la = N.BatchLaunch.make(effect, slab, 0, 0)
+    ctx.simulate([la])
+    _timed_depth_order("C4 shape: 1024 x 65536 in one batch", ctx, la, n_inst, n_inst * cap, n_inst * cap, False)
+    ctx.close()
+    torch.cuda.empty_cache()
+
+    for cap in (4096, 16 << 10):
+        ctx = hb.Context(0, stream.cuda_stream)
+        slab = ctx.slab_create(cap, 32)
+        ctx.slab_fill_c5(slab, 0, cap, 100, 1e9, 1e9)
+        single_instance(ctx, cap, 32, alive=cap)
+        la = N.BatchLaunch.make(ctx.effect_compile(recipes.c5_lowered()), slab, 0, 0)
+        ctx.simulate([la])
+        _timed_depth_order(f"one instance of {cap >> 10} Ki particles (latency)", ctx, la, 1, cap, cap, True)
+        ctx.close()
+
+    P, ctx, slab, effect, stride, dt, rate = _churned()
+    alive = ctx.read_metadata(0).alive_count
+    _timed_depth_order(f"churned {P >> 20} Mi slots, {alive >> 10} Ki alive, permuted list", ctx, N.BatchLaunch.make(effect, slab, 0, rate), 1, P,
+                           alive, False)
+    ctx.close()
+
+
+class _DeviceColumn:
+    """A device column as torch sees it through __cuda_array_interface__."""
+
+    def __init__(self, ptr, shape):
+        self.__cuda_array_interface__ = {"shape": shape, "typestr": "<f4", "data": (ptr, False), "version": 2}
+
+
 def fresh_sector():
     """Cost of sector planes when access IS coalesced: C5 recipe burst + update, like `c5_init`, on a sector slab."""
     w = G.ExprWriter()
@@ -783,7 +878,7 @@ def emitter_relocation():
     ctx.close()
 
 
-SCENARIOS = {"c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "bounds": bounds, "emitter_relocation": emitter_relocation, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
+SCENARIOS = {"c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "bounds": bounds, "depth_order": depth_order, "emitter_relocation": emitter_relocation, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
 if __name__ == "__main__":
     for name in (sys.argv[1:] or list(SCENARIOS)):
         try:
