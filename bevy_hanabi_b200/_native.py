@@ -200,6 +200,7 @@ SIGNATURES = {
     "hnb_effect_generate_source": (i32, [P(EffectDesc), C.c_char_p, C.c_size_t, P(C.c_size_t)]),
     "hnb_effect_generate_source_for_plan": (i32, [P(EffectDesc), u32, P(u32), P(u32), C.c_char_p, C.c_size_t, P(C.c_size_t)]),
     "hnb_effect_column_plan": (i32, [P(EffectDesc), P(u32), P(u32), P(u32)]),
+    "hnb_effect_column_words": (i32, [P(EffectDesc), P(u32), P(u32)]),
     "hnb_nvrtc_check": (i32, [C.c_char_p, P(C.c_size_t)]),
     "hnb_set_sim_params": (i32, [vp, P(SimParams)]),
     "hnb_upload_spawners": (i32, [vp, P(Spawner), u32]),

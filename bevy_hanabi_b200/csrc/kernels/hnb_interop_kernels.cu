@@ -40,8 +40,17 @@ __global__ void __launch_bounds__(TR_THREADS) k_transpose(u32* __restrict__ aos,
         const u32 w = planes.words[p], off = planes.word_off[p];
         const bool aligned16 = ((stride_words | off) & 3u) == 0u;
         for (u32 r = threadIdx.x; r < rows; r += TR_THREADS) {
-            u32* t = tr_tile + r * stride_words + off;
             const u64 grow = u64(first) + row0 + r;
+            if (off & HNB_PLANE_WORD_LIST) {  // a word map: lane l <-> its own record word
+                u32* const rec = tr_tile + r * stride_words;
+                u32* const g = (u32*)planes.ptr[p] + grow * w;
+                for (u32 l = 0; l < w; ++l) {
+                    if (TO_AOS) rec[hnb_plane_word(planes, p, l)] = g[l];
+                    else g[l] = rec[hnb_plane_word(planes, p, l)];
+                }
+                continue;
+            }
+            u32* t = tr_tile + r * stride_words + off;
             if (w == 4u) {
                 uint4* g = (uint4*)planes.ptr[p] + grow;
                 if (aligned16) {  // record stride and piece offset multiples of 16 bytes: one 128-bit shared-memory access

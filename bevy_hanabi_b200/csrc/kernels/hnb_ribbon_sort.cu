@@ -38,7 +38,7 @@ constexpr u32 kLargeWarps = kLargeThreads / 32;
 
 __device__ __forceinline__ u32 load_word(const PlaneSet& planes, u32 row, u32 word) {
     const u32 p = planes.word_to_plane[word];
-    return ((const u32*)planes.ptr[p])[u64(row) * planes.words[p] + (word - planes.word_off[p])];
+    return ((const u32*)planes.ptr[p])[u64(row) * planes.words[p] + hnb_word_lane(planes, word)];
 }
 
 struct Instance {

@@ -426,7 +426,7 @@ __global__ void k_fill_c5(PlaneSet planes, u32* ping, u32* pong, u64* claim, u32
 #pragma unroll
     for (u32 w = 0; w < 8; ++w) {
         const u32 p = planes.word_to_plane[w];
-        ((f32*)planes.ptr[p])[u64(row) * planes.words[p] + (w - planes.word_off[p])] = rec[w];
+        ((f32*)planes.ptr[p])[u64(row) * planes.words[p] + hnb_word_lane(planes, w)] = rec[w];
     }
     ping[row] = i;  // instance-local identity alive list in both columns
     pong[row] = i;
@@ -550,7 +550,13 @@ __device__ __forceinline__ void snapshot_column(const SnapshotArgs& a, u32 p, co
     for (u32 k = 0; k < RP_ITEMS; ++k) {
         const u32 i = i0 + k * RP_THREADS;
         if (i >= n) continue;
-        u32* d = dst + HNB_SNAPSHOT_HEADER_WORDS + u64(i) * a.stride_words + off;
+        u32* d = dst + HNB_SNAPSHOT_HEADER_WORDS + u64(i) * a.stride_words;
+        if (off & HNB_PLANE_WORD_LIST) {  // a word map: each lane to its own record word
+#pragma unroll
+            for (u32 l = 0; l < W; ++l) d[hnb_plane_word(a.planes, p, l)] = v[k].w[l];
+            continue;
+        }
+        d += off;
         if (W >= 4 && al == 4u) snapshot_store<4>(d, v[k]);
         else if (W >= 2 && al >= 2u) snapshot_store<2>(d, v[k]);
         else snapshot_store<1>(d, v[k]);
@@ -648,7 +654,13 @@ __device__ __forceinline__ void restore_column(const SnapshotArgs& a, u32 p, u32
         const u32 i = i0 + k * RP_THREADS;
         if (i >= m + dm) continue;
         const u32 r = i < m ? i : n + (i - m);
-        const u32* s = src + HNB_SNAPSHOT_HEADER_WORDS + u64(r) * a.stride_words + off;
+        const u32* s = src + HNB_SNAPSHOT_HEADER_WORDS + u64(r) * a.stride_words;
+        if (off & HNB_PLANE_WORD_LIST) {  // a word map: each lane from its own record word
+#pragma unroll
+            for (u32 l = 0; l < W; ++l) v[k].w[l] = s[hnb_plane_word(a.planes, p, l)];
+            continue;
+        }
+        s += off;
         if (W >= 4 && al == 4u) snapshot_load<4>(s, v[k]);
         else if (W >= 2 && al >= 2u) snapshot_load<2>(s, v[k]);
         else snapshot_load<1>(s, v[k]);
@@ -755,8 +767,7 @@ __global__ void k_checksum(PlaneSet planes, u32 first, u32 count, u32 stride_wor
         u64 h = 0xcbf29ce484222325ull ^ (index_base + u64(i));
         for (u32 w = 0; w < stride_words; ++w) {
             const u32 p = planes.word_to_plane[w];
-            const u32 lane = w - planes.word_off[p];
-            const u32 x = ((const u32*)planes.ptr[p])[u64(first + i) * planes.words[p] + lane];
+            const u32 x = ((const u32*)planes.ptr[p])[u64(first + i) * planes.words[p] + hnb_word_lane(planes, w)];
             h = (h ^ u64(x)) * 0x100000001b3ull;
         }
         h ^= h >> 29; h *= 0xbf58476d1ce4e5b9ull; h ^= h >> 32;

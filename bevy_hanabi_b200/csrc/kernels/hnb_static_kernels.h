@@ -29,9 +29,26 @@ struct StaticTables {
 struct PlaneSet {
     void* ptr[HNB_MAX_PLANES];
     u32 words[HNB_MAX_PLANES];     // u32 words per row of plane p (4, 2 or 1)
-    u32 word_off[HNB_MAX_PLANES];  // first AoS word covered by plane p
+    // The record words plane p holds, in lane order. A plane of consecutive words: the first one. A word map (a column
+    // plan whose column holds words that are not consecutive, DESIGN.md §4.1): HNB_PLANE_WORD_LIST, and lane l's word in
+    // bits [6l, 6l + 6).
+    u32 word_off[HNB_MAX_PLANES];
     unsigned char word_to_plane[HNB_MAX_PLANES * 4];
 };
+#define HNB_PLANE_WORD_LIST 0x80000000u
+// record word of lane `lane` of plane p
+HNB_HD u32 hnb_plane_word(const PlaneSet& s, u32 p, u32 lane) {
+    const u32 o = s.word_off[p];
+    return (o & HNB_PLANE_WORD_LIST) ? (o >> (6u * lane)) & 63u : o + lane;
+}
+// lane of record word w in its plane word_to_plane[w]
+HNB_HD u32 hnb_word_lane(const PlaneSet& s, u32 w) {
+    const u32 o = s.word_off[s.word_to_plane[w]];
+    if (!(o & HNB_PLANE_WORD_LIST)) return w - o;
+    u32 lane = 0;
+    while (lane < 3u && ((o >> (6u * lane)) & 63u) != w) ++lane;
+    return lane;
+}
 
 // Ribbon sort of one batch (hnb_ribbon_sort.cu): every instance of the batch has its freshly written alive-list
 // column stably sorted by (particle[sort_key_offset], particle[sort_key2_offset]).

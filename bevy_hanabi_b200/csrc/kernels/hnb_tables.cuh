@@ -143,8 +143,14 @@ struct BatchParams {
     // lifetimes of the group's particles, or HNB_LIFE_FLOOR_NONE. NULL: the slab uses no floors. Kept out of SlabView so
     // that the parameter offsets, and the code, of effects without floors stay as they were.
     f32* life_floor;
+    // Common ages of the slab (HNB_GROUP_AGE effects, DESIGN.md §3): one 64-bit word per 32 slab rows, (epoch << 32) | the
+    // age bits every row of the group held after the update of frame `epoch`. Only a word of the previous frame's epoch is
+    // known; all bits set: unknown. NULL: the slab keeps none (always NULL when life_floor is).
+    u64* group_age;
 };
 // All bits set: a NaN, against which every comparison is false, so it proves nothing (0.0 would: ages can be negative).
+// Also the unknown common age (an age column whose bits are all ones never has a known common age).
 #define HNB_LIFE_FLOOR_NONE 0xffffffffu
+#define HNB_GROUP_AGE_NONE 0xffffffffffffffffull
 
 }  // namespace hnb

@@ -102,6 +102,10 @@ struct Slab {
     // the update passes get no floors any more, because a view was handed out or a module without floors was bound.
     DeviceArray<uint32_t> life_floor;
     bool floors_off = false;
+    // Common ages (DESIGN.md §3): one word per 32 rows, (epoch << 32) | the age bits of every row of the group, or all bits
+    // set. Cleared with the floors, and at the epoch wrap. `ages_off`: a module without them was bound.
+    DeviceArray<unsigned long long> group_age;
+    bool ages_off = false;
     // HNB_EFFECT_ORDERED_EVENTS scratch, allocated on first use: per channel the per-row event counts and their block sums
     DeviceArray<uint32_t> event_counts[HNB_MAX_EVENT_BINDINGS];
     DeviceArray<uint32_t> event_block_sums[HNB_MAX_EVENT_BINDINGS];
@@ -112,6 +116,7 @@ struct KernelModule {
     CUfunction init = nullptr, update = nullptr;
     int update_blocks_per_sm = 1;
     bool life_floor = false;  // generated with HNB_LIFE_FLOOR: keeps the slab's lifetime floors (and clears them on init)
+    bool group_age = false;   // generated with HNB_GROUP_AGE: keeps the slab's common ages too
     std::string log;
 };
 
@@ -362,6 +367,8 @@ void flush_arena(hnb_ctx* c, bool with_ranges) {
     if (bytes >= c->lay.off_prefix_sum) c->plan_dirty = false;
 }
 
+void clear_life_floors(hnb_ctx* c, const Slab& s);
+
 void next_epoch(hnb_ctx* c) {
     c->epoch = (c->epoch + 1u) & 0x3fffffffu;
     if (c->epoch == 0) {
@@ -370,6 +377,9 @@ void next_epoch(hnb_ctx* c) {
         c->epoch = 1;
         for (const auto& ts : c->d_tile_state)
             if (ts) CUDA_CHECK(cudaMemsetAsync(ts.get(), 0, ts.size() * 8, c->stream));
+        // the same for a common age stored a whole cycle ago (DESIGN.md §3)
+        for (const Slab& s : c->slabs)
+            if (s.live) clear_life_floors(c, s);
     }
     c->header()->epoch = c->epoch;
     c->header()->num_batches = c->B;
@@ -389,8 +399,12 @@ hnb::PlaneSet plane_set(const std::vector<Plane>& planes, char* block, uint32_t 
     for (size_t p = 0; p < planes.size(); ++p) {
         ps.ptr[p] = block + size_t(capacity) * planes[p].offset;
         ps.words[p] = planes[p].width / 4;
-        ps.word_off[p] = planes[p].offset / 4;
-        for (uint32_t w = 0; w < planes[p].width / 4; ++w) ps.word_to_plane[planes[p].offset / 4 + w] = (unsigned char)p;
+        ps.word_off[p] = planes[p].word[0];
+        if (!planes[p].contiguous()) {
+            ps.word_off[p] = HNB_PLANE_WORD_LIST;
+            for (uint32_t l = 0; l < planes[p].width / 4; ++l) ps.word_off[p] |= uint32_t(planes[p].word[l]) << (6 * l);
+        }
+        for (uint32_t l = 0; l < planes[p].width / 4; ++l) ps.word_to_plane[planes[p].word[l]] = (unsigned char)p;
     }
     return ps;
 }
@@ -402,6 +416,7 @@ void clear_life_floors(hnb_ctx* c, const Slab& s, uint32_t first, uint32_t count
     if (count == 0) return;
     const size_t g0 = first / 32u, g1 = (size_t(first) + count + 31u) / 32u;
     CUDA_CHECK(cudaMemsetAsync(s.life_floor.get() + g0, 0xff, (g1 - g0) * sizeof(uint32_t), c->stream));
+    CUDA_CHECK(cudaMemsetAsync(s.group_age.get() + g0, 0xff, (g1 - g0) * sizeof(unsigned long long), c->stream));
 }
 void clear_life_floors(hnb_ctx* c, const Slab& s) { clear_life_floors(c, s, 0, s.capacity); }
 
@@ -487,6 +502,7 @@ KernelModule* get_module(hnb_ctx* c, const std::string& source, const std::strin
     if (r != CUDA_SUCCESS) fail(HNB_ERR_CUDA, "cuModuleGetFunction(hnb_update): " + cu_error_string(c->drv, r));
     km->update_blocks_per_sm = 1;  // depends on the effect's dynamic shared memory (set_update_smem)
     km->life_floor = source.find("\n#define HNB_LIFE_FLOOR 1\n") != std::string::npos;
+    km->group_age = source.find("\n#define HNB_GROUP_AGE 1\n") != std::string::npos;
     KernelModule* out = km.get();
     c->modules.emplace(hash, std::move(km));
     return out;
@@ -700,6 +716,9 @@ void bind_launch(hnb_ctx* c, LaunchPlan& lp, const hnb_batch_launch& bl, bool se
     // reads a floor of it again.
     if (!lp.km->life_floor) slab.floors_off = true;
     P.life_floor = slab.floors_off ? nullptr : reinterpret_cast<float*>(slab.life_floor.get());
+    // The same for common ages: a module without them writes ages without keeping the words true.
+    if (!lp.km->group_age) slab.ages_off = true;
+    P.group_age = slab.floors_off || slab.ages_off ? nullptr : slab.group_age.get();
     if (consume) P.consume_events = c->event_buffers[bl.consume_events].get();
     for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
         if (bl.emit_events[i] == 0xFFFFFFFFu) continue;
@@ -998,6 +1017,7 @@ int32_t hnb_slab_create_ex(hnb_ctx* c, uint32_t capacity_rows, uint32_t stride, 
         CUDA_CHECK(s.ident_claim.alloc(2));
         clear_ident_claims(c, s);
         CUDA_CHECK(s.life_floor.alloc(size_t(capacity_rows) / 32 + 1));
+        CUDA_CHECK(s.group_age.alloc(size_t(capacity_rows) / 32 + 1));
         clear_life_floors(c, s);
         CUDA_CHECK(hnb::launch_slab_reset(s.ping.get(), s.pong.get(), s.dead.get(), 0, capacity_rows, c->stream));
         c->launches++;
@@ -1534,6 +1554,18 @@ int32_t hnb_effect_column_plan(const hnb_effect_desc* desc, uint32_t* offsets, u
     });
 }
 
+int32_t hnb_effect_column_words(const hnb_effect_desc* desc, uint32_t* words, uint32_t* n) {
+    return guarded([&] {
+        if (!desc || !n) fail(HNB_ERR_INVALID_ARG, "NULL argument");
+        const std::vector<Plane> plan = column_plan(desc->particle_stride, desc->attrs, desc->attrs ? desc->n_attrs : 0, desc->flags);
+        uint32_t k = 0;
+        for (const Plane& p : plan)
+            for (uint32_t l = 0; l < p.width / 4; ++l, ++k)
+                if (words) words[k] = p.word[l];
+        *n = k;
+    });
+}
+
 int32_t hnb_nvrtc_check(const char* source, size_t* cubin_size) {
     return guarded([&] {
         std::string cubin, log;
@@ -1921,9 +1953,10 @@ static hnb::BoundsArgs batch_position_args(hnb_ctx* c, const hnb_batch_launch* b
         const uint32_t word = bp.position->offset / 4 + k, p = ps.word_to_plane[word];
         a.col[k] = static_cast<const uint32_t*>(ps.ptr[p]);
         a.col_words[k] = ps.words[p];
-        a.col_lane[k] = word - ps.word_off[p];
+        a.col_lane[k] = hnb::hnb_word_lane(ps, word);
     }
-    *fast = a.col[2] == a.col[0] && (a.col_lane[0] & 3u) == 0 && (a.col_words[0] & 3u) == 0;
+    *fast = a.col[2] == a.col[0] && (a.col_lane[0] & 3u) == 0 && (a.col_words[0] & 3u) == 0 && a.col_lane[1] == a.col_lane[0] + 1 &&
+            a.col_lane[2] == a.col_lane[0] + 2;
     return a;
 }
 

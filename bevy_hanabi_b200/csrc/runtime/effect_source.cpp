@@ -93,17 +93,63 @@ bool any_read_only(const hnb_attr_layout* attrs, uint32_t n_attrs) {
     return false;
 }
 
-}  // namespace
+const hnb_attr_layout* find_attr(const hnb_attr_layout* attrs, uint32_t n_attrs, const char* name) {
+    for (uint32_t i = 0; i < n_attrs; ++i)
+        if (!strcmp(attrs[i].name, name)) return &attrs[i];
+    return nullptr;
+}
 
-std::vector<Plane> column_plan(uint32_t stride, const hnb_attr_layout* attrs, uint32_t n_attrs, uint32_t effect_flags) {
-    if (effect_flags & HNB_EFFECT_SECTOR_PLANES) return physical_planes(stride, true);
-    std::vector<Plane> cut = cut_planes(stride);
-    if ((effect_flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS) || !any_read_only(attrs, n_attrs)) return cut;
-    const std::vector<bool> written = written_words(stride, attrs, n_attrs);
+// Lifetime floors (DESIGN.md §3) need an f32 lifetime flagged HNB_ATTR_REAP_ONLY and read-only (so the column is never
+// stored and only the standard age / reap code compares it), an f32 age, and the ordered pass (the floor is kept per 32
+// rows of an identity-claimed tile). Slot order keeps none: there inits clear the floors of many groups every frame, and
+// the lifetime loads those groups then need, issued behind the age, cost more than the floors save. The lifetime also
+// needs a 4-byte column of its own in the slab's plan (life_floor_plane).
+bool keeps_floors(const hnb_attr_layout* attrs, uint32_t n_attrs, uint32_t effect_flags) {
+    if (effect_flags & (HNB_EFFECT_SECTOR_PLANES | HNB_EFFECT_RELAXED_ORDER | HNB_EFFECT_SLOT_ORDER)) return false;
+    const hnb_attr_layout* life = find_attr(attrs, n_attrs, "lifetime");
+    const hnb_attr_layout* age = find_attr(attrs, n_attrs, "age");
+    const uint32_t need = HNB_ATTR_UPDATE_READ_ONLY | HNB_ATTR_REAP_ONLY;
+    return life && age && life->value_type == HNB_FLOAT && age->value_type == HNB_FLOAT && (life->flags & need) == need;
+}
+
+// The word map of an effect with floors: the age and the lifetime in f32 columns of their own (the update may then skip
+// either load), the other written words packed in record order into 16-, 8- and 4-byte columns, then the other unwritten
+// words the same way. Columns are laid out widest first, so each sits at a multiple of its width in the slab block.
+std::vector<Plane> word_map_plan(uint32_t stride, const hnb_attr_layout* attrs, uint32_t n_attrs, const std::vector<bool>& written) {
+    const uint32_t age = find_attr(attrs, n_attrs, "age")->offset / 4, life = find_attr(attrs, n_attrs, "lifetime")->offset / 4;
+    std::vector<Plane> cols;
+    auto pack = [&](const std::vector<uint32_t>& words) {
+        for (size_t i = 0; i < words.size();) {
+            const size_t left = words.size() - i, n = left >= 4 ? 4 : left >= 2 ? 2 : 1;
+            Plane p;
+            p.width = uint32_t(4 * n);
+            for (size_t l = 0; l < n; ++l) p.word[l] = uint8_t(words[i + l]);
+            cols.push_back(p);
+            i += n;
+        }
+    };
+    std::vector<uint32_t> w_words, r_words;
+    for (uint32_t w = 0; w < stride / 4; ++w)
+        if (w != age && w != life) (written[w] ? w_words : r_words).push_back(w);
+    pack(w_words);
+    pack({age});
+    pack({life});
+    pack(r_words);
+    std::stable_sort(cols.begin(), cols.end(), [](const Plane& a, const Plane& b) { return a.width > b.width; });
+    uint32_t off = 0;
+    for (Plane& p : cols) {
+        p.offset = off;
+        off += p.width;
+    }
+    return cols;
+}
+
+// Runs of written / unwritten words, each cut into aligned columns.
+std::vector<Plane> column_plan_runs(uint32_t stride, const std::vector<bool>& written) {
     std::vector<Plane> out;
-    for (uint32_t w = 0; w < written.size();) {
+    for (uint32_t w = 0; w < stride / 4;) {
         uint32_t end = w;
-        while (end < written.size() && written[end] == written[w]) ++end;
+        while (end < stride / 4 && written[end] == written[w]) ++end;
         // a column of width W starts at a multiple of W: a slab block carves it at capacity * offset bytes, aligned for
         // W-byte loads whatever the capacity
         for (uint32_t off = 4 * w; off < 4 * end;) {
@@ -114,7 +160,25 @@ std::vector<Plane> column_plan(uint32_t stride, const hnb_attr_layout* attrs, ui
         }
         w = end;
     }
-    return out.size() > HNB_RT_MAX_PLANES ? cut : out;
+    return out;
+}
+
+}  // namespace
+
+std::vector<Plane> column_plan(uint32_t stride, const hnb_attr_layout* attrs, uint32_t n_attrs, uint32_t effect_flags) {
+    if (effect_flags & HNB_EFFECT_SECTOR_PLANES) return physical_planes(stride, true);
+    std::vector<Plane> cut = cut_planes(stride);
+    if ((effect_flags & HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS) || !any_read_only(attrs, n_attrs)) return cut;
+    const std::vector<bool> written = written_words(stride, attrs, n_attrs);
+    std::vector<Plane> out = column_plan_runs(stride, written);
+    if (out.size() > HNB_RT_MAX_PLANES) return cut;
+    // An effect whose lifetime the runs already give a 4-byte column (so that it keeps floors) gets the word map, unless that
+    // takes more columns: a gathered record would then touch more sectors.
+    if (!keeps_floors(attrs, n_attrs, effect_flags)) return out;
+    const uint32_t life = find_attr(attrs, n_attrs, "lifetime")->offset;
+    if (std::none_of(out.begin(), out.end(), [&](const Plane& p) { return p.offset == life && p.width == 4; })) return out;
+    std::vector<Plane> map = word_map_plan(stride, attrs, n_attrs, written);
+    return map.size() <= out.size() ? map : out;
 }
 
 bool is_default_cut(const std::vector<Plane>& plan, uint32_t stride) { return plan == cut_planes(stride); }
@@ -126,12 +190,45 @@ const char* comp_name(int c) {
     return n[c];
 }
 
+// A plan with a column whose words are not consecutive: its RawParticle holds the record words in record order (w0, w1,
+// ...), so that it is the AoS record, and each column load or store moves its words to or from their places.
+bool is_word_map(const std::vector<Plane>& planes) {
+    return std::any_of(planes.begin(), planes.end(), [](const Plane& p) { return !p.contiguous(); });
+}
+
 // lvalue of word `word_in_plane` of plane p inside RawParticle
-std::string raw_word(const Plane& pl, size_t p, uint32_t word_in_plane) {
+std::string raw_word(const Plane& pl, size_t p, uint32_t word_in_plane, bool mapped = false) {
     std::ostringstream s;
+    if (mapped) {
+        s << "r.w" << unsigned(pl.word[word_in_plane]);
+        return s.str();
+    }
     s << "r.q" << p;
     if (pl.width > 4) s << "." << comp_name((int)word_in_plane);
     return s.str();
+}
+
+const char* plane_type(const Plane& pl) { return pl.width == 16 ? "float4" : pl.width == 8 ? "float2" : "f32"; }
+
+// Statements loading column p of row `row` into RawParticle r, of a word map (the other plans load r.qP directly).
+std::string mapped_load(const Plane& pl, size_t p, const std::string& address) {
+    std::ostringstream s;
+    if (pl.width == 4) {
+        s << "    " << raw_word(pl, p, 0, true) << " = HNB_LOAD_PLANE(f32, " << address << ");\n";
+        return s.str();
+    }
+    s << "    { const " << plane_type(pl) << " v = HNB_LOAD_PLANE(" << plane_type(pl) << ", " << address << ");";
+    for (uint32_t l = 0; l < pl.width / 4; ++l) s << " " << raw_word(pl, p, l, true) << " = v." << comp_name(int(l)) << ";";
+    s << " }\n";
+    return s.str();
+}
+
+// The value of column p a store of a word map writes.
+std::string mapped_value(const Plane& pl, size_t p) {
+    if (pl.width == 4) return raw_word(pl, p, 0, true);
+    std::string s = std::string("make_") + plane_type(pl) + "(";
+    for (uint32_t l = 0; l < pl.width / 4; ++l) s += (l ? ", " : "") + raw_word(pl, p, l, true);
+    return s + ")";
 }
 
 struct FieldRef {
@@ -178,16 +275,23 @@ void gen_layout_code(std::ostringstream& o, const char* prefix, const char* stru
         }
     }
     o << "};\n";
+    const bool mapped = is_word_map(planes);
     o << "struct " << prefix << "RawParticle {\n";
-    for (size_t p = 0; p < planes.size(); ++p)
-        o << "    " << (planes[p].width == 16 ? "float4" : planes[p].width == 8 ? "float2" : "f32") << " q" << p << ";\n";
+    if (mapped) {
+        for (uint32_t w = 0; w < stride / 4; ++w) o << "    f32 w" << w << ";\n";
+    } else {
+        for (size_t p = 0; p < planes.size(); ++p)
+            o << "    " << (planes[p].width == 16 ? "float4" : planes[p].width == 8 ? "float2" : "f32") << " q" << p << ";\n";
+    }
     o << "};\n";
     const std::string raw_t = std::string(prefix) + "RawParticle";
     std::string fn_prefix = std::string("hnb_") + (strlen(prefix) ? "parent_" : "");
     // zero
     o << "HNB_DI void " << fn_prefix << "raw_zero(" << raw_t << "& r) {\n";
     for (size_t p = 0; p < planes.size(); ++p) {
-        if (planes[p].width == 16) o << "    r.q" << p << " = make_float4(0.f, 0.f, 0.f, 0.f);\n";
+        if (mapped) {
+            for (uint32_t l = 0; l < planes[p].width / 4; ++l) o << "    " << raw_word(planes[p], p, l, true) << " = 0.f;\n";
+        } else if (planes[p].width == 16) o << "    r.q" << p << " = make_float4(0.f, 0.f, 0.f, 0.f);\n";
         else if (planes[p].width == 8) o << "    r.q" << p << " = make_float2(0.f, 0.f);\n";
         else o << "    r.q" << p << " = 0.f;\n";
     }
@@ -196,14 +300,16 @@ void gen_layout_code(std::ostringstream& o, const char* prefix, const char* stru
     o << "HNB_DI void " << fn_prefix << "load_raw(" << raw_t << "& r, const SlabView& s, u32 row) {\n";
     for (size_t p = 0; p < planes.size(); ++p) {
         const char* t = planes[p].width == 16 ? "float4" : planes[p].width == 8 ? "float2" : "f32";
-        o << "    r.q" << p << " = HNB_LOAD_PLANE(" << t << ", " << piece_address(planes, p, sector) << ");\n";
+        if (mapped) o << mapped_load(planes[p], p, piece_address(planes, p, sector));
+        else o << "    r.q" << p << " = HNB_LOAD_PLANE(" << t << ", " << piece_address(planes, p, sector) << ");\n";
     }
     o << "}\n";
     if (with_store) {
+        const auto value = [&](size_t p) { return mapped ? mapped_value(planes[p], p) : "r.q" + std::to_string(p); };
         o << "HNB_DI void " << fn_prefix << "store_raw(const " << raw_t << "& r, const SlabView& s, u32 row) {\n";
         for (size_t p = 0; p < planes.size(); ++p) {
             const char* t = planes[p].width == 16 ? "float4" : planes[p].width == 8 ? "float2" : "f32";
-            o << "    HNB_STORE_PLANE(" << t << ", " << piece_address(planes, p, sector) << ", r.q" << p << ");\n";
+            o << "    HNB_STORE_PLANE(" << t << ", " << piece_address(planes, p, sector) << ", " << value(p) << ");\n";
         }
         o << "}\n";
         // The update's store: the pieces holding a word the update may write. With no read-only attribute, every piece
@@ -213,10 +319,10 @@ void gen_layout_code(std::ostringstream& o, const char* prefix, const char* stru
         o << "HNB_DI void " << fn_prefix << "store_written(const " << raw_t << "& r, const SlabView& s, u32 row) {\n";
         for (size_t p = 0; p < planes.size(); ++p) {
             bool store = all;
-            for (uint32_t w = 0; w < planes[p].width / 4; ++w) store = store || written[planes[p].offset / 4 + w];
+            for (uint32_t w = 0; w < planes[p].width / 4; ++w) store = store || written[planes[p].word[w]];
             if (!store) continue;
             const char* t = planes[p].width == 16 ? "float4" : planes[p].width == 8 ? "float2" : "f32";
-            o << "    HNB_STORE_PLANE(" << t << ", " << piece_address(planes, p, sector) << ", r.q" << p << ");\n";
+            o << "    HNB_STORE_PLANE(" << t << ", " << piece_address(planes, p, sector) << ", " << value(p) << ");\n";
         }
         o << "}\n";
     }
@@ -224,9 +330,9 @@ void gen_layout_code(std::ostringstream& o, const char* prefix, const char* stru
     o << "HNB_DI void " << fn_prefix << "unpack(const " << raw_t << "& r, " << struct_name << "& p) {\n";
     for (size_t p = 0; p < planes.size(); ++p) {
         for (uint32_t w = 0; w < planes[p].width / 4; ++w) {
-            const auto& f = words[planes[p].offset / 4 + w];
+            const auto& f = words[planes[p].word[w]];
             if (f.expr.empty()) continue;  // padding word
-            std::string src = raw_word(planes[p], p, w);
+            std::string src = raw_word(planes[p], p, w, mapped);
             if (f.kind == 'f') o << "    " << f.expr << " = " << src << ";\n";
             else if (f.kind == 'u') o << "    " << f.expr << " = __float_as_uint(" << src << ");\n";
             else o << "    " << f.expr << " = __float_as_int(" << src << ");\n";
@@ -237,10 +343,10 @@ void gen_layout_code(std::ostringstream& o, const char* prefix, const char* stru
         o << "template <bool HNB_LINKS> HNB_DI void " << fn_prefix << "pack(const " << struct_name << "& p, " << raw_t << "& r) {\n";
         for (size_t p = 0; p < planes.size(); ++p) {
             for (uint32_t w = 0; w < planes[p].width / 4; ++w) {
-                uint32_t aw = planes[p].offset / 4 + w;
+                uint32_t aw = planes[p].word[w];
                 const auto& f = words[aw];
                 if (f.expr.empty()) continue;
-                std::string dst = raw_word(planes[p], p, w);
+                std::string dst = raw_word(planes[p], p, w, mapped);
                 if (skip_pack[aw]) {
                     o << "    if (HNB_LINKS) ";
                 } else {
@@ -270,41 +376,51 @@ const hnb_attr_layout* find_attr(const hnb_effect_desc& d, const char* name) {
 }
 
 // Lifetime floors (DESIGN.md §3): the column of `planes` that holds the lifetime and nothing else, when the update pass of
-// this effect may prove particles alive from a floor instead of loading it; -1 otherwise. That needs an f32 lifetime flagged
-// HNB_ATTR_REAP_ONLY and read-only (so the column is never stored and only the standard age / reap code compares it), an f32
-// age, and the ordered pass (the floor is kept per 32 rows of an identity-claimed tile). Slot order keeps none: there
-// inits clear the floors of many groups every frame, and the lifetime loads those groups then need, issued behind the
-// age, cost more than the floors save.
+// this effect may prove particles alive from a floor instead of loading it (keeps_floors); -1 otherwise.
 int life_floor_plane(const hnb_effect_desc& d, const std::vector<Plane>& planes, bool sector) {
-    if (sector || (d.flags & (HNB_EFFECT_RELAXED_ORDER | HNB_EFFECT_SLOT_ORDER))) return -1;
-    const hnb_attr_layout* life = find_attr(d, "lifetime");
-    const hnb_attr_layout* age = find_attr(d, "age");
-    const uint32_t need = HNB_ATTR_UPDATE_READ_ONLY | HNB_ATTR_REAP_ONLY;
-    if (!life || !age || life->value_type != HNB_FLOAT || age->value_type != HNB_FLOAT || (life->flags & need) != need) return -1;
+    if (sector || !keeps_floors(d.attrs, d.n_attrs, d.flags)) return -1;
+    const uint32_t life = find_attr(d, "lifetime")->offset / 4;
     for (size_t p = 0; p < planes.size(); ++p)
-        if (planes[p].offset == life->offset && planes[p].width == 4) return int(p);
+        if (planes[p].word[0] == life && planes[p].width == 4) return int(p);
     return -1;
 }
 
 // The accessors hnb_update uses with HNB_LIFE_FLOOR: every column load but the lifetime's, the lifetime load, the age word
-// and the lifetime word of a RawParticle.
+// and the lifetime word of a RawParticle. In a word map whose age has a column of its own, HNB_GROUP_AGE too (common ages,
+// DESIGN.md §3): every column load but the lifetime's and the age's, the age load, and a store of the age word. Other
+// plans generate what they generated before word maps.
 void gen_life_floor_code(std::ostringstream& o, const hnb_effect_desc& d, const std::vector<Plane>& planes, int life_plane) {
-    const uint32_t age_off = find_attr(d, "age")->offset;
+    const uint32_t age_word = find_attr(d, "age")->offset / 4;
     size_t age_plane = 0;
-    while (!(planes[age_plane].offset <= age_off && age_off < planes[age_plane].offset + planes[age_plane].width)) ++age_plane;
+    uint32_t age_lane = 0;
+    for (size_t p = 0; p < planes.size(); ++p)
+        for (uint32_t l = 0; l < planes[p].width / 4; ++l)
+            if (planes[p].word[l] == age_word) age_plane = p, age_lane = l;
+    const bool mapped = is_word_map(planes);
+    const auto load = [&](size_t p) {
+        const std::string address = "s.planes[" + std::to_string(p) + "], row";
+        if (mapped) return mapped_load(planes[p], p, address);
+        return "    r.q" + std::to_string(p) + " = HNB_LOAD_PLANE(" + plane_type(planes[p]) + ", " + address + ");\n";
+    };
+    const std::string life = raw_word(planes[life_plane], life_plane, 0, mapped), age = raw_word(planes[age_plane], age_plane, age_lane, mapped);
     o << "#define HNB_LIFE_FLOOR 1\n";
     o << "HNB_DI void hnb_load_raw_but_life(RawParticle& r, const SlabView& s, u32 row) {\n";
-    for (size_t p = 0; p < planes.size(); ++p) {
-        if (int(p) == life_plane) continue;
-        const char* t = planes[p].width == 16 ? "float4" : planes[p].width == 8 ? "float2" : "f32";
-        o << "    r.q" << p << " = HNB_LOAD_PLANE(" << t << ", s.planes[" << p << "], row);\n";
-    }
+    for (size_t p = 0; p < planes.size(); ++p)
+        if (int(p) != life_plane) o << load(p);
     o << "}\n";
-    o << "HNB_DI void hnb_load_life(RawParticle& r, const SlabView& s, u32 row) { r.q" << life_plane << " = HNB_LOAD_PLANE(f32, s.planes["
+    o << "HNB_DI void hnb_load_life(RawParticle& r, const SlabView& s, u32 row) { " << life << " = HNB_LOAD_PLANE(f32, s.planes["
       << life_plane << "], row); }\n";
-    o << "HNB_DI f32 hnb_raw_age(const RawParticle& r) { return "
-      << raw_word(planes[age_plane], age_plane, (age_off - planes[age_plane].offset) / 4) << "; }\n";
-    o << "HNB_DI f32& hnb_raw_life(RawParticle& r) { return r.q" << life_plane << "; }\n";
+    o << "HNB_DI f32 hnb_raw_age(const RawParticle& r) { return " << age << "; }\n";
+    o << "HNB_DI f32& hnb_raw_life(RawParticle& r) { return " << life << "; }\n";
+    if (!mapped || planes[age_plane].width != 4) return;  // common ages come with word maps only
+    o << "#define HNB_GROUP_AGE 1\n";
+    o << "HNB_DI void hnb_load_raw_but_life_age(RawParticle& r, const SlabView& s, u32 row) {\n";
+    for (size_t p = 0; p < planes.size(); ++p)
+        if (int(p) != life_plane && p != age_plane) o << load(p);
+    o << "}\n";
+    o << "HNB_DI void hnb_load_age(RawParticle& r, const SlabView& s, u32 row) { " << age << " = HNB_LOAD_PLANE(f32, s.planes["
+      << age_plane << "], row); }\n";
+    o << "HNB_DI void hnb_set_raw_age(RawParticle& r, f32 age) { " << age << " = age; }\n";
 }
 
 }  // namespace
@@ -346,9 +462,14 @@ uint32_t choose_tile_k(const hnb_effect_desc& d) {
 
 void check_plan(const std::vector<Plane>& plan, uint32_t stride) {
     uint32_t off = 0;
+    std::vector<bool> seen(stride / 4, false);
     for (const Plane& p : plan) {
         if (p.offset != off || (p.width != 4 && p.width != 8 && p.width != 16) || p.offset % p.width)
             throw std::invalid_argument("column plan: columns must be contiguous, 4, 8 or 16 bytes wide and aligned to their width");
+        for (uint32_t l = 0; l < p.width / 4; ++l) {
+            if (p.word[l] >= seen.size() || seen[p.word[l]]) throw std::invalid_argument("column plan: every record word must be in one column");
+            seen[p.word[l]] = true;
+        }
         off += p.width;
     }
     if (off != stride || plan.empty() || plan.size() > HNB_RT_MAX_PLANES) throw std::invalid_argument("column plan does not cover the particle record");

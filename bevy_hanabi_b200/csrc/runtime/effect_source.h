@@ -18,11 +18,28 @@ struct ValueTypeInfo {
 };
 ValueTypeInfo value_type_info(uint32_t value_type);
 
-// One SoA plane: bytes [offset, offset+width) of the reference AoS record; width is 16, 8 or 4.
+// One SoA plane: `width` bytes (16, 8 or 4; 32 for a sector-plane column) per row, at capacity x `offset` bytes of the slab
+// block, holding record words word[0 .. width/4) in lane order. Plane{offset, width} is the piece [offset, offset + width)
+// of the reference AoS record; a word map (column_plan) may give a column words that are not consecutive.
 struct Plane {
-    uint32_t offset;
-    uint32_t width;
-    bool operator==(const Plane& o) const { return offset == o.offset && width == o.width; }
+    uint32_t offset = 0, width = 0;
+    uint8_t word[8] = {};
+    Plane() = default;
+    Plane(uint32_t off, uint32_t w) : offset(off), width(w) {
+        for (uint32_t l = 0; l < w / 4 && l < 8; ++l) word[l] = uint8_t(off / 4 + l);
+    }
+    bool contiguous() const {
+        for (uint32_t l = 0; l < width / 4; ++l)
+            if (word[l] != offset / 4 + l) return false;
+        return true;
+    }
+    bool operator==(const Plane& o) const {
+        if (offset != o.offset || width != o.width) return false;
+        for (uint32_t l = 0; l < width / 4; ++l)
+            if (word[l] != o.word[l]) return false;
+        return true;
+    }
+    bool operator!=(const Plane& o) const { return !(*this == o); }
 };
 // Cut an AoS record of `stride_bytes` into planes: as many 16-byte planes as fit, then an 8- and/or
 // 4-byte tail. Because the reference layout keeps vec3/vec4 16-byte aligned and vec2 8-byte aligned
@@ -31,10 +48,13 @@ std::vector<Plane> cut_planes(uint32_t stride_bytes);
 // Physical columns of a slab: the pieces themselves, or (sector planes) pairs of 16-byte pieces in 32-byte-wide columns.
 std::vector<Plane> physical_planes(uint32_t stride_bytes, bool sector_planes);
 // The effect's column plan (hnb_effect_column_plan): the default cut unless some attribute is HNB_ATTR_UPDATE_READ_ONLY;
-// then runs of written / unwritten words get columns of their own, so the update stores only columns it writes.
+// then runs of written / unwritten words get columns of their own, so the update stores only columns it writes. An effect
+// that keeps lifetime floors gets a word map instead (DESIGN.md §4.1): the age and the lifetime in f32 columns of their own,
+// the other words packed, unless that takes more columns than the runs do.
 std::vector<Plane> column_plan(uint32_t stride_bytes, const hnb_attr_layout* attrs, uint32_t n_attrs, uint32_t effect_flags);
 bool is_default_cut(const std::vector<Plane>& plan, uint32_t stride_bytes);
-// Throws std::invalid_argument unless `plan` is contiguous 4/8/16-byte columns, each aligned to its width, covering the record.
+// Throws std::invalid_argument unless `plan` is 4/8/16-byte columns laid out back to back in the slab block, each aligned to
+// its width, whose words are every record word once.
 void check_plan(const std::vector<Plane>& plan, uint32_t stride_bytes);
 
 // Update tiles are walked by one warp each: tile_rows = 32 lanes * k rows per lane * chunks. k is

@@ -99,8 +99,20 @@ class LoweredEffect:
         check(lib.hnb_effect_column_plan(C.byref(d), off, wid, C.byref(n)))
         return [(off[i], wid[i]) for i in range(n.value)]
 
+    def column_words(self) -> list[list[int]]:
+        """The record words each column of column_plan() holds, in lane order (hnb_effect_column_words)."""
+        d, _keep = self.to_c()
+        words, n = (C.c_uint32 * 64)(), C.c_uint32()
+        check(lib.hnb_effect_column_words(C.byref(d), words, C.byref(n)))
+        out, k = [], 0
+        for _, width in self.column_plan():
+            out.append(list(words[k:k + width // 4]))
+            k += width // 4
+        return out
+
     def generate_source_for_plan(self, plan: Sequence[tuple[int, int]]) -> str:
-        """The translation unit a context compiles for this effect on a slab of column plan `plan`."""
+        """The translation unit a context compiles for this effect on a slab of column plan `plan`, whose column p holds
+        record bytes [offset, offset + width) (a word map cannot be named: see hnb_effect_generate_source_for_plan)."""
         d, _keep = self.to_c()
         off = (C.c_uint32 * 16)(*[o for o, _ in plan])
         wid = (C.c_uint32 * 16)(*[w for _, w in plan])

@@ -385,7 +385,8 @@ HNB_API int32_t hnb_slab_checksum_indirect(hnb_ctx* ctx, hnb_slab slab, uint32_t
  * context stream and involve no host copy. `d_*` pointers are DEVICE pointers. */
 typedef struct hnb_slab_view {
     uint32_t capacity_rows, particle_stride, num_planes, _pad;
-    void* planes[16];          /* column p holds bytes [plane_offset[p], +plane_width[p]) of every record, capacity_rows elements */
+    void* planes[16];          /* column p holds bytes [plane_offset[p], +plane_width[p]) of every record, capacity_rows elements;
+                                  in a word map (hnb_effect_column_plan) it holds the words hnb_effect_column_words names */
     uint32_t plane_offset[16];
     uint32_t plane_width[16];  /* 16, 8 or 4 bytes (32 with HNB_SLAB_SECTOR_PLANES: two 16-byte pieces per element) */
     uint32_t *ping, *pong, *dead; /* the three u32 columns of IndirectEntry */
@@ -538,20 +539,33 @@ HNB_API int32_t hnb_effect_create_from_job(hnb_ctx* ctx, hnb_compile_job* job, h
  * in *len. Used by the CPU test-suite (≙ the reference's naga validation tests).
  */
 HNB_API int32_t hnb_effect_generate_source(const hnb_effect_desc* desc, char* out, size_t cap, size_t* len);
-/** The effect's column plan (no GPU needed): *n columns, column p holding bytes [offsets[p], offsets[p] + widths[p]) of
- *  every record (at most 16; `offsets` / `widths` may be NULL to ask for *n only). A pure function of the stride, the
- *  attributes' offsets and HNB_ATTR_UPDATE_READ_ONLY flags, and the effect flags:
+/** The effect's column plan (no GPU needed): *n columns, column p taking widths[p] bytes per row at capacity x offsets[p]
+ *  bytes of the slab's block (at most 16; `offsets` / `widths` may be NULL to ask for *n only). Unless the plan is a word
+ *  map (below), column p holds bytes [offsets[p], offsets[p] + widths[p]) of every record. A pure function of the stride,
+ *  the attributes' offsets and flags, and the effect flags:
  *   - no read-only attribute, HNB_EFFECT_SECTOR_PLANES or HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS: the default cut (as many
  *     16-byte columns as fit, then an 8- and/or 4-byte tail; 32-byte-wide pairs with sector planes). Children read a
  *     parent slab in the default cut;
+ *   - an effect that keeps lifetime floors (an ordered pass, an f32 age, an f32 lifetime flagged
+ *     HNB_ATTR_UPDATE_READ_ONLY | HNB_ATTR_REAP_ONLY): a word map. The age and the lifetime get 4-byte columns of their
+ *     own, the other words the update may write are packed in record order into 16-, 8- and 4-byte columns, then the
+ *     other words the same way; columns are laid out widest first. hnb_effect_column_words tells which record words each
+ *     column holds. The authored C5: [0,16) = position, velocity.x; [16,24) = velocity.yz; [24,28) = age;
+ *     [28,32) = lifetime. When the map would take more columns than the rule below, that rule applies;
  *   - otherwise every maximal run of words of one class (written by the update, or not: read-only attributes and
  *     padding) is cut into 16-, 8- and 4-byte columns, each at an offset that is a multiple of its width.
  *     C5 with a read-only lifetime: [0,16) [16,24) [24,28) [28,32). A plan of more than 16 columns falls back to the
  *     default cut. */
 HNB_API int32_t hnb_effect_column_plan(const hnb_effect_desc* desc, uint32_t* offsets, uint32_t* widths, uint32_t* n);
+/** The record words (4-byte words of the reference AoS record) the columns of hnb_effect_column_plan hold: words[k] for
+ *  k < *n = particle_stride / 4, column 0's lanes first, then column 1's, and so on (widths[p] / 4 lanes each). `words`
+ *  may be NULL to ask for *n only. */
+HNB_API int32_t hnb_effect_column_words(const hnb_effect_desc* desc, uint32_t* words, uint32_t* n);
 /** hnb_effect_generate_source for the module a context compiles when the effect is bound to a slab whose plan is
  *  `n_planes` columns (`offsets`, `widths`) other than its own: the update stores every column holding a word it may
- *  write. */
+ *  write. The columns named here hold the record bytes [offsets[p], offsets[p] + widths[p]): a word map cannot be named,
+ *  so for a word-map effect, passing its own hnb_effect_column_plan gives the module of a slab cut that way, not its own
+ *  module (which hnb_effect_generate_source gives). */
 HNB_API int32_t hnb_effect_generate_source_for_plan(const hnb_effect_desc* desc, uint32_t n_planes, const uint32_t* offsets,
                                                     const uint32_t* widths, char* out, size_t cap, size_t* len);
 /** NVRTC-compile a translation unit for sm_90a without loading it (no GPU needed). On failure
