@@ -321,7 +321,11 @@ struct PendingTile {
     u32 tile_valid;  // slot order: rows of the tile that were alive before the pass
     // identity claims as read when the instance was bound (a parked tile may be compacted after the instance's last tile has
     // rewritten the claim): read-column rows known to be the identity, length of the write column's claim for this instance
-    u32 trust_r, claim_w, _pad[2];
+    u32 trust_r, claim_w;
+    // not a field of the parked tile: lane 0's running count, over the tile being streamed, of the common-age words it made
+    // deferred less those it found deferred (HNB_GROUP_AGE; kept here rather than in a register, which hnb_update lacks)
+    u32 defer_delta;
+    u32 _pad;
 };
 static_assert(sizeof(PendingTile) == 64, "update_smem_bytes on the host reserves 64 bytes per warp for the parked tile");
 
@@ -539,6 +543,9 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
     // any (streamed != 0), the other one. One counter rather than a buffer index and a has-parked flag: the extra live
     // register made the slot-order and force-field builds of hnb_update spill.
     u32 streamed = 0u;
+#if HNB_GROUP_AGE
+    if (lane == 0) parked->defer_delta = 0u;
+#endif
 
     // cached descriptor of the instance the current tile belongs to (reloaded when a tile leaves
     // [inst_first_tile, inst_end_tile))
@@ -691,19 +698,43 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
         // starts on a 32-row group, row group k of a sub-tile is one slab group, and it lies wholly inside the instance's
         // slice (its rows are below max_update <= capacity): a group shared by two instances is neither read nor stored.
         // P.life_floor is NULL when the slab uses no floors. Any other tile loads whole records, as without floors.
-        const bool floors = P.life_floor != nullptr && tile_known && (base_particle & 31u) == 0u;  // warp-uniform
+        const bool tile_floors = P.life_floor != nullptr && tile_known && (base_particle & 31u) == 0u;  // warp-uniform
 #endif
 #if HNB_GROUP_AGE
         // Common ages (DESIGN.md §3) are read and stored in the same tiles as the floors. P.group_age is NULL when the slab
         // keeps none. A word counts only when the previous frame's update stored it: rows of a group that frame updated
         // outside a floor tile (a tile size or claim that changed, a batch that sat out) leave the word an older epoch.
-        const bool ages = floors && P.group_age != nullptr;  // warp-uniform
+        const bool tile_ages = tile_floors && P.group_age != nullptr;  // warp-uniform
+        // With P.defer_ages a floor tile may leave a group's word deferred: the word then holds the age of all 32 rows and
+        // their age column is stale. Such a group can also reach a tile that is not a floor tile (a tile size or claim that
+        // changed, deaths elsewhere that made the list a gather): there each row reads its group's word next to its record
+        // loads, takes the deferred age, stores its age as usual, and counts itself in the word (below).
+        // Reading every row's word made the churned update 3.4 % slower on the H100 where nothing was deferred: the slab's
+        // count of deferred words (hnb_deferred_groups) gates it.
+        const bool tile_defer_rows = !tile_ages && P.defer_ages != 0u && P.group_age != nullptr &&
+                                     *hnb_deferred_groups(P.group_age, P.slab.capacity_rows) != 0ull;  // warp-uniform
+#endif
+#if HNB_GROUP_AGE
+        // Two copies of the sub-tile loop: copy 0 for floor tiles that keep common ages (`ages` true, `defer_rows` false),
+        // copy 1 for every other tile. With one copy, the code only other tiles run (reading each row's word, counting
+        // rows into deferred words) made the floor tiles 7 % slower on the H100 without running.
+#pragma unroll
+        for (int copy = 0; copy < 2; ++copy) {
+        const bool ages = copy == 0;
+        if (ages != tile_ages) continue;
+        const bool floors = ages || tile_floors, defer_rows = !ages && tile_defer_rows;
+#elif HNB_LIFE_FLOOR
+        {
+        const bool floors = tile_floors;
 #endif
 #pragma unroll 1
         for (u32 j = 0; j < chunks; ++j) {
             u32 pidx[HNB_TILE_K];
             bool valid[HNB_TILE_K];
             RawParticle raw[HNB_TILE_K];
+#if HNB_GROUP_AGE
+            u32 deferred_rows = 0u;  // bit k: row k of this lane took its age from a deferred word outside a floor tile
+#endif
 #if HNB_LIFE_FLOOR
             // lane k < HNB_TILE_K holds the floor of the sub-tile's row group k: one coalesced load
             const u32 g_first = ((base_particle + row0) >> 5u) + j * HNB_TILE_K;  // slab group of row group 0
@@ -733,9 +764,15 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
                 // A known common age A: every row of the group holds A in its age column, which is then not loaded. Every lane
                 // reads the group's word (one broadcast access) right before the row's record loads. Kept across the
                 // sub-tile in one register, as the floors are, the K words spill at 80 registers; read together ahead of the
-                // record loads, they made the pass 1.7 % slower on the H100.
-                const u64 word = ages ? P.group_age[g_first + k] : HNB_GROUP_AGE_NONE;
-                const u32 A = u32(word >> 32) == epoch - 1u ? u32(word) : HNB_LIFE_FLOOR_NONE;
+                // record loads, they made the pass 1.7 % slower on the H100. A deferred word is known whatever its epoch: no
+                // update but the one that consumes it advances its group's ages.
+                u64 word = HNB_GROUP_AGE_NONE;
+                if (ages) word = P.group_age[g_first + k];
+                else if (defer_rows && valid[k]) word = P.group_age[(base_particle + pidx[k]) >> 5u];
+                const bool deferred = hnb_group_age_deferred(word);
+                const u32 A = deferred || u32(word >> 32) == epoch - 1u ? u32(word) : HNB_LIFE_FLOOR_NONE;
+                if (defer_rows && deferred) deferred_rows |= 1u << k;
+                if (ages && deferred && lane == 0) parked->defer_delta -= 1u;
 #endif
                 if (valid[k]) {
 #if HNB_GROUP_AGE
@@ -825,30 +862,83 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
                     // overlap hnb_update, or PREV/NEXT must be declared HNB_ATTR_UPDATE_READ_ONLY (the graph lowering does),
                     // which gives them columns of their own that hnb_store_written never stores.
                     hnb_pack<false>(particle, raw[k]);
+#if HNB_GROUP_AGE
+                    // In a floor tile the age column is stored below, once the warp knows whether the group is deferred; the
+                    // other columns are stored here, as soon as they are packed.
+                    if (ages) hnb_store_written_but_age(raw[k], P.slab, base_particle + pidx[k]);
+                    else
+#endif
                     hnb_store_written(raw[k], P.slab, base_particle + pidx[k]);
                 }
+                const u32 ballot = __ballot_sync(0xffffffffu, alive);
 #if HNB_GROUP_AGE
                 if (ages) {
-                    // Every row of the group was valid and stored its record, dead or alive, so the new ages are what its age
-                    // column now holds: when all 32 are bit-equal (and not the sentinel's bits) they are the group's common
-                    // age as of this epoch. Otherwise nothing is stored: the word's epoch is then stale next frame.
+                    // Every row of the group is valid and stores its record, dead or alive, so the new ages are what its age
+                    // column holds after the store: when all 32 are bit-equal (and not the sentinel's bits) they are the
+                    // group's common age as of this epoch. With P.defer_ages, a group whose 32 rows all survive is left
+                    // deferred instead, and its age column is not stored: none of its rows reaches the dead stack, so the
+                    // next update of the instance walks all of them again. Any other group leaves a word that is not
+                    // deferred: known, or (with P.defer_ages, which may have found it deferred) the sentinel. Without
+                    // P.defer_ages a group of differing ages stores nothing, and its word's epoch is stale next frame.
                     const u32 a = __float_as_uint(hnb_raw_age(raw[k]));
                     const u32 a0 = __shfl_sync(0xffffffffu, a, 0);
                     const bool same = __ballot_sync(0xffffffffu, a == a0) == 0xffffffffu && a0 != HNB_LIFE_FLOOR_NONE;
-                    if (lane == 0 && same) P.group_age[g_first + k] = (u64(epoch) << 32) | a0;
+                    const bool defer = P.defer_ages && same && ballot == 0xffffffffu;
+                    if (!defer) hnb_store_age(raw[k], P.slab, base_particle + pidx[k]);
+                    if (lane == 0) {
+                        if (defer) P.group_age[g_first + k] = HNB_GROUP_AGE_DEFERRED | a0, parked->defer_delta += 1u;
+                        else if (same) P.group_age[g_first + k] = (u64(epoch) << 32) | a0;
+                        else if (P.defer_ages) P.group_age[g_first + k] = HNB_GROUP_AGE_NONE;
+                    }
                 }
 #endif
-                const u32 ballot = __ballot_sync(0xffffffffu, alive);
                 if (lane == 0) survivors[j * HNB_TILE_K + k] = ballot;
                 tile_alive += __popc(ballot);
 #if HNB_SLOT_ORDER
                 if (lane == j * HNB_TILE_K + k) my_new_bits = ballot;
 #endif
             }
+#if HNB_GROUP_AGE
+            if (defer_rows && __ballot_sync(0xffffffffu, deferred_rows != 0u) != 0u) {
+                // Rows that took a deferred age count themselves into its word, one atomic per group and warp. Each of a
+                // deferred group's 32 rows is walked exactly once in the launch, and read the word before it counts, so
+                // the add that makes 32 ends the deferral: the ages are all in the column now. (Outside the loop above,
+                // which the floor tiles' copy of this loop runs without any of it.)
+#pragma unroll
+                for (int k = 0; k < HNB_TILE_K; ++k) {
+                    const bool mine = (deferred_rows >> k) & 1u;
+                    const u32 g = (base_particle + pidx[k]) >> 5u;
+                    for (u32 pending = __ballot_sync(0xffffffffu, mine); pending;) {
+                        const u32 leader = u32(__ffs(pending) - 1);
+                        const u32 lg = __shfl_sync(0xffffffffu, g, int(leader));
+                        const u32 peers = __ballot_sync(0xffffffffu, mine && g == lg);
+                        if (lane == leader) {
+                            const u32 n = u32(__popc(peers));
+                            const u64 old = atomicAdd((unsigned long long*)&P.group_age[lg], (unsigned long long)n << 32);
+                            if (u32(old >> 32) - u32(HNB_GROUP_AGE_DEFERRED >> 32) + n == 32u) {
+                                P.group_age[lg] = HNB_GROUP_AGE_NONE;
+                                atomicAdd((unsigned long long*)hnb_deferred_groups(P.group_age, P.slab.capacity_rows), ~0ull);  // -1
+                            }
+                        }
+                        pending &= ~peers;
+                    }
+                }
+            }
+#endif
 #if HNB_PROFILE
             if (prof_first && j == 0u && lane == 0 && prof_ring) { unsigned long long _g; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(_g)); atomicMax(&prof_ring[2], ~_g); }
 #endif
         }
+#if HNB_LIFE_FLOOR
+        }
+#endif
+#if HNB_GROUP_AGE
+        // (a group this tile made deferred is counted late, but no other walker of this launch meets it)
+        if (lane == 0 && parked->defer_delta != 0u) {
+            atomicAdd((unsigned long long*)hnb_deferred_groups(P.group_age, P.slab.capacity_rows), (unsigned long long)(long long)int(parked->defer_delta));
+            parked->defer_delta = 0u;
+        }
+#endif
         // Publish this tile's survivor count right away: the first tile of an instance knows its prefix (0),
         // the others publish an AGGREGATE that successors can sum over while this tile's own prefix is
         // still unknown.

@@ -396,6 +396,36 @@ __global__ void k_bits_range(u32* bits, u32 first, u32 count, u32 set) {
     else if (set) atomicOr(&bits[w], mask);
     else atomicAnd(&bits[w], ~mask);
 }
+// Common ages of a slab's 32-row groups [g0, g0 + groups) (DESIGN.md §3), one thread per group. A deferred word's age goes
+// back into record word `age_word` of all 32 rows of its group (rows past `capacity` excepted), wherever the column plan
+// keeps it: the warp writes the rows of its deferred groups one group at a time, one row per lane. Then, with `clear` (for
+// writers of records), every word of the range and its lifetime floor become the sentinel; without (for readers), a
+// deferred word becomes the word known at `epoch`, and every other word stays.
+__global__ void k_flush_group_ages(PlaneSet planes, u32 age_word, u64* group_age, u32* life_floor, u32 g0, u32 groups, u32 capacity,
+                                   u32 clear, u32 epoch) {
+    const u32 t = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31u;
+    const bool mine = t < groups;
+    const u32 g = g0 + t;
+    const u64 word = mine ? group_age[g] : HNB_GROUP_AGE_NONE;
+    const bool deferred = hnb_group_age_deferred(word);
+    const u32 p = planes.word_to_plane[age_word], wl = hnb_word_lane(planes, age_word);
+    const u32 deferred_mask = __ballot_sync(0xffffffffu, deferred);
+    if (lane == 0u && deferred_mask != 0u)  // every deferred word of the range stops being deferred below
+        atomicAdd((unsigned long long*)hnb_deferred_groups(group_age, capacity), 0ull - u64(__popc(deferred_mask)));
+    for (u32 pending = deferred_mask; pending; pending &= pending - 1u) {
+        const int src = __ffs(pending) - 1;
+        const u32 row = __shfl_sync(0xffffffffu, g, src) * 32u + lane;
+        const u32 age = __shfl_sync(0xffffffffu, u32(word), src);
+        if (row < capacity) ((u32*)planes.ptr[p])[u64(row) * planes.words[p] + wl] = age;
+    }
+    if (!mine) return;
+    if (clear) {
+        group_age[g] = HNB_GROUP_AGE_NONE;
+        life_floor[g] = HNB_LIFE_FLOOR_NONE;
+    } else if (deferred) {
+        group_age[g] = (u64(epoch) << 32) | u32(word);
+    }
+}
 // ... and the bits of the rows an alive list names: list[i] (instance-local) + base, i < alive_count
 __global__ void k_bits_from_list(u32* bits, const u32* list, u32 base, u32 alive_count) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1535,6 +1565,14 @@ cudaError_t launch_bits_range(u32* bits, u32 first, u32 count, bool set, cudaStr
     if (count == 0) return cudaSuccess;
     const u32 words = u32(((u64(first) + count + 31u) >> 5u) - (first >> 5u));
     k_bits_range<<<blocks_for(words, 256), 256, 0, st>>>(bits, first, count, set ? 1u : 0u);
+    return cudaGetLastError();
+}
+cudaError_t launch_flush_group_ages(const PlaneSet& planes, u32 age_word, u64* group_age, u32* life_floor, u32 first, u32 count,
+                                    u32 capacity, bool clear, u32 epoch, cudaStream_t st) {
+    if (count == 0) return cudaSuccess;
+    const u32 g0 = first >> 5u, groups = u32(((u64(first) + count + 31u) >> 5u) - g0);
+    k_flush_group_ages<<<blocks_for(groups, 256), 256, 0, st>>>(planes, age_word, group_age, life_floor, g0, groups, capacity,
+                                                                           clear ? 1u : 0u, epoch);
     return cudaGetLastError();
 }
 cudaError_t launch_bits_from_list(u32* bits, const u32* list, u32 base, u32 alive_count, cudaStream_t st) {

@@ -210,6 +210,10 @@ cudaError_t launch_slab_reset(u32* ping, u32* pong, u32* dead, u32 first, u32 co
 // alive bitmap of a slab (HNB_EFFECT_SLOT_ORDER): set / clear the bits of a row range; set the bits an alive list names
 cudaError_t launch_bits_range(u32* bits, u32 first, u32 count, bool set, cudaStream_t st);
 cudaError_t launch_bits_from_list(u32* bits, const u32* list, u32 base, u32 alive_count, cudaStream_t st);
+// common ages of the 32-row groups rows [first, first + count) touch (DESIGN.md §3): deferred ages back into the age word of
+// their rows; then, with `clear`, every word and lifetime floor of the range the sentinel, else deferred words known at `epoch`
+cudaError_t launch_flush_group_ages(const PlaneSet& planes, u32 age_word, u64* group_age, u32* life_floor, u32 first, u32 count,
+                                    u32 capacity, bool clear, u32 epoch, cudaStream_t st);
 cudaError_t launch_aos_to_planes(const u32* aos, const PlaneSet& planes, u32 first, u32 count, u32 stride_words, cudaStream_t st);
 cudaError_t launch_planes_to_aos(u32* aos, const PlaneSet& planes, u32 first, u32 count, u32 stride_words, cudaStream_t st);
 cudaError_t launch_indirect_interleave(u32* rows3, const u32* ping, const u32* pong, const u32* dead, u32 first, u32 count, cudaStream_t st);

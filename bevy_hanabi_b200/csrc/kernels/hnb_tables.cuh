@@ -138,7 +138,10 @@ struct BatchParams {
     u32 late_tables;
     // this batch's GpuBatchInfo words the kernels need (the host knows them when it launches: no dependent load for them)
     u32 bi_spawner_base, bi_prefix_sum_offset, bi_prefix_sum_count;
-    u32 first_md_index, _pad1;       // effect_metadata_index of the batch's first instance (used when the batch has exactly one)          // 1: the host-written tables are stored by the kernel just ahead (k_frame_block): read them after the wait
+    u32 first_md_index;              // effect_metadata_index of the batch's first instance (used when the batch has exactly one)          // 1: the host-written tables are stored by the kernel just ahead (k_frame_block): read them after the wait
+    // 1: the update may leave common-age words deferred (HNB_GROUP_AGE_DEFERRED) and consumes the deferred words it meets.
+    // 0: no word is deferred and none is made so.
+    u32 defer_ages;
     // Lifetime floors of the slab (HNB_LIFE_FLOOR effects, DESIGN.md §3): one f32 per 32 slab rows, a lower bound of the
     // lifetimes of the group's particles, or HNB_LIFE_FLOOR_NONE. NULL: the slab uses no floors. Kept out of SlabView so
     // that the parameter offsets, and the code, of effects without floors stay as they were.
@@ -146,8 +149,16 @@ struct BatchParams {
     // Common ages of the slab (HNB_GROUP_AGE effects, DESIGN.md §3): one 64-bit word per 32 slab rows, (epoch << 32) | the
     // age bits every row of the group held after the update of frame `epoch`. Only a word of the previous frame's epoch is
     // known; all bits set: unknown. NULL: the slab keeps none (always NULL when life_floor is).
+    // Deferred (bits 63:62 = 01, with defer_ages): bits 31:0 are the age of every row of the group, whose age column is
+    // stale; bits 37:32 count the rows an update outside a floor tile has already taken the age from (see hnb_update).
+    // The array ends with one more word past the groups' (hnb_deferred_groups): how many words are deferred.
     u64* group_age;
 };
+#define HNB_GROUP_AGE_DEFERRED (1ull << 62)
+HNB_HD bool hnb_group_age_deferred(u64 word) { return (word >> 62) == 1ull; }
+// The count of deferred words of a slab of `capacity_rows` rows: never below the number of deferred words that a walker
+// other than the one that stored them may meet. Updates outside floor tiles read no word while it is 0.
+HNB_HD u64* hnb_deferred_groups(u64* group_age, u32 capacity_rows) { return group_age + (capacity_rows >> 5) + 1u; }
 // All bits set: a NaN, against which every comparison is false, so it proves nothing (0.0 would: ages can be negative).
 // Also the unknown common age (an age column whose bits are all ones never has a known common age).
 #define HNB_LIFE_FLOOR_NONE 0xffffffffu

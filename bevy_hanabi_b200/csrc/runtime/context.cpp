@@ -106,6 +106,10 @@ struct Slab {
     // set. Cleared with the floors, and at the epoch wrap. `ages_off`: a module without them was bound.
     DeviceArray<unsigned long long> group_age;
     bool ages_off = false;
+    // An update may have left words deferred (BatchParams::defer_ages): their groups' ages are in the words, not in record
+    // word `age_word` of the rows. Every other reader or writer of records flushes them first (flush_group_ages).
+    bool defers = false;
+    uint32_t age_word = 0;
     // HNB_EFFECT_ORDERED_EVENTS scratch, allocated on first use: per channel the per-row event counts and their block sums
     DeviceArray<uint32_t> event_counts[HNB_MAX_EVENT_BINDINGS];
     DeviceArray<uint32_t> event_block_sums[HNB_MAX_EVENT_BINDINGS];
@@ -117,6 +121,7 @@ struct KernelModule {
     int update_blocks_per_sm = 1;
     bool life_floor = false;  // generated with HNB_LIFE_FLOOR: keeps the slab's lifetime floors (and clears them on init)
     bool group_age = false;   // generated with HNB_GROUP_AGE: keeps the slab's common ages too
+    uint32_t age_word = 0;    // with group_age: the record word of the age (HNB_GROUP_AGE_WORD)
     std::string log;
 };
 
@@ -260,6 +265,7 @@ struct hnb_ctx {
     DeviceArray<uint32_t> d_sort_hist;
     uint32_t tile_chunks_override = 0;  // HNB_TILE_CHUNKS env: fixed sub-tile count per tile (tuning)
     bool param_upload = true; // HNB_PARAM_UPLOAD=0: always copy the frame block with the copy engine (never as a kernel parameter)
+    bool defer_ages = true;   // HNB_DEFER_AGES=0: no update leaves common ages deferred (DESIGN.md §3; A/B measurements)
     unsigned long long* mailbox = nullptr;  // device alias of the caller's pinned count mailbox (hnb_ctx_set_count_mailbox)
     uint32_t mailbox_rows = 0, mailbox_ring = 0;
     bool plan_dirty = false;  // bind_launch changed a tile-size or range word of the host frame block since the last upload
@@ -367,7 +373,7 @@ void flush_arena(hnb_ctx* c, bool with_ranges) {
     if (bytes >= c->lay.off_prefix_sum) c->plan_dirty = false;
 }
 
-void clear_life_floors(hnb_ctx* c, const Slab& s);
+void clear_life_floors(hnb_ctx* c, Slab& s);
 
 void next_epoch(hnb_ctx* c) {
     c->epoch = (c->epoch + 1u) & 0x3fffffffu;
@@ -378,7 +384,7 @@ void next_epoch(hnb_ctx* c) {
         for (const auto& ts : c->d_tile_state)
             if (ts) CUDA_CHECK(cudaMemsetAsync(ts.get(), 0, ts.size() * 8, c->stream));
         // the same for a common age stored a whole cycle ago (DESIGN.md §3)
-        for (const Slab& s : c->slabs)
+        for (Slab& s : c->slabs)
             if (s.live) clear_life_floors(c, s);
     }
     c->header()->epoch = c->epoch;
@@ -410,15 +416,31 @@ hnb::PlaneSet plane_set(const std::vector<Plane>& planes, char* block, uint32_t 
 }
 hnb::PlaneSet plane_set(const Slab& s) { return plane_set(s.planes, s.d_block.get(), s.capacity); }
 
-// Sets the lifetime floors of every 32-row group that rows [first, first + count) touch to HNB_LIFE_FLOOR_NONE, in stream
-// order: for writers of records other than the update pass (DESIGN.md §3).
-void clear_life_floors(hnb_ctx* c, const Slab& s, uint32_t first, uint32_t count) {
+// Writes the ages of deferred common-age words (DESIGN.md §3) of the 32-row groups rows [first, first + count) touch back to
+// their rows, in stream order, when the slab may hold any. `clear`: then sets every word and lifetime floor of those groups to
+// the sentinel (writers of records). Otherwise a deferred word becomes the word known at the context's epoch, which the next
+// frame's update reads as known (readers of records).
+void flush_group_ages(hnb_ctx* c, const Slab& s, uint32_t first, uint32_t count, bool clear) {
+    if (count == 0 || !s.defers) return;
+    CUDA_CHECK(hnb::launch_flush_group_ages(plane_set(s), s.age_word, s.group_age.get(), s.life_floor.get(), first, count, s.capacity,
+                                            clear, c->epoch, c->stream));
+    c->launches++;
+}
+
+// Sets the lifetime floors and common ages of every 32-row group that rows [first, first + count) touch to the sentinel, in
+// stream order, deferred ages written back first: for writers of records other than the update pass (DESIGN.md §3).
+void clear_life_floors(hnb_ctx* c, Slab& s, uint32_t first, uint32_t count) {
     if (count == 0) return;
+    if (s.defers) {
+        flush_group_ages(c, s, first, count, true);
+        if (first == 0 && count == s.capacity) s.defers = false;  // no word is deferred any more
+        return;
+    }
     const size_t g0 = first / 32u, g1 = (size_t(first) + count + 31u) / 32u;
     CUDA_CHECK(cudaMemsetAsync(s.life_floor.get() + g0, 0xff, (g1 - g0) * sizeof(uint32_t), c->stream));
     CUDA_CHECK(cudaMemsetAsync(s.group_age.get() + g0, 0xff, (g1 - g0) * sizeof(unsigned long long), c->stream));
 }
-void clear_life_floors(hnb_ctx* c, const Slab& s) { clear_life_floors(c, s, 0, s.capacity); }
+void clear_life_floors(hnb_ctx* c, Slab& s) { clear_life_floors(c, s, 0, s.capacity); }
 
 // AoS records <-> columns go through a device staging buffer in chunks of this size.
 constexpr size_t kChunkBytes = size_t(64) << 20;
@@ -438,6 +460,7 @@ void fix_plan(hnb_ctx* c, Slab& s, const std::vector<Plane>& plan) {
             s.plan_fixed = true;
             return;
         }
+        clear_life_floors(c, s);  // (before the records move: a deferred age goes back to the columns it is moved from)
         const hnb::PlaneSet from = plane_set(s), to = plane_set(plan, next.get(), s.capacity);
         uint32_t* stage = reinterpret_cast<uint32_t*>(staging.get());
         for (uint32_t done = 0; done < s.capacity; done += rows_per_chunk) {
@@ -448,7 +471,6 @@ void fix_plan(hnb_ctx* c, Slab& s, const std::vector<Plane>& plan) {
         }
         CUDA_CHECK(cudaStreamSynchronize(c->stream));  // the old block and the staging buffer are released below
         s.d_block.swap(next);
-        clear_life_floors(c, s);
     }
     s.planes = plan;
     s.plan_fixed = true;
@@ -503,6 +525,8 @@ KernelModule* get_module(hnb_ctx* c, const std::string& source, const std::strin
     km->update_blocks_per_sm = 1;  // depends on the effect's dynamic shared memory (set_update_smem)
     km->life_floor = source.find("\n#define HNB_LIFE_FLOOR 1\n") != std::string::npos;
     km->group_age = source.find("\n#define HNB_GROUP_AGE 1\n") != std::string::npos;
+    if (const size_t at = source.find("\n#define HNB_GROUP_AGE_WORD "); at != std::string::npos)
+        km->age_word = uint32_t(strtoul(source.c_str() + at + 27, nullptr, 10));
     KernelModule* out = km.get();
     c->modules.emplace(hash, std::move(km));
     return out;
@@ -719,6 +743,11 @@ void bind_launch(hnb_ctx* c, LaunchPlan& lp, const hnb_batch_launch& bl, bool se
     // The same for common ages: a module without them writes ages without keeping the words true.
     if (!lp.km->group_age) slab.ages_off = true;
     P.group_age = slab.floors_off || slab.ages_off ? nullptr : slab.group_age.get();
+    // Deferred common ages (DESIGN.md §3): a module that keeps none, or keeps the age in another record word, gets the slab
+    // with every age in its column. An update that keeps them may defer (launch_update decides, once every launch of the
+    // frame is bound). Relaxed-order and slot-order modules keep no floors, so they take the first branch.
+    if (slab.defers && (!P.group_age || lp.km->age_word != slab.age_word)) clear_life_floors(c, slab);
+    P.defer_ages = P.group_age && c->defer_ages ? 1u : 0u;
     if (consume) P.consume_events = c->event_buffers[bl.consume_events].get();
     for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
         if (bl.emit_events[i] == 0xFFFFFFFFu) continue;
@@ -778,6 +807,13 @@ void launch_kernel(hnb_ctx* c, CUfunction f, uint32_t blocks, hnb::BatchParams& 
 
 void launch_update(hnb_ctx* c, LaunchPlan& lp, cudaStream_t st = nullptr) {
     if (!st) st = c->stream;
+    // A launch bound after this one may have switched the slab's common ages off (bind_launch): then nothing is deferred.
+    Slab& slab = *lp.slab;
+    if (slab.floors_off || slab.ages_off) lp.params.defer_ages = 0u;
+    if (lp.params.defer_ages) {
+        slab.defers = true;
+        slab.age_word = lp.km->age_word;
+    }
     std::pair<Event, Event> ev;
     if (c->timing) {
         if (!c->ev_free.empty()) { ev = std::move(c->ev_free.back()); c->ev_free.pop_back(); }
@@ -851,6 +887,7 @@ void launch_ribbon_sort(hnb_ctx* c, const LaunchPlan& lp) {
     a.scratch_grid = uint32_t(c->sm_count);
     if (any_large) CUDA_CHECK(cudaMemsetAsync(c->d_sort_hist.get(), 0, size_t(2 * 8 * 256) * 4, c->stream));
     clear_ident_claims(c, *lp.slab);  // the sort permutes the column the update just wrote
+    flush_group_ages(c, *lp.slab, 0, lp.slab->capacity, false);  // its second key is the age
     uint32_t launched = 0;
     CUDA_CHECK(hnb::launch_ribbon_sort(a, any_large, uint32_t(c->sm_count), c->stream, &launched));
     c->launches += launched;
@@ -970,6 +1007,7 @@ int32_t hnb_ctx_create(int32_t cuda_device, uintptr_t external_stream, hnb_ctx**
         if (const char* env = getenv("HNB_TILE_CHUNKS")) c->tile_chunks_override = (uint32_t)atoi(env);
         if (const char* env = getenv("HNB_EPOCH_START")) c->epoch = uint32_t(strtoul(env, nullptr, 0)) & 0x3fffffffu;  // tests: start near the wrap
         if (const char* env = getenv("HNB_PARAM_UPLOAD")) c->param_upload = atoi(env) != 0;
+        if (const char* env = getenv("HNB_DEFER_AGES")) c->defer_ages = atoi(env) != 0;
         ensure_arena(c.get(), 0, 0);
         CUDA_CHECK(grow(c->d_debug, kDebugWords, 0, c->stream));
         *out = c.release();
@@ -1017,8 +1055,9 @@ int32_t hnb_slab_create_ex(hnb_ctx* c, uint32_t capacity_rows, uint32_t stride, 
         CUDA_CHECK(s.ident_claim.alloc(2));
         clear_ident_claims(c, s);
         CUDA_CHECK(s.life_floor.alloc(size_t(capacity_rows) / 32 + 1));
-        CUDA_CHECK(s.group_age.alloc(size_t(capacity_rows) / 32 + 1));
+        CUDA_CHECK(s.group_age.alloc(size_t(capacity_rows) / 32 + 2));  // the groups' words, then hnb_deferred_groups
         clear_life_floors(c, s);
+        CUDA_CHECK(cudaMemsetAsync(hnb::hnb_deferred_groups(s.group_age.get(), capacity_rows), 0, sizeof(unsigned long long), c->stream));
         CUDA_CHECK(hnb::launch_slab_reset(s.ping.get(), s.pong.get(), s.dead.get(), 0, capacity_rows, c->stream));
         c->launches++;
         s.live = true;
@@ -1068,6 +1107,7 @@ void transfer_aos(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, void* 
     if (count == 0) return;
     s.written |= upload;
     if (upload) clear_life_floors(c, s, first, count);
+    else flush_group_ages(c, s, first, count, false);
     const uint32_t rows_per_chunk = (uint32_t)std::max<size_t>(1, kChunkBytes / s.stride);
     DeviceArray<char> staging;
     CUDA_CHECK(staging.alloc(size_t(std::min(rows_per_chunk, count)) * s.stride));
@@ -1137,6 +1177,7 @@ int32_t hnb_slab_export_aos_device(hnb_ctx* c, hnb_slab h, uint32_t first, uint3
         check_rows(s, first, count);
         if (count && !d_dst) fail(HNB_ERR_INVALID_ARG, "d_dst is NULL");
         if ((uintptr_t)d_dst & 3u) fail(HNB_ERR_INVALID_ARG, "d_dst must be 4-byte aligned (16-byte aligned for full speed)");
+        flush_group_ages(c, s, first, count, false);
         CUDA_CHECK(hnb::launch_planes_to_aos((uint32_t*)d_dst, plane_set(s), first, count, s.stride / 4, c->stream));
         c->launches += count ? 1 : 0;
     });
@@ -1178,7 +1219,8 @@ int32_t hnb_slab_device_view(hnb_ctx* c, hnb_slab h, hnb_slab_view* out) {
         Slab& s = get_slab(c, h);
         if (!out) fail(HNB_ERR_INVALID_ARG, "out is NULL");
         fix_default_plan(c, s);  // handed-out columns never move: an unbound slab keeps the default cut from now on
-        s.floors_off = true;     // records written through the view would not clear the floors
+        if (s.defers) clear_life_floors(c, s);  // every age goes back to its column ...
+        s.floors_off = true;     // ... and records written through the view would not clear the floors
         memset(out, 0, sizeof(*out));
         out->capacity_rows = s.capacity;
         out->particle_stride = s.stride;
@@ -1382,6 +1424,7 @@ int32_t instance_snapshot(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadat
         }
         if (rows == 0) return;
         CUDA_CHECK(cudaSetDevice(c->device));
+        flush_group_ages(c, s, first, rows, false);
         CUDA_CHECK(hnb::launch_snapshot_gather(snapshot_args(c, s, metadata_row, first, rows), (uint32_t*)d_dst, c->stream,
                                                emit ? s.dead.get() : nullptr));
         c->launches++;
@@ -1491,6 +1534,7 @@ int32_t hnb_slab_checksum_ex(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t co
     return guarded([&] {
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
+        flush_group_ages(c, s, first, count, false);
         checksum(c, plane_set(s), first, count, s.stride / 4, index_base, out);
     });
 }
@@ -1764,6 +1808,10 @@ int32_t hnb_metadata_insert(hnb_ctx* c, uint32_t row, const hnb_effect_metadata*
     return guarded([&] {
         if (!md) fail(HNB_ERR_INVALID_ARG, "md is NULL");
         c->md_generation++;
+        // A new metadata row may end an instance without any writer of its rows: the slice's next owner would not walk every
+        // row of a deferred group. So every age goes back to its column first (DESIGN.md §3).
+        for (Slab& s : c->slabs)
+            if (s.live && s.defers) clear_life_floors(c, s);
         const uint32_t rows = uint32_t(c->d_metadata.size());
         if (row + 1 > rows) CUDA_CHECK(grow(c->d_metadata, std::max<uint32_t>(row + 1, std::max<uint32_t>(rows * 2, 16)), rows, c->stream));
         CUDA_CHECK(cudaMemcpyAsync(c->d_metadata.get() + row, md, sizeof(*md), cudaMemcpyHostToDevice, c->stream));

@@ -421,6 +421,21 @@ void gen_life_floor_code(std::ostringstream& o, const hnb_effect_desc& d, const 
     o << "HNB_DI void hnb_load_age(RawParticle& r, const SlabView& s, u32 row) { " << age << " = HNB_LOAD_PLANE(f32, s.planes["
       << age_plane << "], row); }\n";
     o << "HNB_DI void hnb_set_raw_age(RawParticle& r, f32 age) { " << age << " = age; }\n";
+    // The record word of the age (the runtime writes deferred ages back to it); the update's store in a floor tile,
+    // hnb_store_written without the age column, and the store of the age column, which a group left deferred skips.
+    o << "#define HNB_GROUP_AGE_WORD " << age_word << "\n";
+    o << "HNB_DI void hnb_store_age(const RawParticle& r, const SlabView& s, u32 row) { HNB_STORE_PLANE(f32, s.planes[" << age_plane
+      << "], row, " << age << "); }\n";
+    const bool all = !any_read_only(d.attrs, d.n_attrs);
+    const std::vector<bool> written = written_words(d.particle_stride, d.attrs, d.n_attrs);
+    o << "HNB_DI void hnb_store_written_but_age(const RawParticle& r, const SlabView& s, u32 row) {\n";
+    for (size_t p = 0; p < planes.size(); ++p) {
+        bool store = all;
+        for (uint32_t w = 0; w < planes[p].width / 4; ++w) store = store || written[planes[p].word[w]];
+        if (!store || p == age_plane) continue;
+        o << "    HNB_STORE_PLANE(" << plane_type(planes[p]) << ", s.planes[" << p << "], row, " << mapped_value(planes[p], p) << ");\n";
+    }
+    o << "}\n";
 }
 
 }  // namespace
