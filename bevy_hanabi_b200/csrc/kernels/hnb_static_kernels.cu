@@ -1125,19 +1125,19 @@ __device__ __forceinline__ u32 depth_sort_key(const float* plane, u32 x, u32 y, 
     return (bits & 0x7FFFFFFFu) > 0x7F800000u ? 0xFFFFFFFFu : ~bounds_key(bits);
 }
 
-// Instance j as k_do_plan recorded it: 8 words.
+// Instance j as the tile plan (do_tile_plan) recorded it in `info`: 8 words.
 struct DepthInstance { u32 first, n, tile_base, tiles, w, rows, mask; };
-__device__ __forceinline__ DepthInstance do_instance(const DepthOrderArgs& a, u32 j) {
-    const u32* in = a.info + u64(j) * 8u;
+__device__ __forceinline__ DepthInstance do_instance(const u32* info, u32 j) {
+    const u32* in = info + u64(j) * 8u;
     return DepthInstance{in[0], in[1], in[2], in[3], in[4], in[5], in[6]};
 }
 // The instance that owns tile g of the call: the largest j with tile_base <= g (tile_base is non-decreasing in j, and
 // instances without tiles share the base of the next one). The caller checks g - tile_base < tiles.
-__device__ __forceinline__ u32 do_find(const DepthOrderArgs& a, u32 count, u32 g) {
+__device__ __forceinline__ u32 do_find(const u32* info, u32 count, u32 g) {
     u32 lo = 0u, hi = count - 1u;
     while (lo < hi) {
         const u32 mid = hi - (hi - lo) / 2u;
-        if (a.info[u64(mid) * 8u + 2u] <= g) lo = mid;
+        if (info[u64(mid) * 8u + 2u] <= g) lo = mid;
         else hi = mid - 1u;
     }
     return lo;
@@ -1196,26 +1196,24 @@ __device__ __forceinline__ u32 do_block_exclusive(u32 v, u32* s_warp) {
     return before + x - v;
 }
 
-// Tiles per instance and their prefix over the batch, kept in `info` for the later launches (CTA 0); the digit totals
-// of the call's instances back to zero (every CTA). An instance whose tiles would pass `max_tiles` (only possible when
-// the tables describe overlapping slices) gets none: it is not sorted, and nothing outside the buffers is touched.
-__global__ void __launch_bounds__(DO_THREADS) k_do_plan(DepthOrderArgs a) {
-    __shared__ u32 s_warp[DO_WARPS];
-    const u32 count = bounds_count(a.src), tid = threadIdx.x;
-    for (u64 k = u64(blockIdx.x) * DO_THREADS + tid; k < u64(count) * 1024u; k += u64(gridDim.x) * DO_THREADS) a.totals[k] = 0u;
-    if (blockIdx.x != 0u) return;
+// Tiles of DO_TILE rows per instance and their prefix over the batch, kept in `info` (8 words per instance) for the
+// later launches of a call, and the call's tile count in `total_tiles`; run by one CTA of DO_THREADS threads. An instance
+// whose tiles would pass `max_tiles` (only possible when the tables describe overlapping slices) gets none: it is not
+// processed, and nothing outside the buffers is touched.
+__device__ __forceinline__ void do_tile_plan(const BoundsArgs& src, u32* info, u32* total_tiles, u32 max_tiles, u32* s_warp) {
+    const u32 count = bounds_count(src), tid = threadIdx.x;
     u64 carry = 0u;
     for (u32 chunk = 0; chunk < count; chunk += DO_THREADS) {
         const u32 j = chunk + tid;
         BoundsInstance b = {0u, 0u, 0u, 0u};
-        if (j < count) b = bounds_instance(a.src, j);
+        if (j < count) b = bounds_instance(src, j);
         const u32 tiles = u32((u64(b.n) + DO_TILE - 1u) / DO_TILE);
         const u32 excl = do_block_exclusive(tiles, s_warp);
         const u64 base = carry + excl;
         if (j < count) {
-            u32* in = a.info + u64(j) * 8u;
-            const bool fits = base + tiles <= a.max_tiles;
-            in[0] = b.first; in[1] = b.n; in[2] = u32(base < a.max_tiles ? base : a.max_tiles); in[3] = fits ? tiles : 0u;
+            u32* in = info + u64(j) * 8u;
+            const bool fits = base + tiles <= max_tiles;
+            in[0] = b.first; in[1] = b.n; in[2] = u32(base < max_tiles ? base : max_tiles); in[3] = fits ? tiles : 0u;
             in[4] = b.w; in[5] = b.rows; in[6] = 0u; in[7] = 0u;
         }
         __syncthreads();
@@ -1223,7 +1221,16 @@ __global__ void __launch_bounds__(DO_THREADS) k_do_plan(DepthOrderArgs a) {
         __syncthreads();
         carry += s_warp[0];
     }
-    if (tid == 0u) *a.total_tiles = u32(carry < a.max_tiles ? carry : a.max_tiles);
+    if (tid == 0u) *total_tiles = u32(carry < max_tiles ? carry : max_tiles);
+}
+
+// The tile plan (CTA 0); the digit totals of the call's instances back to zero (every CTA).
+__global__ void __launch_bounds__(DO_THREADS) k_do_plan(DepthOrderArgs a) {
+    __shared__ u32 s_warp[DO_WARPS];
+    const u32 count = bounds_count(a.src), tid = threadIdx.x;
+    for (u64 k = u64(blockIdx.x) * DO_THREADS + tid; k < u64(count) * 1024u; k += u64(gridDim.x) * DO_THREADS) a.totals[k] = 0u;
+    if (blockIdx.x != 0u) return;
+    do_tile_plan(a.src, a.info, a.total_tiles, a.max_tiles, s_warp);
 }
 
 // Entry, position and key of every live row of the tile; rows below the identity claim of column W load no list entry.
@@ -1271,8 +1278,8 @@ __global__ void __launch_bounds__(DO_THREADS) k_do_keys(DepthOrderArgs a) {
     const u32 count = bounds_count(a.src), total = *a.total_tiles, tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
     const u64 claim0 = hnb_claim_load(&a.src.claim[0]), claim1 = hnb_claim_load(&a.src.claim[1]);
     for (u32 g = blockIdx.x; g < total; g += gridDim.x) {
-        const u32 j = do_find(a, count, g);
-        const DepthInstance in = do_instance(a, j);
+        const u32 j = do_find(a.info, count, g);
+        const DepthInstance in = do_instance(a.info, j);
         const u32 t = g - in.tile_base;
         if (t >= in.tiles) continue;  // CTA-uniform
         const u32 claimed = min(hnb_claim_len(in.w == 0u ? claim0 : claim1, in.first), in.n);
@@ -1337,7 +1344,7 @@ __global__ void __launch_bounds__(DO_THREADS) k_do_scan(DepthOrderArgs a, u32 pa
     const u32 count = bounds_count(a.src);
     if (row >= u64(count) * 256u) return;  // warp-uniform
     const u32 j = u32(row >> 8), d = u32(row & 255u);
-    const DepthInstance in = do_instance(a, j);
+    const DepthInstance in = do_instance(a.info, j);
     if (in.tiles < 2u) return;
     const u32* tot = a.totals + u64(j) * 1024u;
     u32 run;
@@ -1389,7 +1396,7 @@ __global__ void __launch_bounds__(DO_THREADS) k_do_scatter(DepthOrderArgs a, u32
     __shared__ u32 s_cnt[DO_WARPS * 256], s_tot[256];
     const u32 count = bounds_count(a.src), total = *a.total_tiles, tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
     for (u32 g = blockIdx.x; g < total; g += gridDim.x) {
-        const DepthInstance in = do_instance(a, do_find(a, count, g));
+        const DepthInstance in = do_instance(a.info, do_find(a.info, count, g));
         const u32 t = g - in.tile_base;
         if (in.tiles < 2u || t >= in.tiles) continue;  // CTA-uniform
         const u32 i0 = t * DO_TILE + warp * DO_WARP_ROWS + lane;
@@ -1434,7 +1441,7 @@ __global__ void __launch_bounds__(DO_THREADS) k_do_hist(DepthOrderArgs a, u32 pa
     __shared__ u32 s_cnt[256];
     const u32 count = bounds_count(a.src), total = *a.total_tiles, tid = threadIdx.x;
     for (u32 g = blockIdx.x; g < total; g += gridDim.x) {
-        const DepthInstance in = do_instance(a, do_find(a, count, g));
+        const DepthInstance in = do_instance(a.info, do_find(a.info, count, g));
         const u32 t = g - in.tile_base;
         if (in.tiles < 2u || t >= in.tiles || !((in.mask >> pass) & 1u)) continue;  // CTA-uniform
         const u32* keys = a.keys[do_src(in.mask, pass)] + in.first;
@@ -1446,6 +1453,186 @@ __global__ void __launch_bounds__(DO_THREADS) k_do_hist(DepthOrderArgs a, u32 pa
             atomicAdd(&s_cnt[(keys[i] >> (8u * pass)) & 255u], 1u);
         __syncthreads();
         a.hist[u64(in.tile_base) * 256u + u64(tid) * in.tiles + t] = s_cnt[tid];
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Visible particles of every instance of a batch (hnb_batch_cull): the source entries of each instance whose `position`
+// lies inside the instance's six frustum planes, compacted in source order, and the instance's draw arguments with that
+// count. A pure read of the instance, like bounds and depth order.
+//
+// The tiles are depth order's (DO_TILE rows of one instance, planned by do_tile_plan). Row i of a tile is tested by
+// lane i % 32 of warp (i % DO_TILE) / DO_WARP_ROWS, as item (i % DO_WARP_ROWS) / 32, so one ballot per item is one word
+// of the tile's visibility mask. Four launches, whatever the batch holds:
+//   k_cull_plan   the tile plan (one CTA)
+//   k_cull_test   per tile: source entries, positions, the six plane tests; the tile's mask and visible count
+//   k_cull_scan   per instance (one CTA): tile counts -> exclusive prefixes; the instance's draw-args row with its count
+//   k_cull_write  per tile: each visible entry to first + prefix + its rank in the mask, so a warp's stores are consecutive
+// ---------------------------------------------------------------------------------------------
+#define CULL_PLANES 6
+#define CULL_WORDS (DO_TILE / 32)  // mask words per tile: DO_ITEMS per warp
+static_assert(CULL_WORDS == HNB_BATCH_CULL_MASK_WORDS && CULL_WORDS == DO_WARPS * DO_ITEMS, "one mask word per item of a warp");
+#define CULL_ITEMS 8               // items of a thread with loads in flight together (DO_ITEMS / CULL_ITEMS rounds per tile)
+#define CULL_SCAN_ITEMS 16         // tile counts per thread per round of k_cull_scan
+
+// ((a*x + b*y) + c*z) + d >= 0 for all six planes, each step rounded on its own: a NaN fails, -0 passes.
+__device__ __forceinline__ bool cull_inside(const float* f, u32 x, u32 y, u32 z) {
+    bool inside = true;
+#pragma unroll
+    for (int p = 0; p < CULL_PLANES; ++p) {
+        const float* q = f + 4 * p;
+        const float v = do_add(do_add(do_add(do_mul(q[0], __uint_as_float(x)), do_mul(q[1], __uint_as_float(y))),
+                                      do_mul(q[2], __uint_as_float(z))), q[3]);
+        inside &= v >= 0.0f;
+    }
+    return inside;
+}
+
+// Where the source entries of an instance come from: d_src at the instance's rows, or its alive-list column W, whose rows
+// below the identity claim are i (no load). Every entry is clamped to the slice.
+struct CullSource { const u32* list; u32 claimed, last_row; };
+__device__ __forceinline__ CullSource cull_source(const CullArgs& a, const DepthInstance& in, u64 claim0, u64 claim1) {
+    if (a.src_list) return CullSource{a.src_list + in.first, 0u, in.rows - 1u};
+    return CullSource{(in.w == 0u ? a.src.ping : a.src.pong) + in.first, min(hnb_claim_len(in.w == 0u ? claim0 : claim1, in.first), in.n),
+                      in.rows - 1u};
+}
+__device__ __forceinline__ u32 cull_entry(const CullSource& s, u32 i) { return i < s.claimed ? i : min(s.list[i], s.last_row); }
+
+__global__ void __launch_bounds__(DO_THREADS) k_cull_plan(CullArgs a) {
+    __shared__ u32 s_warp[DO_WARPS];
+    do_tile_plan(a.src, a.info, a.total_tiles, a.max_tiles, s_warp);
+}
+
+// Persistent grid over the call's tiles. The instance's frustum is staged in shared memory when a CTA's instance changes
+// (it may sit in pinned host memory). FAST: position in one 16-byte load per row, as k_bounds_reduce.
+template <bool FAST>
+__global__ void __launch_bounds__(DO_THREADS) k_cull_test(CullArgs a) {
+    __shared__ float s_frustum[4 * CULL_PLANES];
+    __shared__ u32 s_count;
+    const u32 count = bounds_count(a.src), total = *a.total_tiles, tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    const u64 claim0 = hnb_claim_load(&a.src.claim[0]), claim1 = hnb_claim_load(&a.src.claim[1]);
+    const BoundsArgs& s = a.src;
+    u32 staged = 0xFFFFFFFFu;
+    for (u32 g = blockIdx.x; g < total; g += gridDim.x) {
+        const u32 j = do_find(a.info, count, g);
+        const DepthInstance in = do_instance(a.info, j);
+        const u32 t = g - in.tile_base;
+        if (t >= in.tiles) continue;  // CTA-uniform
+        __syncthreads();              // the previous tile's readers of s_frustum and s_count are done
+        if (j != staged && tid < 4u * CULL_PLANES) s_frustum[tid] = a.frusta[u64(j) * (4u * CULL_PLANES) + tid];
+        if (tid == 0u) s_count = 0u;
+        staged = j;
+        __syncthreads();
+        const CullSource src = cull_source(a, in, claim0, claim1);
+        const u32 i0 = t * DO_TILE + warp * DO_WARP_ROWS + lane;
+        u32 word = 0u, seen = 0u;
+#pragma unroll
+        for (u32 h = 0; h < DO_ITEMS; h += CULL_ITEMS) {
+            u32 e[CULL_ITEMS];
+            bool vis[CULL_ITEMS];
+#pragma unroll
+            for (u32 k = 0; k < CULL_ITEMS; ++k) {
+                const u32 i = i0 + (h + k) * 32u;
+                e[k] = i < in.n ? cull_entry(src, i) : 0u;
+            }
+            if (FAST) {
+                const RepackPiece<4>* col = (const RepackPiece<4>*)s.col[0];
+                const u32 quads = s.col_words[0] >> 2u, quad = s.col_lane[0] >> 2u;
+                RepackPiece<4> v[CULL_ITEMS];
+#pragma unroll
+                for (u32 k = 0; k < CULL_ITEMS; ++k)
+                    if (i0 + (h + k) * 32u < in.n) v[k] = col[(u64(in.first) + e[k]) * quads + quad];
+#pragma unroll
+                for (u32 k = 0; k < CULL_ITEMS; ++k)
+                    vis[k] = i0 + (h + k) * 32u < in.n && cull_inside(s_frustum, v[k].w[0], v[k].w[1], v[k].w[2]);
+            } else {
+                u32 v[CULL_ITEMS][3];
+#pragma unroll
+                for (u32 k = 0; k < CULL_ITEMS; ++k) {
+                    if (i0 + (h + k) * 32u >= in.n) continue;
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) v[k][c] = s.col[c][(u64(in.first) + e[k]) * s.col_words[c] + s.col_lane[c]];
+                }
+#pragma unroll
+                for (u32 k = 0; k < CULL_ITEMS; ++k)
+                    vis[k] = i0 + (h + k) * 32u < in.n && cull_inside(s_frustum, v[k][0], v[k][1], v[k][2]);
+            }
+#pragma unroll
+            for (u32 k = 0; k < CULL_ITEMS; ++k) {
+                const u32 b = __ballot_sync(0xffffffffu, vis[k]);
+                if (lane == h + k) word = b;
+                seen += __popc(b);
+            }
+        }
+        if (lane < DO_ITEMS) a.mask[u64(g) * CULL_WORDS + warp * DO_ITEMS + lane] = word;
+        if (lane == 0u && seen) atomicAdd(&s_count, seen);
+        __syncthreads();
+        if (tid == 0u) a.prefix[g] = s_count;
+    }
+}
+
+// CTA j, one per instance the call covers: the visible counts of instance j's tiles become exclusive prefixes within the
+// instance, and d_args[j] receives the draw-args row its spawner row names (clamped to the table) with instance_count =
+// the instance's visible total (0 for a j past the batch's device-side count).
+__global__ void __launch_bounds__(DO_THREADS) k_cull_scan(CullArgs a) {
+    __shared__ u32 s_warp[DO_WARPS];
+    __shared__ u32 s_round;
+    const u32 j = blockIdx.x, tid = threadIdx.x;
+    u32 m = 0u;
+    if (j < bounds_count(a.src)) {  // CTA-uniform
+        const DepthInstance in = do_instance(a.info, j);
+        u32* c = a.prefix + in.tile_base;
+        for (u32 t0 = 0; t0 < in.tiles; t0 += DO_THREADS * CULL_SCAN_ITEMS) {
+            const u32 tb = t0 + tid * CULL_SCAN_ITEMS;
+            u32 v[CULL_SCAN_ITEMS], sum = 0u;
+#pragma unroll
+            for (u32 q = 0; q < CULL_SCAN_ITEMS; ++q) {
+                v[q] = tb + q < in.tiles ? c[tb + q] : 0u;
+                sum += v[q];
+            }
+            u32 run = m + do_block_exclusive(sum, s_warp);
+#pragma unroll
+            for (u32 q = 0; q < CULL_SCAN_ITEMS; ++q) {
+                if (tb + q < in.tiles) c[tb + q] = run;
+                run += v[q];
+            }
+            __syncthreads();  // s_round of the previous round is read
+            if (tid == DO_THREADS - 1u) s_round = run;
+            __syncthreads();
+            m = s_round;
+        }
+    }
+    if (tid < HNB_DRAW_INDEXED_INDIRECT_STRIDE) {
+        const u64 row = u64(a.src.batch_info->spawner_base) + j;
+        const Spawner* sp = &a.src.spawners[row < a.src.num_spawners ? row : a.src.num_spawners - 1u];
+        const u32 dri = min(sp->draw_indirect_index, a.num_draw_args - 1u);
+        a.args[u64(j) * HNB_DRAW_INDEXED_INDIRECT_STRIDE + tid] = tid == 1u ? m : a.draw_args[u64(dri) * HNB_DRAW_INDEXED_INDIRECT_STRIDE + tid];
+    }
+}
+
+// Persistent grid over the call's tiles: a visible row's place is its tile's prefix plus the visible rows before it in
+// the tile's mask. The entries are loaded again (only where a mask bit is set); places are clamped to the instance's n.
+__global__ void __launch_bounds__(DO_THREADS) k_cull_write(CullArgs a) {
+    __shared__ u32 s_warp[DO_WARPS];
+    const u32 count = bounds_count(a.src), total = *a.total_tiles, tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    const u64 claim0 = hnb_claim_load(&a.src.claim[0]), claim1 = hnb_claim_load(&a.src.claim[1]);
+    const u32 lt = (1u << lane) - 1u;
+    for (u32 g = blockIdx.x; g < total; g += gridDim.x) {
+        const DepthInstance in = do_instance(a.info, do_find(a.info, count, g));
+        const u32 t = g - in.tile_base;
+        if (t >= in.tiles) continue;  // CTA-uniform
+        // lane k < DO_ITEMS holds mask word k of its warp and the visible rows of the tile before that word
+        const u32 word = lane < DO_ITEMS ? a.mask[u64(g) * CULL_WORDS + warp * DO_ITEMS + lane] : 0u;
+        const u32 before = a.prefix[g] + do_block_exclusive(__popc(word), s_warp);
+        const CullSource src = cull_source(a, in, claim0, claim1);
+        const u32 i0 = t * DO_TILE + warp * DO_WARP_ROWS + lane;
+#pragma unroll
+        for (u32 k = 0; k < DO_ITEMS; ++k) {
+            const u32 wk = __shfl_sync(0xffffffffu, word, k), bk = __shfl_sync(0xffffffffu, before, k);
+            if (!((wk >> lane) & 1u)) continue;
+            const u32 r = min(bk + __popc(wk & lt), in.n - 1u);
+            a.visible[u64(in.first) + r] = cull_entry(src, i0 + k * 32u);
+        }
     }
 }
 
@@ -1673,6 +1860,34 @@ cudaError_t launch_batch_depth_order(const DepthOrderArgs& a, bool fast, u32 sm_
         k_do_scan<<<rows, DO_THREADS, 0, st>>>(a, pass);
         k_do_scatter<<<tiles, DO_THREADS, 0, st>>>(a, pass);
     }
+    return cudaGetLastError();
+}
+// CTAs of `kernel` (DO_THREADS threads) that one SM holds, asked once per kernel
+template <typename K> static cudaError_t do_ctas_per_sm(K kernel, int* cached, u32* out) {
+    if (*cached == 0) {
+        int n = 0;
+        const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, DO_THREADS, 0);
+        if (e != cudaSuccess) return e;
+        *cached = std::max(n, 1);
+    }
+    *out = u32(*cached);
+    return cudaSuccess;
+}
+cudaError_t launch_batch_cull(const CullArgs& a, bool fast, u32 sm_count, cudaStream_t st) {
+    if (a.src.max_instances == 0) return cudaSuccess;
+    static int test_fast = 0, test_any = 0, write = 0;
+    u32 per_test = 1, per_write = 1;
+    cudaError_t e = fast ? do_ctas_per_sm(k_cull_test<true>, &test_fast, &per_test) : do_ctas_per_sm(k_cull_test<false>, &test_any, &per_test);
+    if (e == cudaSuccess) e = do_ctas_per_sm(k_cull_write, &write, &per_write);
+    if (e != cudaSuccess) return e;
+    // tile kernels: every CTA resident at once, and no more CTAs than the call can have tiles
+    const unsigned test_grid = (unsigned)std::max<u64>(1, std::min<u64>(a.max_tiles, u64(sm_count) * per_test));
+    const unsigned write_grid = (unsigned)std::max<u64>(1, std::min<u64>(a.max_tiles, u64(sm_count) * per_write));
+    k_cull_plan<<<1, DO_THREADS, 0, st>>>(a);
+    if (fast) k_cull_test<true><<<test_grid, DO_THREADS, 0, st>>>(a);
+    else k_cull_test<false><<<test_grid, DO_THREADS, 0, st>>>(a);
+    k_cull_scan<<<a.src.max_instances, DO_THREADS, 0, st>>>(a);
+    k_cull_write<<<write_grid, DO_THREADS, 0, st>>>(a);
     return cudaGetLastError();
 }
 cudaError_t launch_measure_sm_clock(u64* out2, u64 window_ns, cudaStream_t st) {

@@ -193,6 +193,30 @@ u64 depth_order_max_tiles(u32 capacity_rows, u32 max_instances);
 cudaError_t launch_batch_depth_order(const DepthOrderArgs& a, bool fast, u32 sm_count, cudaStream_t st);
 #define HNB_BATCH_DEPTH_ORDER_LAUNCHES 13u
 
+// Visible particles of every instance of one batch (hnb_batch_cull): per instance, the source entries whose `position`
+// passes all six planes of the instance's frustum, in source order, at its own slab rows of `visible`, and its draw-args
+// row with that count. The instances and `position` are found as BoundsArgs describes (its acc and out are not used);
+// the tiles are depth order's (depth_order_max_tiles).
+struct CullArgs {
+    BoundsArgs src;
+    const float* frusta;     // 6 planes (a, b, c, d) per instance of the batch
+    const u32* src_list;     // d_src, indexed by slab row; NULL: the alive-list column W
+    u32* visible;            // d_visible: indexed by slab row
+    u32* args;               // d_args: 5 words (a draw-args row) per instance of the batch, 4-byte aligned
+    const u32* draw_args;    // device draw-args table, 5 words per row, `num_draw_args` rows (at least one)
+    u32 num_draw_args;
+    // Scratch, one context-owned buffer: (DO_TILE / 32 + 1) words per tile of the call, 8 words per instance, 1 word.
+    u32* mask;               // DO_TILE / 32 words per tile: bit l of word w = row 32w + l of the tile is visible
+    u32* prefix;             // 1 word per tile: its visible count (k_cull_test), then its exclusive prefix in the instance
+    u32* info;               // 8 words per instance (the tile plan): first, n, tile_base, tiles, W, rows
+    u32* total_tiles;        // [1]: tiles of the call
+    u32 max_tiles;           // depth_order_max_tiles(capacity_rows, max_instances)
+};
+// A fixed sequence of launches whatever the batch holds. `fast`: position's three words share one 16- or 32-byte column.
+cudaError_t launch_batch_cull(const CullArgs& a, bool fast, u32 sm_count, cudaStream_t st);
+#define HNB_BATCH_CULL_LAUNCHES 4u
+#define HNB_BATCH_CULL_MASK_WORDS 128u  // DO_TILE / 32: mask words per tile
+
 cudaError_t launch_indirect(const StaticTables& T, u32 num_effects, cudaStream_t st);
 cudaError_t launch_prefix_sum(const StaticTables& T, u32 num_batches, cudaStream_t st);
 cudaError_t launch_tile_prefix(const StaticTables& T, u32 batch_index, u32 tile, cudaStream_t st);

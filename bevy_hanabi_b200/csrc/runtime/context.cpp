@@ -272,6 +272,7 @@ struct hnb_ctx {
     uint64_t frame_copies = 0, frames = 0;  // hnb_simulate calls that needed the host->device copy of the frame block / all calls
     DeviceArray<unsigned long long> d_bounds_acc;  // hnb_batch_bounds: 8 slots per instance of the largest batch seen, zero between calls
     DeviceArray<uint32_t> d_depth_scratch;  // hnb_batch_depth_order: pass buffers, histograms and instance plan of the largest call seen
+    DeviceArray<uint32_t> d_cull_scratch;  // hnb_batch_cull: tile masks, tile prefixes and instance plan of the largest call seen
     DeviceArray<unsigned long long> d_debug;  // 16 diagnostic counters + a 64-frame timeline ring of 4 words (HNB_PROFILE kernels)
 
     hnb::FrameHeader* header() { return reinterpret_cast<hnb::FrameHeader*>(h_arena.get()); }
@@ -2069,6 +2070,54 @@ int32_t hnb_batch_depth_order(hnb_ctx* c, const hnb_batch_launch* b, const float
         a.max_tiles = uint32_t(max_tiles);
         CUDA_CHECK(hnb::launch_batch_depth_order(a, fast, uint32_t(c->sm_count), c->stream));
         c->launches += HNB_BATCH_DEPTH_ORDER_LAUNCHES;
+    });
+}
+
+int32_t hnb_batch_cull(hnb_ctx* c, const hnb_batch_launch* b, const float* d_frusta, uint32_t frustum_rows, const uint32_t* d_src,
+                       uint32_t src_rows, uint32_t* d_visible, uint32_t visible_rows, hnb_draw_indexed_indirect_args* d_args,
+                       uint32_t args_rows) {
+    return guarded([&] {
+        const std::string w = "hnb_batch_cull";
+        // a ribbon effect is refused before anything else about it is checked
+        if (b && (get_effect(c, b->effect).flags & HNB_EFFECT_RIBBONS))
+            fail(HNB_ERR_INVALID_ARG, w + ": a ribbon effect cannot be culled per particle, its ribbons would be re-linked");
+        const BatchPosition bp = check_batch_position(c, b, w);
+        const hnb_batch_info& bi = *bp.batch;
+        const size_t rows = bp.slab->capacity, inst = bi.prefix_sum_count;
+        if (!d_frusta || ((uintptr_t)d_frusta & 15u)) fail(HNB_ERR_INVALID_ARG, w + ": d_frusta is NULL or not 16-byte aligned");
+        if (frustum_rows < inst) fail(HNB_ERR_INVALID_ARG, w + ": frustum_rows is below the batch's instance count");
+        if (d_src && src_rows < rows) fail(HNB_ERR_INVALID_ARG, w + ": src_rows is below the slab's capacity");
+        if (!d_visible) fail(HNB_ERR_INVALID_ARG, w + ": d_visible is NULL");
+        if (visible_rows < rows) fail(HNB_ERR_INVALID_ARG, w + ": visible_rows is below the slab's capacity");
+        if (d_src && (uintptr_t)d_src < (uintptr_t)(d_visible + visible_rows) && (uintptr_t)d_visible < (uintptr_t)(d_src + src_rows))
+            fail(HNB_ERR_INVALID_ARG, w + ": d_src and d_visible overlap");
+        if (!d_args || ((uintptr_t)d_args & 3u)) fail(HNB_ERR_INVALID_ARG, w + ": d_args is NULL or not 4-byte aligned");
+        if (args_rows < inst) fail(HNB_ERR_INVALID_ARG, w + ": args_rows is below the batch's instance count");
+        if (inst == 0) return;
+        if (c->d_metadata.size() == 0) fail(HNB_ERR_INVALID_ARG, w + ": no metadata row was inserted");
+        if (c->d_draw_args.size() == 0) fail(HNB_ERR_INVALID_ARG, w + ": no draw-args row was inserted");
+        CUDA_CHECK(cudaSetDevice(c->device));
+        // scratch: a mask and a prefix word per tile, 8 words per instance, the tile count
+        const size_t max_tiles = hnb::depth_order_max_tiles(bp.slab->capacity, bi.prefix_sum_count);
+        const size_t words = (HNB_BATCH_CULL_MASK_WORDS + 1) * max_tiles + 8 * inst + 1;
+        if (c->d_cull_scratch.size() < words) CUDA_CHECK(grow(c->d_cull_scratch, words, 0, c->stream));
+
+        bool fast = false;
+        hnb::CullArgs a{};
+        a.src = batch_position_args(c, b, bp, &fast);
+        a.frusta = d_frusta;
+        a.src_list = d_src;
+        a.visible = d_visible;
+        a.args = reinterpret_cast<uint32_t*>(d_args);
+        a.draw_args = c->draw_args();
+        a.num_draw_args = uint32_t(c->d_draw_args.size());
+        a.mask = c->d_cull_scratch.get();
+        a.prefix = a.mask + HNB_BATCH_CULL_MASK_WORDS * max_tiles;
+        a.info = a.prefix + max_tiles;
+        a.total_tiles = a.info + 8 * inst;
+        a.max_tiles = uint32_t(max_tiles);
+        CUDA_CHECK(hnb::launch_batch_cull(a, fast, uint32_t(c->sm_count), c->stream));
+        c->launches += HNB_BATCH_CULL_LAUNCHES;
     });
 }
 

@@ -388,6 +388,18 @@ class Context:
         changes; only enqueues work (hnb_batch_depth_order)."""
         check(lib.hnb_batch_depth_order(self._h, C.byref(launch), d_planes, plane_rows, d_order, order_rows))
 
+    def batch_cull(self, launch: BatchLaunch, d_frusta: int, frustum_rows: int, d_src: int, src_rows: int, d_visible: int,
+                   visible_rows: int, d_args: int, args_rows: int) -> None:
+        """Cull every instance of `launch`'s batch (the descriptor of the last simulate) against its frustum
+        j = d_frusta[24j:24j+24] (six float32 planes a, b, c, d; 16-byte aligned): d_visible[first + k] receives the k-th
+        source entry, in source order, whose `position` passes all six planes, and d_args[j] (a DrawIndexedIndirectArgs) the
+        instance's draw-args row with instance_count = the visible count. Source entries are the alive list (`d_src` 0) or
+        d_src[first + i], e.g. a batch_depth_order result. `d_src` / `d_visible` (uint32, rows >= the slab's capacity,
+        indexed by slab row, not overlapping), `d_frusta` and `d_args` are device or pinned host memory. Same call window as
+        batch_bounds; nothing of the instances changes; only enqueues work (hnb_batch_cull)."""
+        check(lib.hnb_batch_cull(self._h, C.byref(launch), d_frusta, frustum_rows, d_src, src_rows, d_visible, visible_rows,
+                                 d_args, args_rows))
+
     def download_bounds(self, d_out: int, rows: int) -> np.ndarray:
         """Wait for the context stream and return `rows` records batch_bounds wrote to device memory, as BOUNDS_DTYPE."""
         return self.device_download(d_out, rows * BOUNDS_DTYPE.itemsize).view(BOUNDS_DTYPE)

@@ -712,6 +712,52 @@ HNB_API int32_t hnb_batch_bounds(hnb_ctx* ctx, const hnb_batch_launch* batch, hn
 HNB_API int32_t hnb_batch_depth_order(hnb_ctx* ctx, const hnb_batch_launch* batch, const float* d_planes, uint32_t plane_rows,
                                       uint32_t* d_order, uint32_t order_rows);
 
+/**
+ * Cull every instance's live particles against a view frustum on the device, in one call per batch, and write each
+ * instance's draw arguments: a renderer then sets up quads for the visible particles only, without a read-back of counts.
+ *
+ * `batch`, the live set and the call window are those of hnb_batch_bounds. For the batch's j-th instance (spawner row
+ * spawner_base + j), with first = its slab offset, n = min(alive_count, capacity) and W = indirect_write_index, all read on
+ * the DEVICE from the tables of the last simulated frame, the source entries e_i, i < n, each clamped to the slice, are:
+ *   - d_src == NULL: alive-list column W at first + i (entries under the identity claim of column W are i, and are not
+ *     loaded);
+ *   - otherwise: d_src[first + i], for example the d_order of hnb_batch_depth_order, for a culled back-to-front list.
+ * Visibility:
+ *   - Frustum j is d_frusta[24j .. 24j+23]: HNB_FRUSTUM_PLANES planes (a, b, c, d). Entry e is visible when
+ *     ((a*x + b*y) + c*z) + d >= 0 for all six, with (x, y, z) its `position` AS STORED and every operation one fp32
+ *     round-to-nearest step (no contraction). A NaN result fails the test; -0 >= 0 passes. No size attribute is read: the
+ *     caller adds a particle radius to d of normalised planes. For an HNB_EFFECT_LOCAL_SPACE effect, pass the planes
+ *     transformed into the emitter's space.
+ *   - d_visible[first + k] receives the k-th visible entry in ascending i, for k < m_j = the number of visible entries. The
+ *     result depends on device state alone: it is stable and bit-exact. Nothing else of d_visible is written, so one buffer
+ *     of the slab's capacity per view serves every batch of the slab. It is indexed by slab row like the alive-list
+ *     columns: a renderer binds it in place of the column the draw reads (render_indirect_read_index).
+ *   - d_args[j] receives the instance's device draw-args row (row draw_indirect_index of its spawner row, the row
+ *     hnb_read_draw_args reads) with instance_count = m_j: the indirect draw of the visible entries.
+ *
+ * Nothing of the instance is modified: no record, list, identity claim, lifetime floor, group word, alive bit, metadata
+ * word, row of the device draw-args table or mailbox word. The call reads the slab in whatever column plan it has; it
+ * neither fixes the plan of a slab that has none yet nor turns lifetime floors off. Every effect hnb_batch_bounds accepts
+ * is accepted (emitting parents, slot order, relaxed order, sector planes) except an HNB_EFFECT_RIBBONS effect: dropping a
+ * particle from its draw would re-link its ribbon.
+ *
+ * d_frusta, d_src, d_visible and d_args are memory the context's device can read / write: device memory or pinned host
+ * memory (hnb_host_alloc). Work is only enqueued on the context stream (HNB_BATCH_CULL_LAUNCHES = 4 launches, whatever the
+ * batch holds); no synchronisation, and no allocation once a context-owned scratch buffer (516 bytes per 4096 live rows and
+ * 32 bytes per instance) has grown to the largest call seen.
+ *
+ * HNB_ERR_INVALID_ARG, with nothing enqueued: every refusal of hnb_batch_bounds; an HNB_EFFECT_RIBBONS effect; `d_frusta`
+ * NULL or not 16-byte aligned; `frustum_rows` below the batch's instance count; `d_src` not NULL with `src_rows` below the
+ * slab's capacity; `d_visible` NULL; `visible_rows` below the slab's capacity; [d_src, d_src + src_rows) overlapping
+ * [d_visible, d_visible + visible_rows); `d_args` NULL or not 4-byte aligned; `args_rows` below the batch's instance count;
+ * no draw-args row inserted. A batch of zero instances is a no-op. Whatever the device tables hold, no access leaves the
+ * slab, d_frusta[0, 24 * frustum_rows), d_src[0, src_rows), d_visible[0, visible_rows) or d_args[0, args_rows).
+ */
+#define HNB_FRUSTUM_PLANES 6
+HNB_API int32_t hnb_batch_cull(hnb_ctx* ctx, const hnb_batch_launch* batch, const float* d_frusta, uint32_t frustum_rows,
+                               const uint32_t* d_src, uint32_t src_rows, uint32_t* d_visible, uint32_t visible_rows,
+                               hnb_draw_indexed_indirect_args* d_args, uint32_t args_rows);
+
 /* Individual passes, as exercised one by one by the reference's shader contract tests
  * (src/render/shader_contract_tests.rs). They run the un-fused kernels. */
 HNB_API int32_t hnb_pass_init(hnb_ctx* ctx, const hnb_batch_launch* batch);

@@ -629,6 +629,101 @@ def depth_order():
     ctx.close()
 
 
+# Frusta for the cull cases, as (a, b, c, d) planes: x in [0, 2] and the other two axes in [-2, 2] keeps about half of a
+# cloud over [-1, 1]^3; x in [0.998, 2] keeps about 0.1 % of it.
+CULL_HALF = [[1, 0, 0, 0], [-1, 0, 0, 2], [0, 1, 0, 2], [0, -1, 0, 2], [0, 0, 1, 2], [0, 0, -1, 2]]
+CULL_FEW = [[1, 0, 0, -0.998]] + CULL_HALF[1:]
+
+
+def _timed_cull(label, ctx, launch, instances, rows, alive, claimed, frustum, bounds_bytes):
+    """hnb_batch_cull of `launch`'s batch (alive-list source) into device buffers of `rows`, then hnb_batch_bounds of the
+    same batch: one warm-up call each, then the best of 5 CUDA-event windows. GB/s counts what the cull must move: 16 B of
+    position (and 4 B of list where no claim covers the row) read per live particle and 4 B written per visible one."""
+    visible = torch.empty(rows, dtype=torch.int32, device="cuda")
+    args = torch.empty(5 * instances, dtype=torch.int32, device="cuda")
+    frusta = torch.tensor([frustum] * instances, dtype=torch.float32, device="cuda")
+    call = lambda: ctx.batch_cull(launch, frusta.data_ptr(), instances, 0, 0, visible.data_ptr(), rows, args.data_ptr(), instances)  # noqa: E731
+    call()
+    ms = _events_ms(call)
+    m = int(args.view(-1, 5)[:, 1].sum())
+    report(f"cull: {label}", ms, (16 if claimed else 20) * alive + 4 * m,
+           f"{ms * 1e3:.1f} us per call, {m >> 10} Ki of {alive >> 10} Ki particles visible, best of 5")
+    _timed_bounds(f"{label} (beside cull)", ctx, launch, instances, bounds_bytes)
+
+
+def cull():
+    """hnb_batch_cull: the filled 64 Mi C5 instance under its claim with about half and with about 0.1 % of it visible,
+    the same size spawned by one init burst, C4's topology in one call, the 16 Mi-slot churn steady state and single
+    instances of 4 Ki and 16 Ki (latency); each beside hnb_batch_bounds of the same batch, and a 2 GiB device-to-device
+    copy for scale."""
+    _card()
+    a = torch.empty(2 << 30, dtype=torch.uint8, device="cuda")
+    b = torch.empty_like(a)
+    ms = _events_ms(lambda: b.copy_(a))
+    report("cull: 2 GiB device-to-device copy", ms, 2 * a.numel(), "torch copy_ (reads 2 GiB and writes 2 GiB), best of 5")
+    del a, b
+    torch.cuda.empty_cache()
+
+    P = 64 << 20
+    ctx = hb.Context(0, stream.cuda_stream)
+    effect = ctx.effect_compile(recipes.c5_lowered())
+    slab = ctx.slab_create(P, 32)
+    ctx.slab_fill_c5(slab, 0, P, 42, 1e9, 1e9)
+    single_instance(ctx, P, 32, alive=P)
+    la = N.BatchLaunch.make(effect, slab, 0, 0)
+    ctx.simulate([la])
+    _timed_cull("C5 64Mi filled, claim, ~half visible", ctx, la, 1, P, P, True, CULL_HALF, 16 * P)
+    _timed_cull("C5 64Mi filled, claim, ~0.1 % visible", ctx, la, 1, P, P, True, CULL_FEW, 16 * P)
+    ctx.slab_destroy(slab)
+    slab = ctx.slab_create(P, 32)
+    single_instance(ctx, P, 32, alive=0, spawn=P)
+    ctx.simulate([N.BatchLaunch.make(effect, slab, 0, P)])
+    ctx.upload_spawners([R.make_spawner(spawn=0, seed=43)])
+    la = N.BatchLaunch.make(effect, slab, 0, 0)
+    ctx.simulate([la])
+    _timed_cull("C5 64Mi from one init burst, no claim", ctx, la, 1, P, P, False, CULL_HALF, 20 * P)
+    ctx.close()
+    torch.cuda.empty_cache()
+
+    n_inst, cap = 1024, 65536
+    ctx = hb.Context(0, stream.cuda_stream)
+    effect = ctx.effect_compile(recipes.c5_lowered())
+    slab = ctx.slab_create(n_inst * cap, 32)
+    sp = []
+    for i in range(n_inst):
+        ctx.slab_fill_c5(slab, i * cap, cap, 7000 + i, 1e9, 1e9)  # the last fill holds the slab's claim
+        m = R.initial_metadata(cap, i, 8)
+        m.alive_count, m.max_spawn = cap, 0
+        ctx.metadata_insert(i, m)
+        ctx.draw_args_insert(i)
+        sp.append(R.make_spawner(seed=i, effect_metadata_index=i, draw_indirect_index=i, slab_offset=i * cap))
+    ctx.upload_spawners(sp)
+    ctx.upload_batches([N.BatchInfo(0, 0, 0, 0, 0, n_inst)], [0] * n_inst)
+    ctx.set_sim_params(1 / 60, 0.0, n_inst)
+    la = N.BatchLaunch.make(effect, slab, 0, 0)
+    ctx.simulate([la])
+    _timed_cull("C4 shape: 1024 x 65536 in one batch", ctx, la, n_inst, n_inst * cap, n_inst * cap, False, CULL_HALF,
+                20 * n_inst * cap - 4 * cap)
+    ctx.close()
+    torch.cuda.empty_cache()
+
+    for cap in (4096, 16 << 10):
+        ctx = hb.Context(0, stream.cuda_stream)
+        slab = ctx.slab_create(cap, 32)
+        ctx.slab_fill_c5(slab, 0, cap, 100, 1e9, 1e9)
+        single_instance(ctx, cap, 32, alive=cap)
+        la = N.BatchLaunch.make(ctx.effect_compile(recipes.c5_lowered()), slab, 0, 0)
+        ctx.simulate([la])
+        _timed_cull(f"one instance of {cap >> 10} Ki particles (latency)", ctx, la, 1, cap, cap, True, CULL_HALF, 16 * cap)
+        ctx.close()
+
+    P, ctx, slab, effect, stride, dt, rate = _churned()
+    alive = ctx.read_metadata(0).alive_count
+    _timed_cull(f"churned {P >> 20} Mi slots, {alive >> 10} Ki alive, permuted list", ctx, N.BatchLaunch.make(effect, slab, 0, rate), 1, P,
+                alive, False, CULL_HALF, 20 * alive)
+    ctx.close()
+
+
 class _DeviceColumn:
     """A device column as torch sees it through __cuda_array_interface__."""
 
@@ -878,7 +973,7 @@ def emitter_relocation():
     ctx.close()
 
 
-SCENARIOS = {"c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "bounds": bounds, "depth_order": depth_order, "emitter_relocation": emitter_relocation, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
+SCENARIOS = {"cull": cull, "c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "bounds": bounds, "depth_order": depth_order, "emitter_relocation": emitter_relocation, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
 if __name__ == "__main__":
     for name in (sys.argv[1:] or list(SCENARIOS)):
         try:
