@@ -216,6 +216,7 @@ SIGNATURES = {
     "hnb_batch_bounds": (i32, [vp, P(BatchLaunch), vp, u32]),
     "hnb_batch_depth_order": (i32, [vp, P(BatchLaunch), vp, u32, vp, u32]),
     "hnb_batch_cull": (i32, [vp, P(BatchLaunch), vp, u32, vp, u32, vp, u32, vp, u32]),
+    "hnb_batch_cull_views": (i32, [vp, P(BatchLaunch), u32, vp, u32, vp, u32, vp, u32, vp, u32]),
     "hnb_pass_init": (i32, [vp, P(BatchLaunch)]),
     "hnb_pass_indirect": (i32, [vp]),
     "hnb_pass_prefix_sum": (i32, [vp]),

@@ -1468,6 +1468,9 @@ __global__ void __launch_bounds__(DO_THREADS) k_do_hist(DepthOrderArgs a, u32 pa
 //   k_cull_test   per tile: source entries, positions, the six plane tests; the tile's mask and visible count
 //   k_cull_scan   per instance (one CTA): tile counts -> exclusive prefixes; the instance's draw-args row with its count
 //   k_cull_write  per tile: each visible entry to first + prefix + its rank in the mask, so a warp's stores are consecutive
+// Several views with one source (hnb_batch_cull_views) take the same plan and the same tile bodies for every view at
+// once: k_cull_views_test loads each row's entry and position once and keeps a mask and a count per (tile, view),
+// k_cull_views_scan runs per (instance, view), and k_cull_views_write loads an entry once for all views that see it.
 // ---------------------------------------------------------------------------------------------
 #define CULL_PLANES 6
 #define CULL_WORDS (DO_TILE / 32)  // mask words per tile: DO_ITEMS per warp
@@ -1475,16 +1478,16 @@ static_assert(CULL_WORDS == HNB_BATCH_CULL_MASK_WORDS && CULL_WORDS == DO_WARPS 
 #define CULL_ITEMS 8               // items of a thread with loads in flight together (DO_ITEMS / CULL_ITEMS rounds per tile)
 #define CULL_SCAN_ITEMS 16         // tile counts per thread per round of k_cull_scan
 
-// ((a*x + b*y) + c*z) + d >= 0 for all six planes, each step rounded on its own: a NaN fails, -0 passes.
+// ((a*x + b*y) + c*z) + d >= 0 for plane q = (a, b, c, d), each step rounded on its own: a NaN fails, -0 passes.
+__device__ __forceinline__ bool cull_plane(const float* q, u32 x, u32 y, u32 z) {
+    const float v = do_add(do_add(do_add(do_mul(q[0], __uint_as_float(x)), do_mul(q[1], __uint_as_float(y))),
+                                  do_mul(q[2], __uint_as_float(z))), q[3]);
+    return v >= 0.0f;
+}
 __device__ __forceinline__ bool cull_inside(const float* f, u32 x, u32 y, u32 z) {
     bool inside = true;
 #pragma unroll
-    for (int p = 0; p < CULL_PLANES; ++p) {
-        const float* q = f + 4 * p;
-        const float v = do_add(do_add(do_add(do_mul(q[0], __uint_as_float(x)), do_mul(q[1], __uint_as_float(y))),
-                                      do_mul(q[2], __uint_as_float(z))), q[3]);
-        inside &= v >= 0.0f;
-    }
+    for (int p = 0; p < CULL_PLANES; ++p) inside &= cull_plane(f + 4 * p, x, y, z);
     return inside;
 }
 
@@ -1503,12 +1506,17 @@ __global__ void __launch_bounds__(DO_THREADS) k_cull_plan(CullArgs a) {
     do_tile_plan(a.src, a.info, a.total_tiles, a.max_tiles, s_warp);
 }
 
-// Persistent grid over the call's tiles. The instance's frustum is staged in shared memory when a CTA's instance changes
-// (it may sit in pinned host memory). FAST: position in one 16-byte load per row, as k_bounds_reduce.
-template <bool FAST>
-__global__ void __launch_bounds__(DO_THREADS) k_cull_test(CullArgs a) {
-    __shared__ float s_frustum[4 * CULL_PLANES];
-    __shared__ u32 s_count;
+// The tile passes below serve one view (hnb_batch_cull: NV = 1, views = 1) and up to NV views (hnb_batch_cull_views)
+// with one body. View v's scratch is block v of `mask` and `prefix` (max_tiles tiles each); view 0's block is the whole
+// single-view scratch. Only views < `views` are touched.
+
+// Persistent grid over the call's tiles. The instance's frusta, one per view, `frustum_stride` floats apart, are staged
+// in shared memory when a CTA's instance changes (they may sit in pinned host memory). Each row's entry and position are
+// loaded once and tested against every view; each view gets the tile's mask and visible count. FAST: position in one
+// 16-byte load per row, as k_bounds_reduce.
+template <bool FAST, u32 NV>
+__device__ __forceinline__ void cull_test_tiles(const CullArgs& a, u32 views, u64 frustum_stride, float* s_frustum, u32* s_count) {
+    static_assert(4 * CULL_PLANES * NV <= DO_THREADS, "one thread stages one frustum word");
     const u32 count = bounds_count(a.src), total = *a.total_tiles, tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
     const u64 claim0 = hnb_claim_load(&a.src.claim[0]), claim1 = hnb_claim_load(&a.src.claim[1]);
     const BoundsArgs& s = a.src;
@@ -1519,17 +1527,21 @@ __global__ void __launch_bounds__(DO_THREADS) k_cull_test(CullArgs a) {
         const u32 t = g - in.tile_base;
         if (t >= in.tiles) continue;  // CTA-uniform
         __syncthreads();              // the previous tile's readers of s_frustum and s_count are done
-        if (j != staged && tid < 4u * CULL_PLANES) s_frustum[tid] = a.frusta[u64(j) * (4u * CULL_PLANES) + tid];
-        if (tid == 0u) s_count = 0u;
+        if (j != staged && tid < 4u * CULL_PLANES * views) {
+            const u32 v = tid / (4u * CULL_PLANES), k = tid % (4u * CULL_PLANES);
+            s_frustum[tid] = a.frusta[u64(v) * frustum_stride + u64(j) * (4u * CULL_PLANES) + k];
+        }
+        if (tid < views) s_count[tid] = 0u;
         staged = j;
         __syncthreads();
         const CullSource src = cull_source(a, in, claim0, claim1);
         const u32 i0 = t * DO_TILE + warp * DO_WARP_ROWS + lane;
-        u32 word = 0u, seen = 0u;
+        u32 word[NV], seen[NV];
+#pragma unroll
+        for (u32 v = 0; v < NV; ++v) word[v] = seen[v] = 0u;
 #pragma unroll
         for (u32 h = 0; h < DO_ITEMS; h += CULL_ITEMS) {
-            u32 e[CULL_ITEMS];
-            bool vis[CULL_ITEMS];
+            u32 e[CULL_ITEMS], p[CULL_ITEMS][3];
 #pragma unroll
             for (u32 k = 0; k < CULL_ITEMS; ++k) {
                 const u32 i = i0 + (h + k) * 32u;
@@ -1538,50 +1550,78 @@ __global__ void __launch_bounds__(DO_THREADS) k_cull_test(CullArgs a) {
             if (FAST) {
                 const RepackPiece<4>* col = (const RepackPiece<4>*)s.col[0];
                 const u32 quads = s.col_words[0] >> 2u, quad = s.col_lane[0] >> 2u;
-                RepackPiece<4> v[CULL_ITEMS];
 #pragma unroll
-                for (u32 k = 0; k < CULL_ITEMS; ++k)
-                    if (i0 + (h + k) * 32u < in.n) v[k] = col[(u64(in.first) + e[k]) * quads + quad];
+                for (u32 k = 0; k < CULL_ITEMS; ++k) {
+                    if (i0 + (h + k) * 32u >= in.n) continue;
+                    const RepackPiece<4> q = col[(u64(in.first) + e[k]) * quads + quad];
 #pragma unroll
-                for (u32 k = 0; k < CULL_ITEMS; ++k)
-                    vis[k] = i0 + (h + k) * 32u < in.n && cull_inside(s_frustum, v[k].w[0], v[k].w[1], v[k].w[2]);
+                    for (int c = 0; c < 3; ++c) p[k][c] = q.w[c];
+                }
             } else {
-                u32 v[CULL_ITEMS][3];
 #pragma unroll
                 for (u32 k = 0; k < CULL_ITEMS; ++k) {
                     if (i0 + (h + k) * 32u >= in.n) continue;
 #pragma unroll
-                    for (int c = 0; c < 3; ++c) v[k][c] = s.col[c][(u64(in.first) + e[k]) * s.col_words[c] + s.col_lane[c]];
+                    for (int c = 0; c < 3; ++c) p[k][c] = s.col[c][(u64(in.first) + e[k]) * s.col_words[c] + s.col_lane[c]];
+                }
+            }
+#pragma unroll
+            for (u32 v = 0; v < NV; ++v) {
+                if (v >= views) break;  // CTA-uniform
+                bool vis[CULL_ITEMS];
+                if (NV == 1) {
+                    // one view: its planes stay in registers for the whole tile
+#pragma unroll
+                    for (u32 k = 0; k < CULL_ITEMS; ++k)
+                        vis[k] = i0 + (h + k) * 32u < in.n && cull_inside(s_frustum, p[k][0], p[k][1], p[k][2]);
+                } else {
+                    // plane by plane over the items: one read of a plane from shared memory serves CULL_ITEMS rows
+#pragma unroll
+                    for (u32 k = 0; k < CULL_ITEMS; ++k) vis[k] = i0 + (h + k) * 32u < in.n;
+#pragma unroll
+                    for (u32 pl = 0; pl < CULL_PLANES; ++pl) {
+                        float q[4];
+#pragma unroll
+                        for (int c = 0; c < 4; ++c) q[c] = s_frustum[4u * (CULL_PLANES * v + pl) + c];
+#pragma unroll
+                        for (u32 k = 0; k < CULL_ITEMS; ++k) vis[k] = vis[k] && cull_plane(q, p[k][0], p[k][1], p[k][2]);
+                    }
                 }
 #pragma unroll
-                for (u32 k = 0; k < CULL_ITEMS; ++k)
-                    vis[k] = i0 + (h + k) * 32u < in.n && cull_inside(s_frustum, v[k][0], v[k][1], v[k][2]);
-            }
-#pragma unroll
-            for (u32 k = 0; k < CULL_ITEMS; ++k) {
-                const u32 b = __ballot_sync(0xffffffffu, vis[k]);
-                if (lane == h + k) word = b;
-                seen += __popc(b);
+                for (u32 k = 0; k < CULL_ITEMS; ++k) {
+                    const u32 b = __ballot_sync(0xffffffffu, vis[k]);
+                    if (lane == h + k) word[v] = b;
+                    seen[v] += __popc(b);
+                }
             }
         }
-        if (lane < DO_ITEMS) a.mask[u64(g) * CULL_WORDS + warp * DO_ITEMS + lane] = word;
-        if (lane == 0u && seen) atomicAdd(&s_count, seen);
+#pragma unroll
+        for (u32 v = 0; v < NV; ++v) {
+            if (v >= views) break;
+            if (lane < DO_ITEMS) a.mask[(u64(v) * a.max_tiles + g) * CULL_WORDS + warp * DO_ITEMS + lane] = word[v];
+            if (lane == 0u && seen[v]) atomicAdd(&s_count[v], seen[v]);
+        }
         __syncthreads();
-        if (tid == 0u) a.prefix[g] = s_count;
+        if (tid < views) a.prefix[u64(tid) * a.max_tiles + g] = s_count[tid];
     }
 }
 
-// CTA j, one per instance the call covers: the visible counts of instance j's tiles become exclusive prefixes within the
-// instance, and d_args[j] receives the draw-args row its spawner row names (clamped to the table) with instance_count =
-// the instance's visible total (0 for a j past the batch's device-side count).
-__global__ void __launch_bounds__(DO_THREADS) k_cull_scan(CullArgs a) {
-    __shared__ u32 s_warp[DO_WARPS];
-    __shared__ u32 s_round;
-    const u32 j = blockIdx.x, tid = threadIdx.x;
+template <bool FAST>
+__global__ void __launch_bounds__(DO_THREADS) k_cull_test(CullArgs a) {
+    __shared__ float s_frustum[4 * CULL_PLANES];
+    __shared__ u32 s_count[1];
+    cull_test_tiles<FAST, 1>(a, 1u, 0u, s_frustum, s_count);
+}
+
+// One CTA: the visible counts of instance j's tiles in a view's `prefix` block become exclusive prefixes within the
+// instance, and args[j] (of that view's args rows) receives the draw-args row its spawner row names (clamped to the
+// table) with instance_count = the instance's visible total (0 for a j past the batch's device-side count).
+__device__ __forceinline__ void cull_scan_instance(const CullArgs& a, u32 j, u32* prefix, u32* args, u32* s_warp, u32* s_round) {
+    const u32 tid = threadIdx.x;
     u32 m = 0u;
     if (j < bounds_count(a.src)) {  // CTA-uniform
         const DepthInstance in = do_instance(a.info, j);
-        u32* c = a.prefix + in.tile_base;
+        u32* c = prefix + in.tile_base;
         for (u32 t0 = 0; t0 < in.tiles; t0 += DO_THREADS * CULL_SCAN_ITEMS) {
             const u32 tb = t0 + tid * CULL_SCAN_ITEMS;
             u32 v[CULL_SCAN_ITEMS], sum = 0u;
@@ -1597,23 +1637,31 @@ __global__ void __launch_bounds__(DO_THREADS) k_cull_scan(CullArgs a) {
                 run += v[q];
             }
             __syncthreads();  // s_round of the previous round is read
-            if (tid == DO_THREADS - 1u) s_round = run;
+            if (tid == DO_THREADS - 1u) *s_round = run;
             __syncthreads();
-            m = s_round;
+            m = *s_round;
         }
     }
     if (tid < HNB_DRAW_INDEXED_INDIRECT_STRIDE) {
         const u64 row = u64(a.src.batch_info->spawner_base) + j;
         const Spawner* sp = &a.src.spawners[row < a.src.num_spawners ? row : a.src.num_spawners - 1u];
         const u32 dri = min(sp->draw_indirect_index, a.num_draw_args - 1u);
-        a.args[u64(j) * HNB_DRAW_INDEXED_INDIRECT_STRIDE + tid] = tid == 1u ? m : a.draw_args[u64(dri) * HNB_DRAW_INDEXED_INDIRECT_STRIDE + tid];
+        args[u64(j) * HNB_DRAW_INDEXED_INDIRECT_STRIDE + tid] = tid == 1u ? m : a.draw_args[u64(dri) * HNB_DRAW_INDEXED_INDIRECT_STRIDE + tid];
     }
 }
 
-// Persistent grid over the call's tiles: a visible row's place is its tile's prefix plus the visible rows before it in
-// the tile's mask. The entries are loaded again (only where a mask bit is set); places are clamped to the instance's n.
-__global__ void __launch_bounds__(DO_THREADS) k_cull_write(CullArgs a) {
+// CTA j, one per instance the call covers.
+__global__ void __launch_bounds__(DO_THREADS) k_cull_scan(CullArgs a) {
     __shared__ u32 s_warp[DO_WARPS];
+    __shared__ u32 s_round;
+    cull_scan_instance(a, blockIdx.x, a.prefix, a.args, s_warp, &s_round);
+}
+
+// Persistent grid over the call's tiles: a visible row's place in a view is its tile's prefix there plus the visible rows
+// before it in the view's mask. A row's entry is loaded again, once, where any view's mask bit is set, and stored to every
+// such view, whose entries lie `visible_stride` words after the previous view's; places are clamped to the instance's n.
+template <u32 NV>
+__device__ __forceinline__ void cull_write_tiles(const CullArgs& a, u32 views, u64 visible_stride, u32* s_warp) {
     const u32 count = bounds_count(a.src), total = *a.total_tiles, tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
     const u64 claim0 = hnb_claim_load(&a.src.claim[0]), claim1 = hnb_claim_load(&a.src.claim[1]);
     const u32 lt = (1u << lane) - 1u;
@@ -1621,19 +1669,65 @@ __global__ void __launch_bounds__(DO_THREADS) k_cull_write(CullArgs a) {
         const DepthInstance in = do_instance(a.info, do_find(a.info, count, g));
         const u32 t = g - in.tile_base;
         if (t >= in.tiles) continue;  // CTA-uniform
-        // lane k < DO_ITEMS holds mask word k of its warp and the visible rows of the tile before that word
-        const u32 word = lane < DO_ITEMS ? a.mask[u64(g) * CULL_WORDS + warp * DO_ITEMS + lane] : 0u;
-        const u32 before = a.prefix[g] + do_block_exclusive(__popc(word), s_warp);
+        // lane k < DO_ITEMS holds mask word k of its warp in each view and the view's visible rows of the tile before it
+        u32 word[NV], before[NV];
+#pragma unroll
+        for (u32 v = 0; v < NV; ++v) {
+            if (v >= views) break;  // CTA-uniform
+            const u64 vg = u64(v) * a.max_tiles + g;
+            word[v] = lane < DO_ITEMS ? a.mask[vg * CULL_WORDS + warp * DO_ITEMS + lane] : 0u;
+            before[v] = a.prefix[vg] + do_block_exclusive(__popc(word[v]), s_warp);
+        }
         const CullSource src = cull_source(a, in, claim0, claim1);
         const u32 i0 = t * DO_TILE + warp * DO_WARP_ROWS + lane;
 #pragma unroll
         for (u32 k = 0; k < DO_ITEMS; ++k) {
-            const u32 wk = __shfl_sync(0xffffffffu, word, k), bk = __shfl_sync(0xffffffffu, before, k);
-            if (!((wk >> lane) & 1u)) continue;
-            const u32 r = min(bk + __popc(wk & lt), in.n - 1u);
-            a.visible[u64(in.first) + r] = cull_entry(src, i0 + k * 32u);
+            u32 wk[NV], bk[NV], any = 0u;
+#pragma unroll
+            for (u32 v = 0; v < NV; ++v) {
+                if (v >= views) break;
+                wk[v] = __shfl_sync(0xffffffffu, word[v], k);
+                bk[v] = __shfl_sync(0xffffffffu, before[v], k);
+                any |= wk[v];
+            }
+            if (!((any >> lane) & 1u)) continue;
+            const u32 e = cull_entry(src, i0 + k * 32u);
+#pragma unroll
+            for (u32 v = 0; v < NV; ++v) {
+                if (v >= views) break;
+                if (!((wk[v] >> lane) & 1u)) continue;
+                const u32 r = min(bk[v] + __popc(wk[v] & lt), in.n - 1u);
+                a.visible[u64(v) * visible_stride + in.first + r] = e;
+            }
         }
     }
+}
+
+__global__ void __launch_bounds__(DO_THREADS) k_cull_write(CullArgs a) {
+    __shared__ u32 s_warp[DO_WARPS];
+    cull_write_tiles<1>(a, 1u, 0u, s_warp);
+}
+
+// hnb_batch_cull_views: the same passes for a.views views, after the same k_cull_plan.
+template <bool FAST>
+__global__ void __launch_bounds__(DO_THREADS, 2) k_cull_views_test(CullViewsArgs a) {
+    __shared__ float s_frustum[4 * CULL_PLANES * HNB_BATCH_CULL_MAX_VIEWS];
+    __shared__ u32 s_count[HNB_BATCH_CULL_MAX_VIEWS];
+    cull_test_tiles<FAST, HNB_BATCH_CULL_MAX_VIEWS>(a.c, a.views, u64(a.frustum_rows) * (4u * CULL_PLANES), s_frustum, s_count);
+}
+
+// CTA v * max_instances + j: instance j in view v.
+__global__ void __launch_bounds__(DO_THREADS) k_cull_views_scan(CullViewsArgs a) {
+    __shared__ u32 s_warp[DO_WARPS];
+    __shared__ u32 s_round;
+    const u32 j = blockIdx.x % a.c.src.max_instances, v = blockIdx.x / a.c.src.max_instances;
+    cull_scan_instance(a.c, j, a.c.prefix + u64(v) * a.c.max_tiles, a.c.args + u64(v) * a.args_rows * HNB_DRAW_INDEXED_INDIRECT_STRIDE,
+                       s_warp, &s_round);
+}
+
+__global__ void __launch_bounds__(DO_THREADS) k_cull_views_write(CullViewsArgs a) {
+    __shared__ u32 s_warp[DO_WARPS];
+    cull_write_tiles<HNB_BATCH_CULL_MAX_VIEWS>(a.c, a.views, a.visible_rows, s_warp);
 }
 
 // Effective SM clock: cycles elapsed on one SM over ~`window_ns` of the global timer.
@@ -1873,22 +1967,33 @@ template <typename K> static cudaError_t do_ctas_per_sm(K kernel, int* cached, u
     *out = u32(*cached);
     return cudaSuccess;
 }
-cudaError_t launch_batch_cull(const CullArgs& a, bool fast, u32 sm_count, cudaStream_t st) {
-    if (a.src.max_instances == 0) return cudaSuccess;
-    static int test_fast = 0, test_any = 0, write = 0;
+// The four launches of a cull over args `a` (`c`: its single-view part): tile kernels with every CTA resident at once and
+// no more CTAs than the call can have tiles; `scan_ctas` CTAs of `scan`.
+template <typename A>
+static cudaError_t cull_launches(const A& a, const CullArgs& c, void (*test)(A), int* test_cached, void (*scan)(A), u64 scan_ctas,
+                                 void (*write)(A), int* write_cached, u32 sm_count, cudaStream_t st) {
+    if (c.src.max_instances == 0) return cudaSuccess;
     u32 per_test = 1, per_write = 1;
-    cudaError_t e = fast ? do_ctas_per_sm(k_cull_test<true>, &test_fast, &per_test) : do_ctas_per_sm(k_cull_test<false>, &test_any, &per_test);
-    if (e == cudaSuccess) e = do_ctas_per_sm(k_cull_write, &write, &per_write);
+    cudaError_t e = do_ctas_per_sm(test, test_cached, &per_test);
+    if (e == cudaSuccess) e = do_ctas_per_sm(write, write_cached, &per_write);
     if (e != cudaSuccess) return e;
-    // tile kernels: every CTA resident at once, and no more CTAs than the call can have tiles
-    const unsigned test_grid = (unsigned)std::max<u64>(1, std::min<u64>(a.max_tiles, u64(sm_count) * per_test));
-    const unsigned write_grid = (unsigned)std::max<u64>(1, std::min<u64>(a.max_tiles, u64(sm_count) * per_write));
-    k_cull_plan<<<1, DO_THREADS, 0, st>>>(a);
-    if (fast) k_cull_test<true><<<test_grid, DO_THREADS, 0, st>>>(a);
-    else k_cull_test<false><<<test_grid, DO_THREADS, 0, st>>>(a);
-    k_cull_scan<<<a.src.max_instances, DO_THREADS, 0, st>>>(a);
-    k_cull_write<<<write_grid, DO_THREADS, 0, st>>>(a);
+    const unsigned test_grid = (unsigned)std::max<u64>(1, std::min<u64>(c.max_tiles, u64(sm_count) * per_test));
+    const unsigned write_grid = (unsigned)std::max<u64>(1, std::min<u64>(c.max_tiles, u64(sm_count) * per_write));
+    k_cull_plan<<<1, DO_THREADS, 0, st>>>(c);
+    test<<<test_grid, DO_THREADS, 0, st>>>(a);
+    scan<<<(unsigned)scan_ctas, DO_THREADS, 0, st>>>(a);
+    write<<<write_grid, DO_THREADS, 0, st>>>(a);
     return cudaGetLastError();
+}
+cudaError_t launch_batch_cull(const CullArgs& a, bool fast, u32 sm_count, cudaStream_t st) {
+    static int test_fast = 0, test_any = 0, write = 0;
+    return cull_launches(a, a, fast ? k_cull_test<true> : k_cull_test<false>, fast ? &test_fast : &test_any, k_cull_scan,
+                         a.src.max_instances, k_cull_write, &write, sm_count, st);
+}
+cudaError_t launch_batch_cull_views(const CullViewsArgs& a, bool fast, u32 sm_count, cudaStream_t st) {
+    static int test_fast = 0, test_any = 0, write = 0;
+    return cull_launches(a, a.c, fast ? k_cull_views_test<true> : k_cull_views_test<false>, fast ? &test_fast : &test_any,
+                         k_cull_views_scan, u64(a.c.src.max_instances) * a.views, k_cull_views_write, &write, sm_count, st);
 }
 cudaError_t launch_measure_sm_clock(u64* out2, u64 window_ns, cudaStream_t st) {
     k_measure_sm_clock<<<1, 1, 0, st>>>(out2, window_ns);

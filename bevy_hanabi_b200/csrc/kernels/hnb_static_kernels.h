@@ -217,6 +217,21 @@ cudaError_t launch_batch_cull(const CullArgs& a, bool fast, u32 sm_count, cudaSt
 #define HNB_BATCH_CULL_LAUNCHES 4u
 #define HNB_BATCH_CULL_MASK_WORDS 128u  // DO_TILE / 32: mask words per tile
 
+// Visible particles of every instance of one batch in up to HNB_BATCH_CULL_MAX_VIEWS views (hnb_batch_cull_views), with
+// one shared source: view v's part of each stacked buffer is what a CullArgs with v's frusta, visible and args would
+// name. The scratch holds `views` blocks of masks, then `views` blocks of prefixes (max_tiles tiles each), then the
+// plan: c.mask, c.prefix = c.mask + views * DO_TILE / 32 * max_tiles, c.info = c.prefix + views * max_tiles.
+struct CullViewsArgs {
+    CullArgs c;              // view 0's frusta, visible and args, the shared source and the scratch
+    u32 views;               // 1 .. HNB_BATCH_CULL_MAX_VIEWS
+    u32 frustum_rows;        // view v's frusta: c.frusta + 24 * v * frustum_rows
+    u32 visible_rows;        // view v's entries: c.visible + v * visible_rows
+    u32 args_rows;           // view v's args rows: c.args + 5 * v * args_rows
+};
+// The launches of launch_batch_cull (HNB_BATCH_CULL_LAUNCHES), whatever `views` is.
+cudaError_t launch_batch_cull_views(const CullViewsArgs& a, bool fast, u32 sm_count, cudaStream_t st);
+#define HNB_BATCH_CULL_MAX_VIEWS 8u
+
 cudaError_t launch_indirect(const StaticTables& T, u32 num_effects, cudaStream_t st);
 cudaError_t launch_prefix_sum(const StaticTables& T, u32 num_batches, cudaStream_t st);
 cudaError_t launch_tile_prefix(const StaticTables& T, u32 batch_index, u32 tile, cudaStream_t st);

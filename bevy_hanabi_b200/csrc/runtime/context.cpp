@@ -36,6 +36,7 @@ static_assert(sizeof(hnb_effect_metadata) == 60 && sizeof(hnb::EffectMetadata) =
 static_assert(sizeof(hnb_batch_info) == 24 && sizeof(hnb::BatchInfo) == 24, "GpuBatchInfo is 24 bytes");
 static_assert(sizeof(hnb_sim_params) == 28 && sizeof(hnb::SimParams) == 28, "GpuSimParams is 28 bytes");
 static_assert(sizeof(hnb_draw_indexed_indirect_args) == 20, "GpuDrawIndexedIndirectArgs is 20 bytes");
+static_assert(HNB_BATCH_CULL_MAX_VIEWS == HNB_CULL_MAX_VIEWS, "the multi-view cull kernels hold every view the C API accepts");
 static_assert(sizeof(hnb_indirect_index) == 12, "GpuIndirectIndex is 12 bytes");
 static_assert(sizeof(hnb_child_info) == 8 && sizeof(hnb::ChildInfo) == 8, "GpuChildInfo is 8 bytes");
 static_assert(sizeof(hnb::FrameHeader) == 64, "frame header is 64 bytes");
@@ -2073,51 +2074,76 @@ int32_t hnb_batch_depth_order(hnb_ctx* c, const hnb_batch_launch* b, const float
     });
 }
 
+// hnb_batch_cull (views = 1) and hnb_batch_cull_views: `views` views stacked view-major in d_frusta, d_visible and
+// d_args, with one source. Refusals name the entry point `w`.
+static void batch_cull(hnb_ctx* c, const hnb_batch_launch* b, const std::string& w, uint32_t views, const float* d_frusta,
+                       uint32_t frustum_rows, const uint32_t* d_src, uint32_t src_rows, uint32_t* d_visible, uint32_t visible_rows,
+                       hnb_draw_indexed_indirect_args* d_args, uint32_t args_rows) {
+    // a ribbon effect is refused before anything else about it is checked
+    if (b && (get_effect(c, b->effect).flags & HNB_EFFECT_RIBBONS))
+        fail(HNB_ERR_INVALID_ARG, w + ": a ribbon effect cannot be culled per particle, its ribbons would be re-linked");
+    if (views == 0 || views > HNB_CULL_MAX_VIEWS) fail(HNB_ERR_INVALID_ARG, w + ": views is 0 or above HNB_CULL_MAX_VIEWS");
+    const BatchPosition bp = check_batch_position(c, b, w);
+    const hnb_batch_info& bi = *bp.batch;
+    const size_t rows = bp.slab->capacity, inst = bi.prefix_sum_count;
+    if (!d_frusta || ((uintptr_t)d_frusta & 15u)) fail(HNB_ERR_INVALID_ARG, w + ": d_frusta is NULL or not 16-byte aligned");
+    if (frustum_rows < inst) fail(HNB_ERR_INVALID_ARG, w + ": frustum_rows is below the batch's instance count");
+    if (d_src && src_rows < rows) fail(HNB_ERR_INVALID_ARG, w + ": src_rows is below the slab's capacity");
+    if (!d_visible) fail(HNB_ERR_INVALID_ARG, w + ": d_visible is NULL");
+    if (visible_rows < rows) fail(HNB_ERR_INVALID_ARG, w + ": visible_rows is below the slab's capacity");
+    // d_src against every view's entries
+    if (d_src && (uintptr_t)d_src < (uintptr_t)(d_visible + size_t(views) * visible_rows) && (uintptr_t)d_visible < (uintptr_t)(d_src + src_rows))
+        fail(HNB_ERR_INVALID_ARG, w + ": d_src and d_visible overlap");
+    if (!d_args || ((uintptr_t)d_args & 3u)) fail(HNB_ERR_INVALID_ARG, w + ": d_args is NULL or not 4-byte aligned");
+    if (args_rows < inst) fail(HNB_ERR_INVALID_ARG, w + ": args_rows is below the batch's instance count");
+    if (inst == 0) return;
+    if (c->d_metadata.size() == 0) fail(HNB_ERR_INVALID_ARG, w + ": no metadata row was inserted");
+    if (c->d_draw_args.size() == 0) fail(HNB_ERR_INVALID_ARG, w + ": no draw-args row was inserted");
+    CUDA_CHECK(cudaSetDevice(c->device));
+    // scratch: per view a mask and a prefix word per tile; 8 words per instance, the tile count
+    const size_t max_tiles = hnb::depth_order_max_tiles(bp.slab->capacity, bi.prefix_sum_count);
+    const size_t words = views * (HNB_BATCH_CULL_MASK_WORDS + 1) * max_tiles + 8 * inst + 1;
+    if (c->d_cull_scratch.size() < words) CUDA_CHECK(grow(c->d_cull_scratch, words, 0, c->stream));
+
+    bool fast = false;
+    hnb::CullViewsArgs v{};
+    hnb::CullArgs& a = v.c;
+    a.src = batch_position_args(c, b, bp, &fast);
+    a.frusta = d_frusta;
+    a.src_list = d_src;
+    a.visible = d_visible;
+    a.args = reinterpret_cast<uint32_t*>(d_args);
+    a.draw_args = c->draw_args();
+    a.num_draw_args = uint32_t(c->d_draw_args.size());
+    a.mask = c->d_cull_scratch.get();
+    a.prefix = a.mask + views * HNB_BATCH_CULL_MASK_WORDS * max_tiles;
+    a.info = a.prefix + views * max_tiles;
+    a.total_tiles = a.info + 8 * inst;
+    a.max_tiles = uint32_t(max_tiles);
+    v.views = views;
+    v.frustum_rows = frustum_rows;
+    v.visible_rows = visible_rows;
+    v.args_rows = args_rows;
+    // one view runs the single-view kernels
+    if (views == 1) CUDA_CHECK(hnb::launch_batch_cull(a, fast, uint32_t(c->sm_count), c->stream));
+    else CUDA_CHECK(hnb::launch_batch_cull_views(v, fast, uint32_t(c->sm_count), c->stream));
+    c->launches += HNB_BATCH_CULL_LAUNCHES;
+}
+
 int32_t hnb_batch_cull(hnb_ctx* c, const hnb_batch_launch* b, const float* d_frusta, uint32_t frustum_rows, const uint32_t* d_src,
                        uint32_t src_rows, uint32_t* d_visible, uint32_t visible_rows, hnb_draw_indexed_indirect_args* d_args,
                        uint32_t args_rows) {
     return guarded([&] {
-        const std::string w = "hnb_batch_cull";
-        // a ribbon effect is refused before anything else about it is checked
-        if (b && (get_effect(c, b->effect).flags & HNB_EFFECT_RIBBONS))
-            fail(HNB_ERR_INVALID_ARG, w + ": a ribbon effect cannot be culled per particle, its ribbons would be re-linked");
-        const BatchPosition bp = check_batch_position(c, b, w);
-        const hnb_batch_info& bi = *bp.batch;
-        const size_t rows = bp.slab->capacity, inst = bi.prefix_sum_count;
-        if (!d_frusta || ((uintptr_t)d_frusta & 15u)) fail(HNB_ERR_INVALID_ARG, w + ": d_frusta is NULL or not 16-byte aligned");
-        if (frustum_rows < inst) fail(HNB_ERR_INVALID_ARG, w + ": frustum_rows is below the batch's instance count");
-        if (d_src && src_rows < rows) fail(HNB_ERR_INVALID_ARG, w + ": src_rows is below the slab's capacity");
-        if (!d_visible) fail(HNB_ERR_INVALID_ARG, w + ": d_visible is NULL");
-        if (visible_rows < rows) fail(HNB_ERR_INVALID_ARG, w + ": visible_rows is below the slab's capacity");
-        if (d_src && (uintptr_t)d_src < (uintptr_t)(d_visible + visible_rows) && (uintptr_t)d_visible < (uintptr_t)(d_src + src_rows))
-            fail(HNB_ERR_INVALID_ARG, w + ": d_src and d_visible overlap");
-        if (!d_args || ((uintptr_t)d_args & 3u)) fail(HNB_ERR_INVALID_ARG, w + ": d_args is NULL or not 4-byte aligned");
-        if (args_rows < inst) fail(HNB_ERR_INVALID_ARG, w + ": args_rows is below the batch's instance count");
-        if (inst == 0) return;
-        if (c->d_metadata.size() == 0) fail(HNB_ERR_INVALID_ARG, w + ": no metadata row was inserted");
-        if (c->d_draw_args.size() == 0) fail(HNB_ERR_INVALID_ARG, w + ": no draw-args row was inserted");
-        CUDA_CHECK(cudaSetDevice(c->device));
-        // scratch: a mask and a prefix word per tile, 8 words per instance, the tile count
-        const size_t max_tiles = hnb::depth_order_max_tiles(bp.slab->capacity, bi.prefix_sum_count);
-        const size_t words = (HNB_BATCH_CULL_MASK_WORDS + 1) * max_tiles + 8 * inst + 1;
-        if (c->d_cull_scratch.size() < words) CUDA_CHECK(grow(c->d_cull_scratch, words, 0, c->stream));
+        batch_cull(c, b, "hnb_batch_cull", 1, d_frusta, frustum_rows, d_src, src_rows, d_visible, visible_rows, d_args, args_rows);
+    });
+}
 
-        bool fast = false;
-        hnb::CullArgs a{};
-        a.src = batch_position_args(c, b, bp, &fast);
-        a.frusta = d_frusta;
-        a.src_list = d_src;
-        a.visible = d_visible;
-        a.args = reinterpret_cast<uint32_t*>(d_args);
-        a.draw_args = c->draw_args();
-        a.num_draw_args = uint32_t(c->d_draw_args.size());
-        a.mask = c->d_cull_scratch.get();
-        a.prefix = a.mask + HNB_BATCH_CULL_MASK_WORDS * max_tiles;
-        a.info = a.prefix + max_tiles;
-        a.total_tiles = a.info + 8 * inst;
-        a.max_tiles = uint32_t(max_tiles);
-        CUDA_CHECK(hnb::launch_batch_cull(a, fast, uint32_t(c->sm_count), c->stream));
-        c->launches += HNB_BATCH_CULL_LAUNCHES;
+int32_t hnb_batch_cull_views(hnb_ctx* c, const hnb_batch_launch* b, uint32_t views, const float* d_frusta, uint32_t frustum_rows,
+                             const uint32_t* d_src, uint32_t src_rows, uint32_t* d_visible, uint32_t visible_rows,
+                             hnb_draw_indexed_indirect_args* d_args, uint32_t args_rows) {
+    return guarded([&] {
+        batch_cull(c, b, "hnb_batch_cull_views", views, d_frusta, frustum_rows, d_src, src_rows, d_visible, visible_rows, d_args,
+                   args_rows);
     });
 }
 

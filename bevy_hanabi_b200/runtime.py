@@ -400,6 +400,16 @@ class Context:
         check(lib.hnb_batch_cull(self._h, C.byref(launch), d_frusta, frustum_rows, d_src, src_rows, d_visible, visible_rows,
                                  d_args, args_rows))
 
+    def batch_cull_views(self, launch: BatchLaunch, views: int, d_frusta: int, frustum_rows: int, d_src: int, src_rows: int,
+                         d_visible: int, visible_rows: int, d_args: int, args_rows: int) -> None:
+        """batch_cull for `views` (1 .. HNB_CULL_MAX_VIEWS) cameras in one call, which reads each particle's source entry
+        and position once. Every buffer but d_src holds the views stacked view-major: view v's frustum for instance j is
+        d_frusta[24 * (v * frustum_rows + j):+24], its entries go to d_visible[v * visible_rows + first + k] and its args
+        row to d_args[v * args_rows + j]. View v's output is byte for byte what batch_cull writes with those slices; the
+        source (the alive list, or d_src) is shared by every view. Only enqueues work (hnb_batch_cull_views)."""
+        check(lib.hnb_batch_cull_views(self._h, C.byref(launch), views, d_frusta, frustum_rows, d_src, src_rows, d_visible,
+                                       visible_rows, d_args, args_rows))
+
     def download_bounds(self, d_out: int, rows: int) -> np.ndarray:
         """Wait for the context stream and return `rows` records batch_bounds wrote to device memory, as BOUNDS_DTYPE."""
         return self.device_download(d_out, rows * BOUNDS_DTYPE.itemsize).view(BOUNDS_DTYPE)

@@ -758,6 +758,41 @@ HNB_API int32_t hnb_batch_cull(hnb_ctx* ctx, const hnb_batch_launch* batch, cons
                                const uint32_t* d_src, uint32_t src_rows, uint32_t* d_visible, uint32_t visible_rows,
                                hnb_draw_indexed_indirect_args* d_args, uint32_t args_rows);
 
+/**
+ * hnb_batch_cull for `views` cameras at once (split-screen, an editor viewport beside the game view, two eyes, a minimap
+ * or a reflection camera), in one call that reads each live particle's source entry and `position` once for all views.
+ *
+ * Each buffer holds the views stacked view-major. For view v < views and the batch's j-th instance:
+ *   - its frustum is d_frusta[24 * (v * frustum_rows + j) .. +23];
+ *   - its visible entries go to d_visible + v * visible_rows, indexed by slab row as in hnb_batch_cull;
+ *   - its draw-args row goes to d_args[v * args_rows + j].
+ * The source entries are shared by every view: the alive list when d_src is NULL, d_src otherwise. View v's output is
+ * byte for byte what
+ *   hnb_batch_cull(ctx, batch, d_frusta + 24*v*frustum_rows, frustum_rows, d_src, src_rows,
+ *                  d_visible + v*visible_rows, visible_rows, d_args + v*args_rows, args_rows)
+ * writes: the same live set, clamping, plane test, source order, and every other row left unwritten. A renderer binds view
+ * v's slice of d_visible in place of the alive-list column and draws with view v's args rows; it picks visible_rows >= the
+ * slab's capacity such that the byte offset 4 * v * visible_rows meets its graphics API's storage-buffer offset alignment.
+ *
+ * One source serves all views, so a blended effect, which needs its own back-to-front order per view, still takes one
+ * hnb_batch_depth_order and one hnb_batch_cull per view.
+ *
+ * Work is only enqueued on the context stream: HNB_BATCH_CULL_LAUNCHES = 4 launches whatever `views` is, no
+ * synchronisation, and no allocation once the context's cull scratch (views * 516 bytes per 4096 live rows and 32 bytes
+ * per instance) has grown to the largest call seen. d_frusta, d_src, d_visible and d_args may be device memory or pinned
+ * host memory (hnb_host_alloc).
+ *
+ * HNB_ERR_INVALID_ARG, with nothing enqueued: every refusal of hnb_batch_cull, checked over the whole stacked ranges
+ * (HNB_EFFECT_RIBBONS effects included); `views` 0 or above HNB_CULL_MAX_VIEWS; [d_src, d_src + src_rows) overlapping
+ * [d_visible, d_visible + views * visible_rows). A batch of zero instances is a no-op. Whatever the device tables hold, no
+ * access leaves the slab, d_frusta[0, 24 * views * frustum_rows), d_src[0, src_rows), d_visible[0, views * visible_rows)
+ * or d_args[0, views * args_rows).
+ */
+#define HNB_CULL_MAX_VIEWS 8
+HNB_API int32_t hnb_batch_cull_views(hnb_ctx* ctx, const hnb_batch_launch* batch, uint32_t views, const float* d_frusta,
+                                     uint32_t frustum_rows, const uint32_t* d_src, uint32_t src_rows, uint32_t* d_visible,
+                                     uint32_t visible_rows, hnb_draw_indexed_indirect_args* d_args, uint32_t args_rows);
+
 /* Individual passes, as exercised one by one by the reference's shader contract tests
  * (src/render/shader_contract_tests.rs). They run the un-fused kernels. */
 HNB_API int32_t hnb_pass_init(hnb_ctx* ctx, const hnb_batch_launch* batch);

@@ -651,19 +651,11 @@ def _timed_cull(label, ctx, launch, instances, rows, alive, claimed, frustum, bo
     _timed_bounds(f"{label} (beside cull)", ctx, launch, instances, bounds_bytes)
 
 
-def cull():
-    """hnb_batch_cull: the filled 64 Mi C5 instance under its claim with about half and with about 0.1 % of it visible,
-    the same size spawned by one init burst, C4's topology in one call, the 16 Mi-slot churn steady state and single
-    instances of 4 Ki and 16 Ki (latency); each beside hnb_batch_bounds of the same batch, and a 2 GiB device-to-device
-    copy for scale."""
-    _card()
-    a = torch.empty(2 << 30, dtype=torch.uint8, device="cuda")
-    b = torch.empty_like(a)
-    ms = _events_ms(lambda: b.copy_(a))
-    report("cull: 2 GiB device-to-device copy", ms, 2 * a.numel(), "torch copy_ (reads 2 GiB and writes 2 GiB), best of 5")
-    del a, b
-    torch.cuda.empty_cache()
-
+def _cull_worlds(small_caps):
+    """The cull cases, one at a time: (label, ctx, launch, instances, rows, alive, claimed, bounds_bytes, filled) for the
+    filled 64 Mi C5 instance under its claim, the same size spawned by one init burst, C4's topology in one call, single
+    instances of each of `small_caps` (latency) and the 16 Mi-slot churn steady state. Each context is closed after its
+    case."""
     P = 64 << 20
     ctx = hb.Context(0, stream.cuda_stream)
     effect = ctx.effect_compile(recipes.c5_lowered())
@@ -672,8 +664,7 @@ def cull():
     single_instance(ctx, P, 32, alive=P)
     la = N.BatchLaunch.make(effect, slab, 0, 0)
     ctx.simulate([la])
-    _timed_cull("C5 64Mi filled, claim, ~half visible", ctx, la, 1, P, P, True, CULL_HALF, 16 * P)
-    _timed_cull("C5 64Mi filled, claim, ~0.1 % visible", ctx, la, 1, P, P, True, CULL_FEW, 16 * P)
+    yield "C5 64Mi filled, claim", ctx, la, 1, P, P, True, 16 * P, True
     ctx.slab_destroy(slab)
     slab = ctx.slab_create(P, 32)
     single_instance(ctx, P, 32, alive=0, spawn=P)
@@ -681,7 +672,7 @@ def cull():
     ctx.upload_spawners([R.make_spawner(spawn=0, seed=43)])
     la = N.BatchLaunch.make(effect, slab, 0, 0)
     ctx.simulate([la])
-    _timed_cull("C5 64Mi from one init burst, no claim", ctx, la, 1, P, P, False, CULL_HALF, 20 * P)
+    yield "C5 64Mi from one init burst, no claim", ctx, la, 1, P, P, False, 20 * P, False
     ctx.close()
     torch.cuda.empty_cache()
 
@@ -702,26 +693,99 @@ def cull():
     ctx.set_sim_params(1 / 60, 0.0, n_inst)
     la = N.BatchLaunch.make(effect, slab, 0, 0)
     ctx.simulate([la])
-    _timed_cull("C4 shape: 1024 x 65536 in one batch", ctx, la, n_inst, n_inst * cap, n_inst * cap, False, CULL_HALF,
-                20 * n_inst * cap - 4 * cap)
+    yield "C4 shape: 1024 x 65536 in one batch", ctx, la, n_inst, n_inst * cap, n_inst * cap, False, 20 * n_inst * cap - 4 * cap, False
     ctx.close()
     torch.cuda.empty_cache()
 
-    for cap in (4096, 16 << 10):
+    for cap in small_caps:
         ctx = hb.Context(0, stream.cuda_stream)
         slab = ctx.slab_create(cap, 32)
         ctx.slab_fill_c5(slab, 0, cap, 100, 1e9, 1e9)
         single_instance(ctx, cap, 32, alive=cap)
         la = N.BatchLaunch.make(ctx.effect_compile(recipes.c5_lowered()), slab, 0, 0)
         ctx.simulate([la])
-        _timed_cull(f"one instance of {cap >> 10} Ki particles (latency)", ctx, la, 1, cap, cap, True, CULL_HALF, 16 * cap)
+        yield f"one instance of {cap >> 10} Ki particles (latency)", ctx, la, 1, cap, cap, True, 16 * cap, False
         ctx.close()
 
     P, ctx, slab, effect, stride, dt, rate = _churned()
     alive = ctx.read_metadata(0).alive_count
-    _timed_cull(f"churned {P >> 20} Mi slots, {alive >> 10} Ki alive, permuted list", ctx, N.BatchLaunch.make(effect, slab, 0, rate), 1, P,
-                alive, False, CULL_HALF, 20 * alive)
+    yield (f"churned {P >> 20} Mi slots, {alive >> 10} Ki alive, permuted list", ctx, N.BatchLaunch.make(effect, slab, 0, rate), 1, P,
+           alive, False, 20 * alive, False)
     ctx.close()
+
+
+def _copy_for_scale(name):
+    a = torch.empty(2 << 30, dtype=torch.uint8, device="cuda")
+    b = torch.empty_like(a)
+    ms = _events_ms(lambda: b.copy_(a))
+    report(f"{name}: 2 GiB device-to-device copy", ms, 2 * a.numel(), "torch copy_ (reads 2 GiB and writes 2 GiB), best of 5")
+    del a, b
+    torch.cuda.empty_cache()
+
+
+def cull():
+    """hnb_batch_cull: the filled 64 Mi C5 instance under its claim with about half and with about 0.1 % of it visible,
+    the same size spawned by one init burst, C4's topology in one call, the 16 Mi-slot churn steady state and single
+    instances of 4 Ki and 16 Ki (latency); each beside hnb_batch_bounds of the same batch, and a 2 GiB device-to-device
+    copy for scale."""
+    _card()
+    _copy_for_scale("cull")
+    for label, ctx, la, instances, rows, alive, claimed, bounds_bytes, filled in _cull_worlds((4096, 16 << 10)):
+        if filled:
+            _timed_cull(f"{label}, ~half visible", ctx, la, instances, rows, alive, claimed, CULL_HALF, bounds_bytes)
+            _timed_cull(f"{label}, ~0.1 % visible", ctx, la, instances, rows, alive, claimed, CULL_FEW, bounds_bytes)
+        else:
+            _timed_cull(label, ctx, la, instances, rows, alive, claimed, CULL_HALF, bounds_bytes)
+
+
+def view_frusta(views):
+    """One frustum per view, each keeping about half of a cloud around the origin from a different direction: the half
+    space n_v . p >= 0, with n_v turning around the y axis and tilting up and down, inside a box of half-width 2. (views,
+    6, 4) float32."""
+    out = []
+    for v in range(views):
+        t = 2 * np.pi * v / max(views, 1)
+        n = np.array([np.cos(t), 0.3 * (-1) ** v, np.sin(t)])
+        n /= np.linalg.norm(n)
+        out.append([[*n, 0.0]] + CULL_HALF[1:])
+    return np.array(out, dtype=np.float32)
+
+
+def _timed_cull_views(label, ctx, launch, instances, rows, alive, claimed):
+    """hnb_batch_cull_views of `launch`'s batch (alive-list source) at 1, 2, 4 and 8 views, beside as many hnb_batch_cull
+    calls over the same stacked buffers: one warm-up each, then the best of 5 CUDA-event windows for each. GB/s counts
+    what one multi-view call must move: 16 B of position (and 4 B of list where no claim covers the row) read per live
+    particle once, and 4 B written per visible entry of each view."""
+    vr = (rows + 63) // 64 * 64  # each view's slice 256-byte aligned
+    visible = torch.empty(8 * vr, dtype=torch.int32, device="cuda")
+    args = torch.empty(8 * 5 * instances, dtype=torch.int32, device="cuda")
+    for views in (1, 2, 4, 8):
+        frusta = torch.tensor(np.repeat(view_frusta(views)[:, None], instances, axis=1), device="cuda")
+        fp, vp, ap = frusta.data_ptr(), visible.data_ptr(), args.data_ptr()
+        one = lambda: ctx.batch_cull_views(launch, views, fp, instances, 0, 0, vp, vr, ap, instances)  # noqa: E731
+
+        def separate():
+            for v in range(views):
+                ctx.batch_cull(launch, fp + 96 * v * instances, instances, 0, 0, vp + 4 * v * vr, vr, ap + 20 * v * instances, instances)
+        one()
+        ms_one = _events_ms(one)
+        m = [int(x) for x in args.view(8, -1, 5)[:views, :, 1].sum(dim=1).tolist()]
+        separate()
+        ms_sep = _events_ms(separate)
+        read = (16 if claimed else 20) * alive
+        report(f"cull_views: {label}, V={views}", ms_one, read + 4 * sum(m),
+               f"{ms_one * 1e3:.1f} us per call; {views} x cull: {ms_sep:.4f} ms ({ms_sep / ms_one:.2f}x); "
+               f"visible per view {', '.join(f'{100 * x / max(alive, 1):.0f} %' for x in m)}; best of 5")
+
+
+def cull_views():
+    """hnb_batch_cull_views at 1, 2, 4 and 8 views, each view seeing about half of the cloud from another direction,
+    beside as many hnb_batch_cull calls, on the cull cases: the filled 64 Mi C5 instance under its claim, the same size
+    from one init burst, C4's topology in one call, the 16 Mi-slot churn steady state and one 4 Ki instance."""
+    _card()
+    _copy_for_scale("cull_views")
+    for label, ctx, la, instances, rows, alive, claimed, _, _ in _cull_worlds((4096,)):
+        _timed_cull_views(label, ctx, la, instances, rows, alive, claimed)
 
 
 class _DeviceColumn:
@@ -973,7 +1037,7 @@ def emitter_relocation():
     ctx.close()
 
 
-SCENARIOS = {"cull": cull, "c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "bounds": bounds, "depth_order": depth_order, "emitter_relocation": emitter_relocation, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
+SCENARIOS = {"cull": cull, "cull_views": cull_views, "c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "bounds": bounds, "depth_order": depth_order, "emitter_relocation": emitter_relocation, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
 if __name__ == "__main__":
     for name in (sys.argv[1:] or list(SCENARIOS)):
         try:
