@@ -710,9 +710,11 @@ extern "C" __global__ void __launch_bounds__(HNB_BLOCK, HNB_MIN_BLOCKS) hnb_upda
         // changed, deaths elsewhere that made the list a gather): there each row reads its group's word next to its record
         // loads, takes the deferred age, stores its age as usual, and counts itself in the word (below).
         // Reading every row's word made the churned update 3.4 % slower on the H100 where nothing was deferred: the slab's
-        // count of deferred words (hnb_deferred_groups) gates it.
+        // count of deferred words (hnb_deferred_groups) gates it. Other warps change the count while this one reads it, so
+        // lanes may read different values: the ballot makes the gate warp-uniform (the ballots under it need every lane),
+        // and a lane that read 0 still reads its group's word when another lane of the warp saw a deferred one.
         const bool tile_defer_rows = !tile_ages && P.defer_ages != 0u && P.group_age != nullptr &&
-                                     *hnb_deferred_groups(P.group_age, P.slab.capacity_rows) != 0ull;  // warp-uniform
+                                     __ballot_sync(0xffffffffu, *hnb_deferred_groups(P.group_age, P.slab.capacity_rows) != 0ull) != 0u;
 #endif
 #if HNB_GROUP_AGE
         // Two copies of the sub-tile loop: copy 0 for floor tiles that keep common ages (`ages` true, `defer_rows` false),

@@ -444,6 +444,16 @@ void clear_life_floors(hnb_ctx* c, Slab& s, uint32_t first, uint32_t count) {
 }
 void clear_life_floors(hnb_ctx* c, Slab& s) { clear_life_floors(c, s, 0, s.capacity); }
 
+// clear_life_floors for writers of alive lists and dead stacks at positions [first, first + count): their entries name rows
+// anywhere in an instance's slice, not the rows at those positions. A row of a deferred group that such a write moves to the
+// dead stack breaks the invariant that every row of the group is alive, and no later update would walk all 32 rows of it
+// (DESIGN.md §3). So a slab that may hold deferred words is flushed and cleared whole.
+void clear_list_groups(hnb_ctx* c, Slab& s, uint32_t first, uint32_t count) {
+    if (count == 0) return;
+    if (s.defers) clear_life_floors(c, s);
+    else clear_life_floors(c, s, first, count);
+}
+
 // AoS records <-> columns go through a device staging buffer in chunks of this size.
 constexpr size_t kChunkBytes = size_t(64) << 20;
 
@@ -1093,7 +1103,7 @@ int32_t hnb_slab_rebuild_alive_bits(hnb_ctx* c, hnb_slab h, uint32_t first, uint
         Slab& s = get_slab(c, h);
         check_rows(s, first, rows);
         if (column > 1 || alive_count > rows) fail(HNB_ERR_INVALID_ARG, "bad alive-list column or count");
-        clear_life_floors(c, s, first, rows);  // slots may become alive whose lifetimes no floor covers
+        clear_list_groups(c, s, first, rows);  // slots may become alive whose lifetimes no floor covers
         CUDA_CHECK(hnb::launch_bits_range(s.alive_bits.get(), first, rows, false, c->stream));
         CUDA_CHECK(hnb::launch_bits_from_list(s.alive_bits.get(), (column ? s.pong : s.ping).get() + first, first, alive_count, c->stream));
         c->launches += rows ? 1 + (alive_count ? 1 : 0) : 0;
@@ -1149,7 +1159,7 @@ int32_t hnb_slab_upload_indirect(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_
         CUDA_CHECK(stage.alloc(size_t(count) * 3));
         CUDA_CHECK(cudaMemcpyAsync(stage.get(), rows, size_t(count) * 12, cudaMemcpyHostToDevice, c->stream));
         clear_ident_claims(c, s);
-        clear_life_floors(c, s, first, count);
+        clear_list_groups(c, s, first, count);
         CUDA_CHECK(hnb::launch_indirect_deinterleave(stage.get(), s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
         c->launches++;
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
@@ -1211,7 +1221,7 @@ int32_t hnb_slab_import_indirect_device(hnb_ctx* c, hnb_slab h, uint32_t first, 
         check_rows(s, first, count);
         if (count && !d_src) fail(HNB_ERR_INVALID_ARG, "d_src is NULL");
         clear_ident_claims(c, s);
-        clear_life_floors(c, s, first, count);
+        clear_list_groups(c, s, first, count);
         CUDA_CHECK(hnb::launch_indirect_deinterleave((const uint32_t*)d_src, s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
         c->launches += count ? 1 : 0;
     });
@@ -2283,6 +2293,14 @@ int32_t hnb_read_tile_size(hnb_ctx* c, uint32_t row, uint32_t* out) {
         if (!out) fail(HNB_ERR_INVALID_ARG, "NULL argument");
         if (row >= c->B) fail(HNB_ERR_OUT_OF_RANGE, "batch row out of range");
         *out = c->h_at<uint32_t>(c->lay.off_tile_size)[row];  // host copy of the word bind_launch passed to the batch's last launch
+    });
+}
+int32_t hnb_slab_deferred_groups(hnb_ctx* c, hnb_slab h, uint64_t* out) {
+    return guarded([&] {
+        if (!out) fail(HNB_ERR_INVALID_ARG, "NULL argument");
+        const Slab& s = get_slab(c, h);
+        // a plain read of the count word after the stream's work: nothing is flushed, so the words stay as the updates left them
+        read_back(c, out, hnb::hnb_deferred_groups(s.group_age.get(), s.capacity), sizeof(uint64_t));
     });
 }
 

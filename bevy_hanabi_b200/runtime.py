@@ -646,3 +646,9 @@ class Context:
         w = N.u32()
         check(lib.hnb_read_tile_size(self._h, row, C.byref(w)))
         return w.value & 0xFFFF
+
+    def slab_deferred_groups(self, slab: int) -> int:
+        """Groups of `slab` whose common age is deferred, after the stream's work; flushes nothing (hnb_slab_deferred_groups)."""
+        n = C.c_uint64(0)
+        check(lib.hnb_slab_deferred_groups(self._h, slab, C.byref(n)))
+        return n.value

@@ -818,6 +818,10 @@ HNB_API int32_t hnb_read_dispatch_args(hnb_ctx* ctx, uint32_t row, hnb_dispatch_
 /** Tile size word of batch `row` as its last update launch used it (0 before the first launch): rows per update tile
  *  (low 16 bits: 32 x K rows per sub-tile x the sub-tile count, see HNB_TILE_CHUNKS) | 0x80000000 for HNB_EFFECT_SLOT_ORDER. */
 HNB_API int32_t hnb_read_tile_size(hnb_ctx* ctx, uint32_t row, uint32_t* out);
+/** Number of the slab's 32-row groups whose common age is deferred (section 3 of DESIGN.md: the age lives in the group's
+ *  word and the age column of its rows is stale), after the context stream's work so far: 0 for a slab that never ran a
+ *  deferring update. Waits for the stream; flushes nothing and changes nothing. */
+HNB_API int32_t hnb_slab_deferred_groups(hnb_ctx* ctx, hnb_slab slab, uint64_t* out);
 /** Enqueue an async copy of draw-args rows [first,first+count) into caller PINNED memory. */
 HNB_API int32_t hnb_read_draw_args_async(hnb_ctx* ctx, uint32_t first, uint32_t count,
                                          hnb_draw_indexed_indirect_args* pinned_out);
