@@ -87,7 +87,7 @@ def load() -> C.CDLL:
                                u32, vp, vp]
     lib.orc_init.restype = None
     lib.orc_init.argtypes = [P(SimParams), vp, u32, vp, P(Spawner), P(u32), P(BatchInfo), P(EffectMetadata), u32, vp, vp]
-    for n in ("orc_body_update_noop", "orc_body_update_c5", "orc_body_init_const"):
+    for n in ("orc_body_update_noop", "orc_body_update_c5", "orc_body_init_const", "orc_body_init_sparks"):
         getattr(lib, n).restype = vp
         getattr(lib, n).argtypes = []
     lib.orc_fill_c5.restype = None
@@ -102,6 +102,8 @@ def load() -> C.CDLL:
     lib.orc_indirect_reset.argtypes = [vp, u32, u32]
     lib.orc_checksum_ex.restype = C.c_uint64
     lib.orc_checksum_ex.argtypes = [vp, u32, u32, u32, C.c_uint64]
+    lib.orc_row_digests.restype = None
+    lib.orc_row_digests.argtypes = [vp, u32, u32, vp]
     lib.orc_set_threads.restype = None
     lib.orc_set_threads.argtypes = [C.c_int]
     lib.orc_max_threads.restype = C.c_int

@@ -332,6 +332,9 @@ ORC_API void orc_init(const orc_sim_params* sim_params, uint32_t* particle_buffe
         uint32_t spawn_count = (uint32_t)spawner->spawn;
         if (location.update_index >= spawn_count) continue;
         uint32_t alive_index = em->alive_count++;
+        /* the slot of the thread 16 ahead, which spawns too: its dead-stack entry is read and its record written soon */
+        if (location.update_index + 16u < max_spawn && location.update_index + 16u < spawn_count)
+            __builtin_prefetch(particle_buffer + (size_t)indirect_buffer[base_particle + alive_index + 16u].dead_index * stride_words, 1);
         uint32_t slab_particle_dead_index = indirect_buffer[base_particle + alive_index].dead_index;
         uint32_t particle_index = slab_particle_dead_index - base_particle;
         uint32_t particle_counter = em->particle_counter++;
@@ -392,6 +395,25 @@ static void body_init_const(uint32_t* particle, orc_thread* t) {
     memcpy(particle, ci->words, (size_t)ci->stride_words * 4);
 }
 ORC_API orc_init_body orc_body_init_const(void) { return body_init_const; }
+
+/* tests/effects.py::drifting_sparks' init, in the generated code's order of PRNG calls: position = frand3() * 2 - 1,
+ * velocity = frand3() * 2 - 1, age = 0, lifetime = lo + frand() * (hi - lo), then the Global simulation space's
+ * position += the spawner's translation. Same record layout as C5, so its update is body_update_c5 with ACCEL_DRAG.
+ * user -> float[2] {lifetime_lo, lifetime_hi}. */
+static void body_init_sparks(uint32_t* particle, orc_thread* t) {
+    const float* life = (const float*)t->user;
+    const float* tr = t->spawner->transform;
+    float* p = (float*)particle;
+    float r[3];
+    orc_frand3(t->seed, r);
+    p[0] = r[0] * 2.0f - 1.0f; p[1] = r[1] * 2.0f - 1.0f; p[2] = r[2] * 2.0f - 1.0f;
+    orc_frand3(t->seed, r);
+    p[4] = r[0] * 2.0f - 1.0f; p[5] = r[1] * 2.0f - 1.0f; p[6] = r[2] * 2.0f - 1.0f;
+    p[3] = 0.0f;
+    p[7] = life[0] + orc_frand(t->seed) * (life[1] - life[0]);
+    p[0] = p[0] + tr[3]; p[1] = p[1] + tr[7]; p[2] = p[2] + tr[11];
+}
+ORC_API orc_init_body orc_body_init_sparks(void) { return body_init_sparks; }
 
 /* ---- synthetic C5 state, same counter-based generator as hnb_slab_fill_c5 ---------------------- */
 /* `logical_first`: row of the LOGICAL instance that slab row `first` holds. A shard of an instance split by index range
@@ -463,6 +485,8 @@ ORC_API uint32_t orc_update_c5_parallel(const orc_sim_params* sim_params, uint32
         uint64_t lo = (uint64_t)max_update * tid / nt, hi = (uint64_t)max_update * (tid + 1) / nt;
         uint32_t alive = 0;
         for (uint64_t row = lo; row < hi; ++row) {
+            if (row + 16 < hi) /* a churned list is a gather: keep later records in flight (speed only) */
+                __builtin_prefetch(particle_buffer + (size_t)(base_particle + indirect_buffer[base_particle + row + 16].particle_index[read_index]) * 8, 1);
             uint32_t particle_index = indirect_buffer[base_particle + row].particle_index[read_index];
             float* p = particle_buffer + (size_t)(base_particle + particle_index) * 8;
             float rec[8];
@@ -515,6 +539,19 @@ ORC_API uint64_t orc_checksum_ex(const uint32_t* words, uint32_t first, uint32_t
         acc += h;
     }
     return acc;
+}
+
+/* The high 32 bits of each row's term of orc_checksum_ex (index_base 0): a digest per row, so that two slabs whose
+ * checksums differ can be told apart row by row without keeping either. */
+ORC_API void orc_row_digests(const uint32_t* words, uint32_t count, uint32_t stride_words, uint32_t* out) {
+#pragma omp parallel for schedule(static)
+    for (int64_t i = 0; i < (int64_t)count; ++i) {
+        uint64_t h = 0xcbf29ce484222325ull ^ (uint64_t)i;
+        const uint32_t* row = words + (size_t)i * stride_words;
+        for (uint32_t w = 0; w < stride_words; ++w) h = (h ^ (uint64_t)row[w]) * 0x100000001b3ull;
+        h ^= h >> 29; h *= 0xbf58476d1ce4e5b9ull; h ^= h >> 32;
+        out[i] = (uint32_t)(h >> 32);
+    }
 }
 
 ORC_API uint64_t orc_checksum(const uint32_t* words, uint32_t first, uint32_t count, uint32_t stride_words) {

@@ -235,6 +235,11 @@ def c5_init():
     return ci
 
 
+def sparks_init(lifetime=(0.2, 0.9)):
+    """The user struct of the C oracle's drifting_sparks init (orc_body_init_sparks): {lifetime_lo, lifetime_hi}."""
+    return (C.c_float * 2)(*lifetime)
+
+
 def fill_c5(ref, rng, life_lo, life_hi):
     """C5 records of the initially alive rows of every instance: random positions and velocities, age 0, lifetimes in
     [life_lo, life_hi)."""

@@ -57,6 +57,18 @@ def at_tile_sizes(argnames, values, ids=None, forced_values=()):
     return pytest.mark.parametrize(["tiled_ctx"] + names, params, indirect=["tiled_ctx"])
 
 
+def sorted_slots(entries: np.ndarray, capacity: int) -> np.ndarray:
+    """np.sort(entries) for an alive list: distinct slots below `capacity`, in O(capacity) through a presence mask. A list
+    that is not such a set (a test may hand one in) is sorted by np.sort."""
+    if len(entries) and int(entries.max()) < capacity:
+        mask = np.zeros(capacity, dtype=bool)
+        mask[entries] = True
+        out = np.flatnonzero(mask).astype(np.uint32)
+        if len(out) == len(entries):
+            return out
+    return np.sort(entries)
+
+
 @dataclass
 class Instance:
     slab_offset: int
@@ -68,6 +80,11 @@ class Instance:
 
 class RefWorld:
     """Oracle-side state of one slab in reference layouts (AoS particles, interleaved indirect rows)."""
+
+    # C5 bodies only (records of 8 words): oracle_update runs orc_update_c5_parallel once per instance of the batch, in batch
+    # order, on `parallel_c5` threads, instead of the serial orc_update (same results: test_churn_oracle_cpu.py). A class
+    # default, so that tables built without __init__ (object.__new__) have it too.
+    parallel_c5 = 0
 
     def __init__(self, slab_rows: int, stride_words: int, instances: Sequence[Instance], batches: Sequence[Sequence[int]] | None = None,
                  dt: float = 1.0 / 60.0):
@@ -173,7 +190,7 @@ class RefWorld:
             md, sp = self.metadata[i], self.spawners[i]
             col, base, n = 1 - md.indirect_write_index, sp.slab_offset, md.max_update
             saved.append((col, base, n, self.indirect[base:base + n, col].copy()))
-            self.indirect[base:base + n, col] = np.sort(self.indirect[base:base + n, col])
+            self.indirect[base:base + n, col] = sorted_slots(self.indirect[base:base + n, col], md.capacity)
         return saved
 
     def restore_read_lists(self, saved):
@@ -189,6 +206,15 @@ class RefWorld:
             finally:
                 self.slot_order = True
                 self.restore_read_lists(saved)
+            return
+        if self.parallel_c5:
+            u32p = C.POINTER(C.c_uint32)
+            for i in self.batches[b]:
+                md = self.metadata[i]
+                flags = np.empty(max(md.max_update, 1), dtype=np.uint8)
+                orc.orc_update_c5_parallel(C.byref(self.sim), self.draw.ctypes.data_as(u32p), O.ptr(self.particles),
+                                           O.ptr(self.indirect), C.byref(self.spawners[i]), C.byref(md),
+                                           C.cast(user, C.POINTER(C.c_float)), O.ptr(flags), self.parallel_c5)
             return
         threads = int(self.dispatch[3 * b]) * 64  # indirect dispatch: x workgroups of 64 threads
         orc.orc_update(C.byref(self.sim), self.draw.ctypes.data_as(C.POINTER(C.c_uint32)), O.ptr(self.particles),

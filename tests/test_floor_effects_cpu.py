@@ -56,7 +56,7 @@ def test_every_effect_is_listed():
     """A builder added to tests/effects.py or recipes.py must be entered above."""
     import inspect
     builders = {n for n, f in inspect.getmembers(E, inspect.isfunction) if f.__module__ == E.__name__ and not n.startswith("_")}
-    builders -= {"table_asset", "table_props", "tile_k", "edge_counts", "c5_init", "fill_c5", "exact_expr"}  # not effects
+    builders -= {"table_asset", "table_props", "tile_k", "edge_counts", "c5_init", "sparks_init", "fill_c5", "exact_expr"}  # not effects
     listed = {n.split(".")[0] for n in EXPECTED}
     assert builders <= listed, f"not listed: {sorted(builders - listed)}"
     assert set(E.EFFECTS) - {"trails48", "matrix144"} <= listed  # trails48 and matrix144 are firework_trails and matrix_asset
