@@ -176,6 +176,7 @@ SIGNATURES = {
     "hnb_instance_snapshot_bytes": (C.c_size_t, [u32, u32]),
     "hnb_instance_snapshot": (i32, [vp, u32, u32, u32, u32, u32, vp, C.c_size_t]),
     "hnb_instance_restore": (i32, [vp, u32, u32, u32, u32, u32, vp, C.c_size_t]),
+    "hnb_instance_append": (i32, [vp, u32, u32, u32, u32, u32, vp, C.c_size_t]),
     "hnb_slab_repack_events": (i32, [vp, u32, u32, u32, u32, u32, P(u32)]),
     "hnb_instance_snapshot_events_bytes": (C.c_size_t, [u32, u32, P(u32)]),
     "hnb_instance_snapshot_events": (i32, [vp, u32, u32, u32, u32, u32, P(u32), vp, C.c_size_t]),

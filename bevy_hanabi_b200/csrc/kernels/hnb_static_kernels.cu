@@ -673,6 +673,21 @@ __device__ __forceinline__ RestoreSpan restore_span(const SnapshotArgs& a, const
     return s;
 }
 
+// column p's piece of record r of the snapshot at `src`; `al` = snapshot_align(stride_words, word_off[p])
+template <int W>
+__device__ __forceinline__ void snapshot_piece(const SnapshotArgs& a, u32 p, u32 off, u32 al, const u32* src, u32 r, RepackPiece<W>& v) {
+    const u32* s = src + HNB_SNAPSHOT_HEADER_WORDS + u64(r) * a.stride_words;
+    if (off & HNB_PLANE_WORD_LIST) {  // a word map: each lane from its own record word
+#pragma unroll
+        for (u32 l = 0; l < W; ++l) v.w[l] = s[hnb_plane_word(a.planes, p, l)];
+        return;
+    }
+    s += off;
+    if (W >= 4 && al == 4u) snapshot_load<4>(s, v);
+    else if (W >= 2 && al >= 2u) snapshot_load<2>(s, v);
+    else snapshot_load<1>(s, v);
+}
+
 // rows i0 + k * RP_THREADS < m + dm of column p from records i (i < m) and n + i - m (the dead records)
 template <int W>
 __device__ __forceinline__ void restore_column(const SnapshotArgs& a, u32 p, u32 i0, u32 m, u32 dm, u32 n, const u32* src) {
@@ -683,17 +698,7 @@ __device__ __forceinline__ void restore_column(const SnapshotArgs& a, u32 p, u32
     for (u32 k = 0; k < RP_ITEMS; ++k) {
         const u32 i = i0 + k * RP_THREADS;
         if (i >= m + dm) continue;
-        const u32 r = i < m ? i : n + (i - m);
-        const u32* s = src + HNB_SNAPSHOT_HEADER_WORDS + u64(r) * a.stride_words;
-        if (off & HNB_PLANE_WORD_LIST) {  // a word map: each lane from its own record word
-#pragma unroll
-            for (u32 l = 0; l < W; ++l) v[k].w[l] = s[hnb_plane_word(a.planes, p, l)];
-            continue;
-        }
-        s += off;
-        if (W >= 4 && al == 4u) snapshot_load<4>(s, v[k]);
-        else if (W >= 2 && al >= 2u) snapshot_load<2>(s, v[k]);
-        else snapshot_load<1>(s, v[k]);
+        snapshot_piece<W>(a, p, off, al, src, i < m ? i : n + (i - m), v[k]);
     }
 #pragma unroll
     for (u32 k = 0; k < RP_ITEMS; ++k)
@@ -735,6 +740,81 @@ __device__ __forceinline__ void restore_scatter(const SnapshotArgs& a, const u32
 __global__ void __launch_bounds__(RP_THREADS) k_restore_scatter(SnapshotArgs a, const u32* src) { restore_scatter<false>(a, src, 0u); }
 __global__ void __launch_bounds__(RP_THREADS) k_restore_scatter_dead(SnapshotArgs a, const u32* src, u32 channels) {
     restore_scatter<true>(a, src, channels);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Append to one instance (hnb_instance_append): record k < m takes the slot the k-th spawn of an init would take,
+// s_k = dead[first + n + k] - first, with m = min(count, max_spawn, rows - n, records the buffer holds) and n =
+// min(alive_count, rows). The scatter reads n and max_spawn, so the metadata words and the claim cut follow in a second
+// launch (k_append_commit).
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ u32 append_count(const AppendArgs& a, const u32* src, u32 n) {
+    return min(min(restore_count(a.s, src), a.s.metadata->max_spawn), a.s.rows - n);
+}
+
+// records i0 + k * RP_THREADS < m of column p -> local rows slot[k]
+template <int W>
+__device__ __forceinline__ void append_column(const SnapshotArgs& a, u32 p, const u32 (&slot)[RP_ITEMS], u32 i0, u32 m, const u32* src) {
+    RepackPiece<W>* col = (RepackPiece<W>*)a.planes.ptr[p] + a.first;
+    const u32 off = a.planes.word_off[p], al = snapshot_align(a.stride_words, off);
+    RepackPiece<W> v[RP_ITEMS];
+#pragma unroll
+    for (u32 k = 0; k < RP_ITEMS; ++k)
+        if (i0 + k * RP_THREADS < m) snapshot_piece<W>(a, p, off, al, src, i0 + k * RP_THREADS, v[k]);
+#pragma unroll
+    for (u32 k = 0; k < RP_ITEMS; ++k)
+        if (i0 + k * RP_THREADS < m) col[slot[k]] = v[k];
+}
+
+// What the store half of an init does for each appended record (hnb_particle_kernels.cuh, hnb_init): the record in every
+// column, list_W[first + n + k] = s_k, the alive bit (slot order) and the slot's group words the sentinel.
+__global__ void __launch_bounds__(RP_THREADS) k_append_scatter(AppendArgs a, const u32* src) {
+    const EffectMetadata* md = a.s.metadata;
+    const u32 n = min(md->alive_count, a.s.rows);
+    const u32 m = append_count(a, src, n);
+    const u32 i0 = blockIdx.x * RP_ROWS_PER_BLOCK + threadIdx.x;
+    if (i0 >= m) return;
+    const u32 base = a.s.first;
+    u32 slot[RP_ITEMS];
+#pragma unroll
+    for (u32 k = 0; k < RP_ITEMS; ++k) {
+        const u32 i = i0 + k * RP_THREADS;
+        slot[k] = i < m ? min(a.dead[base + n + i] - base, a.s.rows - 1u) : 0u;  // clamped as repack_source
+    }
+    for (u32 p = 0; p < a.s.num_planes; ++p) {
+        switch (a.s.planes.words[p]) {
+        case 1: append_column<1>(a.s, p, slot, i0, m, src); break;
+        case 2: append_column<2>(a.s, p, slot, i0, m, src); break;
+        case 4: append_column<4>(a.s, p, slot, i0, m, src); break;
+        default: append_column<8>(a.s, p, slot, i0, m, src); break;
+        }
+    }
+    u32* list = md->indirect_write_index == 0u ? a.ping : a.pong;
+#pragma unroll
+    for (u32 k = 0; k < RP_ITEMS; ++k) {
+        const u32 i = i0 + k * RP_THREADS;
+        if (i >= m) continue;
+        const u32 row = base + slot[k];
+        list[base + n + i] = slot[k];
+        if (a.alive_bits) atomicOr(&a.alive_bits[row >> 5u], 1u << (row & 31u));
+        // the slot's lifetime and age changed: its group's floor and common age prove nothing until an update stores them
+        a.life_floor[row >> 5u] = HNB_LIFE_FLOOR_NONE;
+        a.group_age[row >> 5u] = HNB_GROUP_AGE_NONE;
+    }
+}
+
+// After the scatter: alive_count = n + m, max_spawn -= m, particle_counter += m, and the identity claim of column W cut to
+// n (the first appended row ends what it can cover). Nothing for m = 0.
+__global__ void k_append_commit(AppendArgs a, const u32* src) {
+    EffectMetadata* md = a.s.metadata;
+    const u32 n = min(md->alive_count, a.s.rows);
+    const u32 m = append_count(a, src, n);
+    if (m == 0u) return;
+    md->alive_count = n + m;
+    md->max_spawn -= m;
+    md->particle_counter += m;
+    u64* const claim = &a.claim[md->indirect_write_index];
+    if (hnb_claim_len(hnb_claim_load(claim), a.s.first) > n) hnb_claim_store(claim, hnb_claim_pack(a.s.first, n));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1893,6 +1973,19 @@ cudaError_t launch_restore_scatter(const SnapshotArgs& a, const u32* src, cudaSt
     if (a.rows == 0) return cudaSuccess;
     if (channels) k_restore_scatter_dead<<<blocks_for(a.rows, RP_ROWS_PER_BLOCK), RP_THREADS, 0, st>>>(a, src, *channels);
     else k_restore_scatter<<<blocks_for(a.rows, RP_ROWS_PER_BLOCK), RP_THREADS, 0, st>>>(a, src);
+    return cudaGetLastError();
+}
+cudaError_t launch_append(const AppendArgs& a, const u32* src, cudaStream_t st, u32* launches) {
+    // m is at most the records the buffer holds and at most rows: no more threads than the smaller of the two
+    const u64 held = (a.s.src_bytes - HNB_SNAPSHOT_HEADER_WORDS * 4u) / (a.s.stride_words * 4u);
+    const u32 bound = u32(held < a.s.rows ? held : a.s.rows);
+    if (bound == 0u) return cudaSuccess;
+    k_append_scatter<<<blocks_for(bound, RP_ROWS_PER_BLOCK), RP_THREADS, 0, st>>>(a, src);
+    ++*launches;
+    cudaError_t err = cudaGetLastError();
+    if (err != cudaSuccess) return err;
+    k_append_commit<<<1, 1, 0, st>>>(a, src);
+    ++*launches;
     return cudaGetLastError();
 }
 cudaError_t launch_repack_inverse(const RepackArgs& a, u32* inv, cudaStream_t st) {

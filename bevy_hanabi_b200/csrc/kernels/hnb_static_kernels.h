@@ -125,6 +125,22 @@ cudaError_t launch_snapshot_gather(const SnapshotArgs& a, u32* dst, cudaStream_t
 // `channels` != NULL: a version-2 snapshot of that many event channels; also the dead records and max_update.
 cudaError_t launch_restore_scatter(const SnapshotArgs& a, const u32* src, cudaStream_t st, const u32* channels = nullptr);
 
+// Append of a version-1 snapshot to one instance (hnb_instance_append): its records go to the slots the next spawns of an
+// init would take. Pointers are the slab's row-0 columns; the group words are indexed by slab row / 32.
+struct AppendArgs {
+    SnapshotArgs s;    // the slice, its planes, its metadata row (read, then written by the commit) and src_bytes
+    u32* ping;         // alive-list columns: entries [first + n, first + n + m) of column W are written
+    u32* pong;
+    const u32* dead;   // dead stack: entries [first + n, first + n + m) name the slots
+    u32* alive_bits;   // NULL unless the effect has HNB_EFFECT_SLOT_ORDER
+    u32* life_floor;   // the slab's lifetime floors and common ages: the written slots' groups become the sentinel
+    u64* group_age;
+    u64* claim;        // [2]: the slab's identity claims; column W's is cut to n
+};
+// The scatter (records, list entries, bits, group words), then one thread for the metadata words and the claim cut.
+// Nothing is launched when src_bytes holds no record; `launches` counts the launches made.
+cudaError_t launch_append(const AppendArgs& a, const u32* src, cudaStream_t st, u32* launches);
+
 // The event buffers an emitting instance appends to (hnb_batch_launch.emit_events), channels b < count. Channel b's
 // pending count is child_infos[metadata->base_child_index + b].event_count (none when that row does not exist).
 #define HNB_SNAPSHOT_EVENTS_VERSION_WORD 2u

@@ -1312,7 +1312,10 @@ void check_instance_slice(hnb_ctx* c, const Slab& s, const Effect& fx, uint32_t 
     if (!emit) {
         if (emits)
             fail(HNB_ERR_INVALID_ARG, w + ": pending GPU spawn events name parent slots; an emitting effect cannot be " +
-                                          (w == "hnb_slab_repack" ? "repacked" : "snapshot or restored") + " without its event buffers");
+                                          (w == "hnb_slab_repack"       ? "repacked"
+                                           : w == "hnb_instance_append" ? "appended to"
+                                                                        : "snapshot or restored") +
+                                          " without its event buffers");
         return;
     }
     if (!emits) fail(HNB_ERR_INVALID_ARG, w + ": the effect does not have HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS");
@@ -1481,6 +1484,40 @@ int32_t instance_restore(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata
         c->launches++;
     });
 }
+
+// hnb_instance_append (two launches: the records, list entries, bits and group words, then the metadata words and the claim
+// cut, which the first reads). No slice-wide flush: the written slots are free, and under the update invariant a free slot
+// never lies in a deferred group, so only the groups of the written slots change (DESIGN.md §4.12).
+int32_t instance_append(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                        const void* d_src, size_t src_bytes) {
+    return guarded([&] {
+        Slab& s = get_slab(c, h);
+        const Effect& fx = get_effect(c, e);
+        const char* what = "hnb_instance_append";
+        const std::string w = what;
+        check_instance_slice(c, s, fx, metadata_row, first, rows, what);
+        if (!d_src || ((uintptr_t)d_src & 15u)) fail(HNB_ERR_INVALID_ARG, w + ": d_src is NULL or not 16-byte aligned");
+        if (src_bytes < sizeof(hnb_instance_snapshot_header)) fail(HNB_ERR_INVALID_ARG, w + ": src_bytes is below the 64-byte header");
+        if (rows == 0) return;
+        CUDA_CHECK(cudaSetDevice(c->device));
+        fix_plan(c, s, fx.plan);
+        s.written = true;
+        hnb::AppendArgs a{};
+        a.s = snapshot_args(c, s, metadata_row, first, rows);
+        a.s.src_bytes = src_bytes;
+        a.ping = s.ping.get();
+        a.pong = s.pong.get();
+        a.dead = s.dead.get();
+        a.alive_bits = (fx.flags & HNB_EFFECT_SLOT_ORDER) ? s.alive_bits.get() : nullptr;
+        a.life_floor = s.life_floor.get();
+        a.group_age = s.group_age.get();
+        a.claim = s.ident_claim.get();
+        uint32_t launches = 0;
+        const cudaError_t err = hnb::launch_append(a, (const uint32_t*)d_src, c->stream, &launches);
+        c->launches += launches;
+        CUDA_CHECK(err);
+    });
+}
 }  // namespace
 
 int32_t hnb_slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows) {
@@ -1524,6 +1561,10 @@ int32_t hnb_instance_restore_events(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32
                                     const hnb_event_buffer emit_events[HNB_MAX_EVENT_BINDINGS], const void* d_src, size_t src_bytes) {
     if (!emit_events) return guarded([] { fail(HNB_ERR_INVALID_ARG, "hnb_instance_restore_events: emit_events is NULL"); });
     return instance_restore(c, h, e, metadata_row, first, rows, emit_events, d_src, src_bytes, "hnb_instance_restore_events");
+}
+int32_t hnb_instance_append(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
+                            const void* d_src, size_t src_bytes) {
+    return instance_append(c, h, e, metadata_row, first, rows, d_src, src_bytes);
 }
 
 int32_t hnb_slab_checksum(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, uint64_t* out) {

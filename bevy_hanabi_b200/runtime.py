@@ -348,6 +348,13 @@ class Context:
         leaves. `src_bytes`: bytes readable at `d_src` (>= 64). Only enqueues work."""
         check(lib.hnb_instance_restore(self._h, slab, effect, metadata_row, first, rows, d_src, src_bytes))
 
+    def instance_append(self, slab: int, effect: int, metadata_row: int, first: int, rows: int, d_src: int,
+                        src_bytes: int) -> None:
+        """Add the records of a snapshot (or of any buffer in its format) to the live particles of the instance at slab
+        rows [first, first+rows), in the free slots its next spawns would take; at most max_spawn of them. The counts are
+        read on the device, so a kernel may write the buffer (hnb_instance_append). Only enqueues work."""
+        check(lib.hnb_instance_append(self._h, slab, effect, metadata_row, first, rows, d_src, src_bytes))
+
     def slab_repack_events(self, slab: int, effect: int, metadata_row: int, first: int, rows: int, emit_events) -> None:
         """slab_repack for an instance of an effect that emits GPU spawn events: `emit_events` (one event buffer per
         channel of the effect, as given to its update launch) have their pending events rewritten to the rows their

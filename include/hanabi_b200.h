@@ -314,6 +314,35 @@ HNB_API int32_t hnb_instance_restore(hnb_ctx* ctx, hnb_slab slab, hnb_effect eff
                                      uint32_t rows, const void* d_src, size_t src_bytes);
 
 /**
+ * Append the records of a version-1 snapshot to the live particles of the instance at slab rows [first, first+rows)
+ * (`rows` = its capacity), as spawns would take them: sparks at many explicit points in one frame, or the particles of a
+ * dying instance handed to a shared one (append its hnb_instance_snapshot). The arguments are hnb_instance_restore's;
+ * `d_src` may be written by the host or by a kernel, since every count is read on the DEVICE. With n = min(alive_count,
+ * rows), W = indirect_write_index and `dead` the slab's dead stack:
+ *   - m = min(header.count, max_spawn, rows - n, (src_bytes - 64) / stride), or 0 when magic, version (1 only) or
+ *     particle_stride do not match the effect. An append of m = 0 writes nothing.
+ *   - Record k < m goes where the k-th spawn of an init would put it: slot s_k = dead[first + n + k] - first (clamped to
+ *     the slice), slab row first + s_k of every column, and list_W[first + n + k] = s_k.
+ *   - As after a spawn: the identity claim of column W is cut to n if it reaches further, the alive bit of each written
+ *     slot is set (HNB_EFFECT_SLOT_ORDER), and the lifetime floor and common age of each written slot's 32-row group
+ *     become unknown. Floors and common ages of other groups are kept: a free slot never lies in a deferred group.
+ *   - The metadata row gets alive_count = n + m, max_spawn -= m and particle_counter += m (the header's particle_counter
+ *     and rows are ignored).
+ * Nothing else changes: dead-stack entries, max_update, draw args, spawners, the other list column and claim, the count
+ * mailbox (the next frame's indirect pass rewrites instance_count). Bounds, depth order, cull and snapshot calls made
+ * before the next hnb_simulate see the appended particles, and two appends in a row compose. Ribbon, slot-order,
+ * relaxed-order and sector-plane effects and children of GPU events are accepted; appended records keep their own
+ * RIBBON_ID and PREV/NEXT words.
+ *
+ * Call between hnb_simulate calls; work is only enqueued on the context stream (no synchronisation, no allocation). No
+ * access leaves the slice or d_src[0, src_bytes), whatever the device holds. HNB_ERR_INVALID_ARG, with nothing enqueued,
+ * on every input hnb_instance_restore refuses, HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS effects included (their pending events
+ * name the dead slots an append would fill). rows == 0 is a no-op.
+ */
+HNB_API int32_t hnb_instance_append(hnb_ctx* ctx, hnb_slab slab, hnb_effect effect, uint32_t metadata_row, uint32_t first,
+                                    uint32_t rows, const void* d_src, size_t src_bytes);
+
+/**
  * Repack, snapshot and restore of an instance whose effect has HNB_EFFECT_EMIT_GPU_SPAWN_EVENTS, together with the events
  * it appended in its last update, which the children's next init consumes. Between frames a pending event is an
  * instance-local parent slot: a live slot, or one of the D = min(max_update - n, rows - n) slots the last update freed,

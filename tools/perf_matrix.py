@@ -457,6 +457,93 @@ def snapshot_restore():
     ctx.close()
 
 
+def _timed_append(label, ctx, slab, effect, rows, stride, src, src_bytes, md):
+    """Best of 5 CUDA-event windows around hnb_instance_append of `src` into metadata row 0, after a warm-up call. Before
+    every call the metadata row is put back to `md` (outside the window), so each call makes the same m appends into the
+    same slots. Bytes: 4 B of dead-stack entry, S B of record read, S B of record written and 4 B of list per record."""
+    best = float("inf")
+    for rep in range(6):
+        ctx.metadata_insert(0, md)
+        ctx.sync()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        ctx.instance_append(slab, effect, 0, 0, rows, src, src_bytes)
+        e1.record(stream)
+        e1.synchronize()
+        if rep:
+            best = min(best, e0.elapsed_time(e1))
+    m = ctx.read_metadata(0).alive_count - md.alive_count
+    report(f"append: {label}", best, (8 + 2 * stride) * m, f"{m} records, best of 5")
+    return m
+
+
+def append():
+    """hnb_instance_append: 1, 64 and 4096 records into a small C5 instance (latency); 1 Mi records into the 16 Mi-slot
+    churn steady state (permuted dead stack, scattered slots); 1 Mi records into a 64 Mi-row C5 instance whose last 1 Mi
+    slots are free, in stack order and permuted; a 2 GiB device-to-device torch copy for scale."""
+    _card()
+    a = torch.empty(2 << 30, dtype=torch.uint8, device="cuda")
+    b = torch.empty_like(a)
+    ms = _events_ms(lambda: b.copy_(a))
+    report("append: 2 GiB device-to-device copy", ms, 2 * a.numel(), "torch copy_, best of 5")
+    del a, b
+    torch.cuda.empty_cache()
+
+    def c5_source(k):
+        """A version-1 snapshot of k random C5 records, in device memory (torch)."""
+        g = torch.Generator(device="cuda").manual_seed(k)
+        words = torch.empty(16 + 8 * k, dtype=torch.int32, device="cuda")
+        words[16:] = (torch.rand(8 * k, device="cuda", generator=g) * 2 - 1).view(torch.int32)
+        words[:16] = torch.tensor([0x53424E48, 1, 32, k] + [0] * 12, dtype=torch.int64).to(torch.int32).cuda()
+        return words
+
+    # latency: a 64 Ki-row C5 instance, 16 Ki alive
+    P, alive = 64 << 10, 16 << 10
+    ctx = hb.Context(0, stream.cuda_stream)
+    slab = ctx.slab_create(P, 32)
+    ctx.slab_fill_c5(slab, 0, alive, 42, 1e9, 1e9)
+    effect = ctx.effect_compile(recipes.c5_lowered())
+    md = R.initial_metadata(P, 0, 8)
+    md.alive_count, md.max_spawn = alive, P - alive
+    for k in (1, 64, 4096):
+        src = c5_source(k)
+        _timed_append(f"{k} records into a {P >> 10} Ki-row C5 instance", ctx, slab, effect, P, 32, src.data_ptr(), 4 * src.numel(), md)
+    ctx.close()
+
+    # the churn steady state: records from a snapshot of the instance itself, src_bytes cut to 1 Mi records
+    P, ctx, slab, effect, stride, dt, rate = _churned()
+    md = ctx.read_metadata(0)
+    F = 1 << 20
+    assert md.max_spawn >= F
+    nbytes = ctx.instance_snapshot_bytes(stride, P)
+    buf = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
+    ctx.instance_snapshot(slab, effect, 0, 0, P, buf.data_ptr(), nbytes)
+    ind = ctx.slab_download_indirect(slab, md.alive_count, F)
+    jumps = np.abs(np.diff(ind[:, 2].astype(np.int64)))
+    _timed_append(f"1 Mi records into the 16 Mi churn steady state, {md.alive_count >> 10} Ki alive", ctx, slab, effect, P, stride,
+                  buf.data_ptr(), 64 + F * stride, md)
+    print(f"    median |slot jump| between consecutive dead-stack entries {np.median(jumps):.0f}", flush=True)
+    del buf
+    ctx.close()
+    torch.cuda.empty_cache()
+
+    # a 64 Mi-row C5 instance with its last 1 Mi slots free
+    P = 64 << 20
+    ctx = hb.Context(0, stream.cuda_stream)
+    slab = ctx.slab_create(P, 32)
+    ctx.slab_fill_c5(slab, 0, P, 42, 1e9, 1e9)
+    effect = ctx.effect_compile(recipes.c5_lowered())
+    md = R.initial_metadata(P, 0, 8)
+    md.alive_count, md.max_spawn = P - F, F
+    src = c5_source(F)
+    _timed_append("1 Mi records into a 64 Mi C5 instance, stack order", ctx, slab, effect, P, 32, src.data_ptr(), 4 * src.numel(), md)
+    rows3 = ctx.slab_download_indirect(slab, P - F, F)
+    rows3[:, 2] = np.random.default_rng(1).permutation(rows3[:, 2])
+    ctx.slab_upload_indirect(slab, P - F, rows3)
+    _timed_append("1 Mi records into a 64 Mi C5 instance, permuted", ctx, slab, effect, P, 32, src.data_ptr(), 4 * src.numel(), md)
+    ctx.close()
+
+
 def _timed_bounds(label, ctx, launch, instances, bytes_, extra=""):
     """hnb_batch_bounds of `launch`'s batch into a device buffer: one warm-up call, then the best of 5 CUDA-event windows.
     `bytes_`: what the pass must read (16 B of position per live particle, 4 B of list where no claim covers the row)."""
@@ -1037,7 +1124,7 @@ def emitter_relocation():
     ctx.close()
 
 
-SCENARIOS = {"cull": cull, "cull_views": cull_views, "c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "bounds": bounds, "depth_order": depth_order, "emitter_relocation": emitter_relocation, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
+SCENARIOS = {"append": append, "cull": cull, "cull_views": cull_views, "c2_small": c2_small, "c4_recipe": c4_recipe, "c3_chain": c3_chain, "churn_slot": churn_slot, "c5_slot": c5_slot, "chunks": chunks_sweep, "interop": interop, "frame_chain": frame_chain, "churn": churn, "churn_sector": churn_sector, "churn_repack": churn_repack, "snapshot_restore": snapshot_restore, "bounds": bounds, "depth_order": depth_order, "emitter_relocation": emitter_relocation, "fresh_sector": fresh_sector, "many": many_batches, "c5": c5_update, "c5_dying": c5_dying, "c4": c4_topology, "c5_init": c5_init_burst, "c2": c2_trails, "c3": c3_force_field, "c3_fast": c3_fast_math}
 if __name__ == "__main__":
     for name in (sys.argv[1:] or list(SCENARIOS)):
         try:
