@@ -27,6 +27,7 @@
 #include "effect_source.h"
 #include "hanabi_b200.h"
 #include "nvrtc_compile.h"
+#include "slab_access_rule.h"
 #include "tile_state_rule.h"
 
 using namespace hnb_rt;
@@ -89,28 +90,16 @@ struct Slab {
     uint32_t capacity = 0, stride = 0;
     bool sector_planes = false;  // HNB_SLAB_SECTOR_PLANES
     // Physical columns, carved from one zero-filled block of capacity x stride bytes: column p starts at capacity x
-    // planes[p].offset. The first effect bound to the slab fixes the plan (fix_plan); before that, calls that write
-    // records write the default cut (`written`).
+    // planes[p].offset.
     std::vector<Plane> planes;
-    bool plan_fixed = false, written = false;
     DeviceArray<char> d_block;
     char* column(size_t p) const { return d_block.get() + size_t(capacity) * planes[p].offset; }
     DeviceArray<uint32_t> ping, pong, dead;
     DeviceArray<uint32_t> alive_bits;  // one bit per row (HNB_EFFECT_SLOT_ORDER effects keep it current)
     DeviceArray<unsigned long long> ident_claim;  // [2]: identity claims of ping / pong (hnb_claim_pack)
-    // Lifetime floors (DESIGN.md §3): one f32 per 32 rows, HNB_LIFE_FLOOR_NONE (all bits set) until an update of an effect
-    // with floors stores one. Every other writer of records clears the groups it touches (clear_life_floors). `floors_off`:
-    // the update passes get no floors any more, because a view was handed out or a module without floors was bound.
-    DeviceArray<uint32_t> life_floor;
-    bool floors_off = false;
-    // Common ages (DESIGN.md §3): one word per 32 rows, (epoch << 32) | the age bits of every row of the group, or all bits
-    // set. Cleared with the floors, and at the epoch wrap. `ages_off`: a module without them was bound.
-    DeviceArray<unsigned long long> group_age;
-    bool ages_off = false;
-    // An update may have left words deferred (BatchParams::defer_ages): their groups' ages are in the words, not in record
-    // word `age_word` of the rows. Every other reader or writer of records flushes them first (flush_group_ages).
-    bool defers = false;
-    uint32_t age_word = 0;
+    DeviceArray<uint32_t> life_floor;             // one f32 per 32 rows
+    DeviceArray<unsigned long long> group_age;    // one word per 32 rows, then hnb_deferred_groups
+    hnb_rt::SlabState state;  // what the claims, group words and plan may be trusted for (slab_access_rule.h)
     // HNB_EFFECT_ORDERED_EVENTS scratch, allocated on first use: per channel the per-row event counts and their block sums
     DeviceArray<uint32_t> event_counts[HNB_MAX_EVENT_BINDINGS];
     DeviceArray<uint32_t> event_block_sums[HNB_MAX_EVENT_BINDINGS];
@@ -120,9 +109,7 @@ struct KernelModule {
     CUmodule mod = nullptr;
     CUfunction init = nullptr, update = nullptr;
     int update_blocks_per_sm = 1;
-    bool life_floor = false;  // generated with HNB_LIFE_FLOOR: keeps the slab's lifetime floors (and clears them on init)
-    bool group_age = false;   // generated with HNB_GROUP_AGE: keeps the slab's common ages too
-    uint32_t age_word = 0;    // with group_age: the record word of the age (HNB_GROUP_AGE_WORD)
+    hnb_rt::ModuleWords words;  // what it keeps of the slab's group words
     std::string log;
 };
 
@@ -375,7 +362,8 @@ void flush_arena(hnb_ctx* c, bool with_ranges) {
     if (bytes >= c->lay.off_prefix_sum) c->plan_dirty = false;
 }
 
-void clear_life_floors(hnb_ctx* c, Slab& s);
+void prepare_slab(hnb_ctx* c, Slab& s, hnb_rt::SlabAccess access, uint32_t first = 0, uint32_t count = 0,
+                  const hnb_rt::ModuleWords& m = {});
 
 void next_epoch(hnb_ctx* c) {
     c->epoch = (c->epoch + 1u) & 0x3fffffffu;
@@ -387,7 +375,7 @@ void next_epoch(hnb_ctx* c) {
             if (ts) CUDA_CHECK(cudaMemsetAsync(ts.get(), 0, ts.size() * 8, c->stream));
         // the same for a common age stored a whole cycle ago (DESIGN.md §3)
         for (Slab& s : c->slabs)
-            if (s.live) clear_life_floors(c, s);
+            if (s.live) prepare_slab(c, s, hnb_rt::SlabAccess::Invalidate);
     }
     c->header()->epoch = c->epoch;
     c->header()->num_batches = c->B;
@@ -418,40 +406,22 @@ hnb::PlaneSet plane_set(const std::vector<Plane>& planes, char* block, uint32_t 
 }
 hnb::PlaneSet plane_set(const Slab& s) { return plane_set(s.planes, s.d_block.get(), s.capacity); }
 
-// Writes the ages of deferred common-age words (DESIGN.md §3) of the 32-row groups rows [first, first + count) touch back to
-// their rows, in stream order, when the slab may hold any. `clear`: then sets every word and lifetime floor of those groups to
-// the sentinel (writers of records). Otherwise a deferred word becomes the word known at the context's epoch, which the next
-// frame's update reads as known (readers of records).
-void flush_group_ages(hnb_ctx* c, const Slab& s, uint32_t first, uint32_t count, bool clear) {
-    if (count == 0 || !s.defers) return;
-    CUDA_CHECK(hnb::launch_flush_group_ages(plane_set(s), s.age_word, s.group_age.get(), s.life_floor.get(), first, count, s.capacity,
-                                            clear, c->epoch, c->stream));
-    c->launches++;
-}
-
-// Sets the lifetime floors and common ages of every 32-row group that rows [first, first + count) touch to the sentinel, in
-// stream order, deferred ages written back first: for writers of records other than the update pass (DESIGN.md §3).
-void clear_life_floors(hnb_ctx* c, Slab& s, uint32_t first, uint32_t count) {
-    if (count == 0) return;
-    if (s.defers) {
-        flush_group_ages(c, s, first, count, true);
-        if (first == 0 && count == s.capacity) s.defers = false;  // no word is deferred any more
-        return;
+// Enqueues, in stream order, what `access` to rows [first, first + count) of the slab must do first (slab_access_rule.h):
+// drops the identity claims, then writes the deferred ages of the rows' 32-row groups back to their rows (k_flush_group_ages)
+// and, for writers, sets every word and lifetime floor of those groups to the sentinel. A deferred word a reader flushes
+// becomes the word known at the context's epoch, which the next frame's update reads as known.
+void prepare_slab(hnb_ctx* c, Slab& s, hnb_rt::SlabAccess access, uint32_t first, uint32_t count, const hnb_rt::ModuleWords& m) {
+    const hnb_rt::SlabWork w = hnb_rt::slab_access(s.state, access, first, count, s.capacity, m);
+    if (w.drop_claims) CUDA_CHECK(cudaMemsetAsync(s.ident_claim.get(), 0, 2 * sizeof(unsigned long long), c->stream));
+    if (w.flush) {
+        CUDA_CHECK(hnb::launch_flush_group_ages(plane_set(s), s.state.age_word, s.group_age.get(), s.life_floor.get(), w.first, w.count,
+                                                s.capacity, w.clear, c->epoch, c->stream));
+        c->launches++;
+    } else if (w.clear) {
+        const size_t g0 = w.first / 32u, g1 = (size_t(w.first) + w.count + 31u) / 32u;
+        CUDA_CHECK(cudaMemsetAsync(s.life_floor.get() + g0, 0xff, (g1 - g0) * sizeof(uint32_t), c->stream));
+        CUDA_CHECK(cudaMemsetAsync(s.group_age.get() + g0, 0xff, (g1 - g0) * sizeof(unsigned long long), c->stream));
     }
-    const size_t g0 = first / 32u, g1 = (size_t(first) + count + 31u) / 32u;
-    CUDA_CHECK(cudaMemsetAsync(s.life_floor.get() + g0, 0xff, (g1 - g0) * sizeof(uint32_t), c->stream));
-    CUDA_CHECK(cudaMemsetAsync(s.group_age.get() + g0, 0xff, (g1 - g0) * sizeof(unsigned long long), c->stream));
-}
-void clear_life_floors(hnb_ctx* c, Slab& s) { clear_life_floors(c, s, 0, s.capacity); }
-
-// clear_life_floors for writers of alive lists and dead stacks at positions [first, first + count): their entries name rows
-// anywhere in an instance's slice, not the rows at those positions. A row of a deferred group that such a write moves to the
-// dead stack breaks the invariant that every row of the group is alive, and no later update would walk all 32 rows of it
-// (DESIGN.md §3). So a slab that may hold deferred words is flushed and cleared whole.
-void clear_list_groups(hnb_ctx* c, Slab& s, uint32_t first, uint32_t count) {
-    if (count == 0) return;
-    if (s.defers) clear_life_floors(c, s);
-    else clear_life_floors(c, s, first, count);
 }
 
 // AoS records <-> columns go through a device staging buffer in chunks of this size.
@@ -463,16 +433,17 @@ constexpr size_t kChunkBytes = size_t(64) << 20;
 // bytes and one synchronisation; when that block cannot be allocated the slab keeps its default cut (the effect then runs
 // a module generated for it). Callers validate everything else first: a failure here leaves the slab as it was.
 void fix_plan(hnb_ctx* c, Slab& s, const std::vector<Plane>& plan) {
-    if (s.plan_fixed) return;
-    if (plan != s.planes && s.written) {
+    if (s.state.plan_fixed) return;
+    if (plan != s.planes && s.state.written) {
         DeviceArray<char> next, staging;
         const uint32_t rows_per_chunk = (uint32_t)std::min<size_t>(s.capacity, std::max<size_t>(1, kChunkBytes / s.stride));
         if (next.alloc(size_t(s.capacity) * s.stride) != cudaSuccess || staging.alloc(size_t(rows_per_chunk) * s.stride) != cudaSuccess) {
             (void)cudaGetLastError();
-            s.plan_fixed = true;
+            s.state.plan_fixed = true;
             return;
         }
-        clear_life_floors(c, s);  // (before the records move: a deferred age goes back to the columns it is moved from)
+        // before the records move: a deferred age goes back to the columns it is moved from
+        prepare_slab(c, s, hnb_rt::SlabAccess::Invalidate);
         const hnb::PlaneSet from = plane_set(s), to = plane_set(plan, next.get(), s.capacity);
         uint32_t* stage = reinterpret_cast<uint32_t*>(staging.get());
         for (uint32_t done = 0; done < s.capacity; done += rows_per_chunk) {
@@ -485,7 +456,7 @@ void fix_plan(hnb_ctx* c, Slab& s, const std::vector<Plane>& plan) {
         s.d_block.swap(next);
     }
     s.planes = plan;
-    s.plan_fixed = true;
+    s.state.plan_fixed = true;
 }
 void fix_default_plan(hnb_ctx* c, Slab& s) { fix_plan(c, s, physical_planes(s.stride, s.sector_planes)); }
 
@@ -499,11 +470,6 @@ hnb::SlabView slab_view(const Slab& s) {
     v.ident_claim = s.ident_claim.get();
     v.capacity_rows = s.capacity;
     return v;
-}
-
-// Drops both identity claims of the slab, in stream order: for writers of the index columns that do not keep them true.
-void clear_ident_claims(hnb_ctx* c, const Slab& s) {
-    CUDA_CHECK(cudaMemsetAsync(s.ident_claim.get(), 0, 2 * sizeof(unsigned long long), c->stream));
 }
 
 // Copies `bytes` from the device to the host in stream order (and then zeroes the source when `clear`), and waits.
@@ -535,10 +501,10 @@ KernelModule* get_module(hnb_ctx* c, const std::string& source, const std::strin
     r = c->drv.ModuleGetFunction(&km->update, km->mod, "hnb_update");
     if (r != CUDA_SUCCESS) fail(HNB_ERR_CUDA, "cuModuleGetFunction(hnb_update): " + cu_error_string(c->drv, r));
     km->update_blocks_per_sm = 1;  // depends on the effect's dynamic shared memory (set_update_smem)
-    km->life_floor = source.find("\n#define HNB_LIFE_FLOOR 1\n") != std::string::npos;
-    km->group_age = source.find("\n#define HNB_GROUP_AGE 1\n") != std::string::npos;
+    km->words.life_floor = source.find("\n#define HNB_LIFE_FLOOR 1\n") != std::string::npos;
+    km->words.group_age = source.find("\n#define HNB_GROUP_AGE 1\n") != std::string::npos;
     if (const size_t at = source.find("\n#define HNB_GROUP_AGE_WORD "); at != std::string::npos)
-        km->age_word = uint32_t(strtoul(source.c_str() + at + 27, nullptr, 10));
+        km->words.age_word = uint32_t(strtoul(source.c_str() + at + 27, nullptr, 10));
     KernelModule* out = km.get();
     c->modules.emplace(hash, std::move(km));
     return out;
@@ -748,17 +714,10 @@ void bind_launch(hnb_ctx* c, LaunchPlan& lp, const hnb_batch_launch& bl, bool se
     P.properties_stride = fx.props_stride;
     P.slab = slab_view(slab);
     if (lp.parent) P.parent_slab = slab_view(*lp.parent);
-    // A module without floors neither keeps nor clears them, and it may write lifetimes: once one runs on the slab, no update
-    // reads a floor of it again.
-    if (!lp.km->life_floor) slab.floors_off = true;
-    P.life_floor = slab.floors_off ? nullptr : reinterpret_cast<float*>(slab.life_floor.get());
-    // The same for common ages: a module without them writes ages without keeping the words true.
-    if (!lp.km->group_age) slab.ages_off = true;
-    P.group_age = slab.floors_off || slab.ages_off ? nullptr : slab.group_age.get();
-    // Deferred common ages (DESIGN.md §3): a module that keeps none, or keeps the age in another record word, gets the slab
-    // with every age in its column. An update that keeps them may defer (launch_update decides, once every launch of the
-    // frame is bound). Relaxed-order and slot-order modules keep no floors, so they take the first branch.
-    if (slab.defers && (!P.group_age || lp.km->age_word != slab.age_word)) clear_life_floors(c, slab);
+    // An update that keeps the common ages may defer them (launch_update decides, once every launch of the frame is bound).
+    prepare_slab(c, slab, hnb_rt::SlabAccess::Bind, 0, 0, lp.km->words);
+    P.life_floor = slab.state.floors_off ? nullptr : reinterpret_cast<float*>(slab.life_floor.get());
+    P.group_age = hnb_rt::keeps_group_ages(slab.state) ? slab.group_age.get() : nullptr;
     P.defer_ages = P.group_age && c->defer_ages ? 1u : 0u;
     if (consume) P.consume_events = c->event_buffers[bl.consume_events].get();
     for (int i = 0; i < HNB_MAX_EVENT_BINDINGS; ++i) {
@@ -821,11 +780,8 @@ void launch_update(hnb_ctx* c, LaunchPlan& lp, cudaStream_t st = nullptr) {
     if (!st) st = c->stream;
     // A launch bound after this one may have switched the slab's common ages off (bind_launch): then nothing is deferred.
     Slab& slab = *lp.slab;
-    if (slab.floors_off || slab.ages_off) lp.params.defer_ages = 0u;
-    if (lp.params.defer_ages) {
-        slab.defers = true;
-        slab.age_word = lp.km->age_word;
-    }
+    if (!hnb_rt::keeps_group_ages(slab.state)) lp.params.defer_ages = 0u;
+    if (lp.params.defer_ages) prepare_slab(c, slab, hnb_rt::SlabAccess::DeferringUpdate, 0, 0, lp.km->words);
     std::pair<Event, Event> ev;
     if (c->timing) {
         if (!c->ev_free.empty()) { ev = std::move(c->ev_free.back()); c->ev_free.pop_back(); }
@@ -898,8 +854,8 @@ void launch_ribbon_sort(hnb_ctx* c, const LaunchPlan& lp) {
     a.scratch_rows = uint32_t(sort_rows);
     a.scratch_grid = uint32_t(c->sm_count);
     if (any_large) CUDA_CHECK(cudaMemsetAsync(c->d_sort_hist.get(), 0, size_t(2 * 8 * 256) * 4, c->stream));
-    clear_ident_claims(c, *lp.slab);  // the sort permutes the column the update just wrote
-    flush_group_ages(c, *lp.slab, 0, lp.slab->capacity, false);  // its second key is the age
+    // the sort permutes the column the update just wrote, and its second key is the age
+    prepare_slab(c, *lp.slab, hnb_rt::SlabAccess::ListSort);
     uint32_t launched = 0;
     CUDA_CHECK(hnb::launch_ribbon_sort(a, any_large, uint32_t(c->sm_count), c->stream, &launched));
     c->launches += launched;
@@ -1057,7 +1013,7 @@ int32_t hnb_slab_create_ex(hnb_ctx* c, uint32_t capacity_rows, uint32_t stride, 
         s.stride = stride;
         s.sector_planes = (flags & HNB_SLAB_SECTOR_PLANES) != 0;
         s.planes = physical_planes(stride, s.sector_planes);
-        s.plan_fixed = s.sector_planes;  // sector-plane effects address the sector cut only
+        s.state.plan_fixed = s.sector_planes;  // sector-plane effects address the sector cut only
         // zero-filled (debug builds of the reference poison the particle buffer instead, effect_cache.rs:284-296)
         CUDA_CHECK(grow(s.d_block, size_t(capacity_rows) * stride, 0, c->stream));
         CUDA_CHECK(s.ping.alloc(capacity_rows));
@@ -1065,10 +1021,9 @@ int32_t hnb_slab_create_ex(hnb_ctx* c, uint32_t capacity_rows, uint32_t stride, 
         CUDA_CHECK(s.dead.alloc(capacity_rows));
         CUDA_CHECK(grow(s.alive_bits, size_t(capacity_rows) / 32 + 2, 0, c->stream));
         CUDA_CHECK(s.ident_claim.alloc(2));
-        clear_ident_claims(c, s);
         CUDA_CHECK(s.life_floor.alloc(size_t(capacity_rows) / 32 + 1));
         CUDA_CHECK(s.group_age.alloc(size_t(capacity_rows) / 32 + 2));  // the groups' words, then hnb_deferred_groups
-        clear_life_floors(c, s);
+        prepare_slab(c, s, hnb_rt::SlabAccess::RowReset, 0, capacity_rows);
         CUDA_CHECK(cudaMemsetAsync(hnb::hnb_deferred_groups(s.group_age.get(), capacity_rows), 0, sizeof(unsigned long long), c->stream));
         CUDA_CHECK(hnb::launch_slab_reset(s.ping.get(), s.pong.get(), s.dead.get(), 0, capacity_rows, c->stream));
         c->launches++;
@@ -1090,8 +1045,7 @@ int32_t hnb_slab_reset_rows(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t cou
     return guarded([&] {
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
-        clear_ident_claims(c, s);
-        clear_life_floors(c, s, first, count);
+        prepare_slab(c, s, hnb_rt::SlabAccess::RowReset, first, count);
         CUDA_CHECK(hnb::launch_slab_reset(s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
         CUDA_CHECK(hnb::launch_bits_range(s.alive_bits.get(), first, count, false, c->stream));
         c->launches += 2;
@@ -1103,7 +1057,7 @@ int32_t hnb_slab_rebuild_alive_bits(hnb_ctx* c, hnb_slab h, uint32_t first, uint
         Slab& s = get_slab(c, h);
         check_rows(s, first, rows);
         if (column > 1 || alive_count > rows) fail(HNB_ERR_INVALID_ARG, "bad alive-list column or count");
-        clear_list_groups(c, s, first, rows);  // slots may become alive whose lifetimes no floor covers
+        prepare_slab(c, s, hnb_rt::SlabAccess::AliveBitsWrite, first, rows);  // slots may become alive whose lifetimes no floor covers
         CUDA_CHECK(hnb::launch_bits_range(s.alive_bits.get(), first, rows, false, c->stream));
         CUDA_CHECK(hnb::launch_bits_from_list(s.alive_bits.get(), (column ? s.pong : s.ping).get() + first, first, alive_count, c->stream));
         c->launches += rows ? 1 + (alive_count ? 1 : 0) : 0;
@@ -1117,9 +1071,7 @@ void transfer_aos(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t count, void* 
     Slab& s = get_slab(c, h);
     check_rows(s, first, count);
     if (count == 0) return;
-    s.written |= upload;
-    if (upload) clear_life_floors(c, s, first, count);
-    else flush_group_ages(c, s, first, count, false);
+    prepare_slab(c, s, upload ? hnb_rt::SlabAccess::RecordWrite : hnb_rt::SlabAccess::RecordRead, first, count);
     const uint32_t rows_per_chunk = (uint32_t)std::max<size_t>(1, kChunkBytes / s.stride);
     DeviceArray<char> staging;
     CUDA_CHECK(staging.alloc(size_t(std::min(rows_per_chunk, count)) * s.stride));
@@ -1158,8 +1110,7 @@ int32_t hnb_slab_upload_indirect(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_
         DeviceArray<uint32_t> stage;
         CUDA_CHECK(stage.alloc(size_t(count) * 3));
         CUDA_CHECK(cudaMemcpyAsync(stage.get(), rows, size_t(count) * 12, cudaMemcpyHostToDevice, c->stream));
-        clear_ident_claims(c, s);
-        clear_list_groups(c, s, first, count);
+        prepare_slab(c, s, hnb_rt::SlabAccess::ListWrite, first, count);
         CUDA_CHECK(hnb::launch_indirect_deinterleave(stage.get(), s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
         c->launches++;
         CUDA_CHECK(cudaStreamSynchronize(c->stream));
@@ -1189,7 +1140,7 @@ int32_t hnb_slab_export_aos_device(hnb_ctx* c, hnb_slab h, uint32_t first, uint3
         check_rows(s, first, count);
         if (count && !d_dst) fail(HNB_ERR_INVALID_ARG, "d_dst is NULL");
         if ((uintptr_t)d_dst & 3u) fail(HNB_ERR_INVALID_ARG, "d_dst must be 4-byte aligned (16-byte aligned for full speed)");
-        flush_group_ages(c, s, first, count, false);
+        prepare_slab(c, s, hnb_rt::SlabAccess::RecordRead, first, count);
         CUDA_CHECK(hnb::launch_planes_to_aos((uint32_t*)d_dst, plane_set(s), first, count, s.stride / 4, c->stream));
         c->launches += count ? 1 : 0;
     });
@@ -1200,8 +1151,7 @@ int32_t hnb_slab_import_aos_device(hnb_ctx* c, hnb_slab h, uint32_t first, uint3
         check_rows(s, first, count);
         if (count && !d_src) fail(HNB_ERR_INVALID_ARG, "d_src is NULL");
         if ((uintptr_t)d_src & 3u) fail(HNB_ERR_INVALID_ARG, "d_src must be 4-byte aligned (16-byte aligned for full speed)");
-        s.written = true;
-        clear_life_floors(c, s, first, count);
+        prepare_slab(c, s, hnb_rt::SlabAccess::RecordWrite, first, count);
         CUDA_CHECK(hnb::launch_aos_to_planes((const uint32_t*)d_src, plane_set(s), first, count, s.stride / 4, c->stream));
         c->launches += count ? 1 : 0;
     });
@@ -1220,8 +1170,7 @@ int32_t hnb_slab_import_indirect_device(hnb_ctx* c, hnb_slab h, uint32_t first, 
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
         if (count && !d_src) fail(HNB_ERR_INVALID_ARG, "d_src is NULL");
-        clear_ident_claims(c, s);
-        clear_list_groups(c, s, first, count);
+        prepare_slab(c, s, hnb_rt::SlabAccess::ListWrite, first, count);
         CUDA_CHECK(hnb::launch_indirect_deinterleave((const uint32_t*)d_src, s.ping.get(), s.pong.get(), s.dead.get(), first, count, c->stream));
         c->launches += count ? 1 : 0;
     });
@@ -1231,8 +1180,7 @@ int32_t hnb_slab_device_view(hnb_ctx* c, hnb_slab h, hnb_slab_view* out) {
         Slab& s = get_slab(c, h);
         if (!out) fail(HNB_ERR_INVALID_ARG, "out is NULL");
         fix_default_plan(c, s);  // handed-out columns never move: an unbound slab keeps the default cut from now on
-        if (s.defers) clear_life_floors(c, s);  // every age goes back to its column ...
-        s.floors_off = true;     // ... and records written through the view would not clear the floors
+        prepare_slab(c, s, hnb_rt::SlabAccess::ViewOut);
         memset(out, 0, sizeof(*out));
         out->capacity_rows = s.capacity;
         out->particle_stride = s.stride;
@@ -1284,8 +1232,7 @@ int32_t hnb_slab_fill_c5_ex(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t cou
         check_rows(s, first, count);
         if (s.stride != 32) fail(HNB_ERR_LAYOUT, "hnb_slab_fill_c5 needs the 32-byte {position,age,velocity,lifetime} layout");
         if (s.sector_planes) fail(HNB_ERR_LAYOUT, "hnb_slab_fill_c5 writes the default or a column plan; spawn through the init pass or use hnb_slab_upload_aos");
-        s.written = true;
-        clear_life_floors(c, s, first, count);
+        prepare_slab(c, s, hnb_rt::SlabAccess::RecordWrite, first, count);
         CUDA_CHECK(hnb::launch_fill_c5(plane_set(s), s.ping.get(), s.pong.get(), s.ident_claim.get(), first, count, seed, lo, hi,
                                        logical_first, c->stream));
         CUDA_CHECK(hnb::launch_bits_range(s.alive_bits.get(), first, count, true, c->stream));
@@ -1385,7 +1332,7 @@ int32_t slab_repack(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row,
         fix_plan(c, s, fx.plan);
         CUDA_CHECK(cudaSetDevice(c->device));
         const hnb::RepackArgs a = repack_args(c, s, metadata_row, first, rows);
-        clear_life_floors(c, s, first, rows);
+        prepare_slab(c, s, hnb_rt::SlabAccess::InstanceRewrite, first, rows);
         uint32_t widest = 0;
         for (const Plane& p : s.planes) widest = std::max(widest, p.width);
         void* scratch = nullptr;
@@ -1439,7 +1386,7 @@ int32_t instance_snapshot(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadat
         }
         if (rows == 0) return;
         CUDA_CHECK(cudaSetDevice(c->device));
-        flush_group_ages(c, s, first, rows, false);
+        prepare_slab(c, s, hnb_rt::SlabAccess::RecordRead, first, rows);
         CUDA_CHECK(hnb::launch_snapshot_gather(snapshot_args(c, s, metadata_row, first, rows), (uint32_t*)d_dst, c->stream,
                                                emit ? s.dead.get() : nullptr));
         c->launches++;
@@ -1470,8 +1417,7 @@ int32_t instance_restore(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata
         if (rows == 0) return;
         CUDA_CHECK(cudaSetDevice(c->device));
         fix_plan(c, s, fx.plan);
-        s.written = true;
-        clear_life_floors(c, s, first, rows);
+        prepare_slab(c, s, hnb_rt::SlabAccess::InstanceRewrite, first, rows);
         hnb::SnapshotArgs a = snapshot_args(c, s, metadata_row, first, rows);
         a.src_bytes = src_bytes;
         const hnb::EventChannels ev = emit ? event_channels(c, fx, emit) : hnb::EventChannels{};
@@ -1486,8 +1432,7 @@ int32_t instance_restore(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata
 }
 
 // hnb_instance_append (two launches: the records, list entries, bits and group words, then the metadata words and the claim
-// cut, which the first reads). No slice-wide flush: the written slots are free, and under the update invariant a free slot
-// never lies in a deferred group, so only the groups of the written slots change (DESIGN.md §4.12).
+// cut, which the first reads).
 int32_t instance_append(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_row, uint32_t first, uint32_t rows,
                         const void* d_src, size_t src_bytes) {
     return guarded([&] {
@@ -1501,7 +1446,7 @@ int32_t instance_append(hnb_ctx* c, hnb_slab h, hnb_effect e, uint32_t metadata_
         if (rows == 0) return;
         CUDA_CHECK(cudaSetDevice(c->device));
         fix_plan(c, s, fx.plan);
-        s.written = true;
+        prepare_slab(c, s, hnb_rt::SlabAccess::Append, first, rows);
         hnb::AppendArgs a{};
         a.s = snapshot_args(c, s, metadata_row, first, rows);
         a.s.src_bytes = src_bytes;
@@ -1587,7 +1532,7 @@ int32_t hnb_slab_checksum_ex(hnb_ctx* c, hnb_slab h, uint32_t first, uint32_t co
     return guarded([&] {
         Slab& s = get_slab(c, h);
         check_rows(s, first, count);
-        flush_group_ages(c, s, first, count, false);
+        prepare_slab(c, s, hnb_rt::SlabAccess::RecordRead, first, count);
         checksum(c, plane_set(s), first, count, s.stride / 4, index_base, out);
     });
 }
@@ -1864,7 +1809,7 @@ int32_t hnb_metadata_insert(hnb_ctx* c, uint32_t row, const hnb_effect_metadata*
         // A new metadata row may end an instance without any writer of its rows: the slice's next owner would not walk every
         // row of a deferred group. So every age goes back to its column first (DESIGN.md §3).
         for (Slab& s : c->slabs)
-            if (s.live && s.defers) clear_life_floors(c, s);
+            if (s.live) prepare_slab(c, s, hnb_rt::SlabAccess::MetadataWrite);
         const uint32_t rows = uint32_t(c->d_metadata.size());
         if (row + 1 > rows) CUDA_CHECK(grow(c->d_metadata, std::max<uint32_t>(row + 1, std::max<uint32_t>(rows * 2, 16)), rows, c->stream));
         CUDA_CHECK(cudaMemcpyAsync(c->d_metadata.get() + row, md, sizeof(*md), cudaMemcpyHostToDevice, c->stream));
